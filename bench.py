@@ -2,8 +2,9 @@
 sharded over N GPUs of one node (STRONG scaling: the global batch is fixed at 64, per-GPU batch = 64/N).
 
   python bench.py --gpus N --steps K --warmup W            # our arm (libmmg.so through the drop-in classes + parallel.generate_sharded)
-  python bench.py --impl reference --gpus N --steps K ...  # the UNMODIFIED reference's MaskGit.generate() on the host cores (baseline/_ref)
+  python bench.py --impl reference --gpus N --steps K ...  # the UNMODIFIED reference's MaskGit.generate() on the host cores (oracle/_ref)
   python bench.py --config C2|C4|C5                        # secondary configs of BASELINE.json (one JSON line each; C3 is the default)
+  python bench.py --dump-outputs DIR ...                   # also write what the last timed step returned to DIR/<name>.npy (float32)
 
 One "step" = one full generate() call over the rank's shard (18 decode steps + VAE decode + (N>1) one NCCL all-gather of
 the decoded images).  `value` is timed with the text embeddings already resident in HBM; `e2e` times the same public call
@@ -42,8 +43,23 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(tflops=d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1400.0)), hbm=d.get("hbm_gbs", 6650.0), src="measured")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback")
+        return dict(tflops=d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0)), hbm=d.get("hbm_gbs", 3350.0), src="measured")
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet (dense bf16, HBM3)")
+
+
+DUMP_FULL_BYTES = 48 << 20           # outputs up to this size are written whole
+DUMP_SAMPLE = 4 << 20                # larger ones: this many elements at fixed seeded positions (the same for every build)
+
+
+def dump_output(dirname, name, t):
+    """--dump-outputs: one output of the last timed step -> dirname/name.npy as float32 (a fixed seeded sample when it is large)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    flat = t.detach().reshape(-1)
+    if flat.numel() * 4 > DUMP_FULL_BYTES:
+        idx = torch.randint(flat.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(0)).sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(dirname, name + ".npy"), flat.float().cpu().numpy() if flat.numel() != t.numel() else t.detach().float().cpu().numpy())
 
 
 def text_embeddings(batch, seed=1):
@@ -54,7 +70,7 @@ def text_embeddings(batch, seed=1):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     def __init__(self, index):
         super().__init__(daemon=True)
         self.rows, self.proc, self.index = [], None, index
@@ -161,8 +177,11 @@ def run_ours(args):
     sampler = ClockSampler(local) if rank == 0 else None
     if sampler:
         sampler.start()
-    ms, launches = timed_loop(dist, world, device, lambda: step(False), args.steps)
+    last = {}
+    ms, launches = timed_loop(dist, world, device, lambda: last.update(images=step(False)), args.steps)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_output(args.dump_outputs, "images", last["images"])          # the [64, 3, 256, 256] decoded images (48 MB as float32)
     step(True)
     ms_e2e, _ = timed_loop(dist, world, device, lambda: step(True), args.steps)
 
@@ -185,7 +204,7 @@ def run_ours(args):
                     "h2d_bytes_per_step": te_host.numel() * 4 * world, "d2h_bytes_per_step": host_out.numel() * 4},
             "gpu_launches": (launches if launches > 0 else roof["launches_per_step_all_kernels"]) * args.steps,   # graph replays re-issue the captured kernel nodes
             "launches_per_decode_step": round(roof["launches_per_step_all_kernels"] / TIMESTEPS, 1),
-            "simt_fallbacks": __import__("muse_maskgit_pytorch_b200")._lib.simt_fallback_count(),      # bf16 products that left the tcgen05 path (must be 0 here)
+            "simt_fallbacks": __import__("muse_maskgit_pytorch_b200")._lib.simt_fallback_count(),      # bf16 products that left the wgmma path (must be 0 here)
             "clocks": clocks,
             "roofline": roof,
             "dense_flop_frac_of_peak": round(value * GFLOP_PER_IMAGE / 1e3 / world / pk["tflops"], 4),
@@ -223,7 +242,7 @@ def _gemm_flops(name, a):
 def kernel_roofline(mg, texts, te_dev, pk):
     """Per-entry-point device time of ONE generate(): every libmmg call is bracketed by CUDA events.  Preferred: the events are
     captured INTO a CUDA graph of the call (external event-record nodes) and read after a replay, so the durations are the in-situ ones
-    of the replayed graph; fallback: an eager pass (launch gaps then contaminate small kernels).  The dominant kernel is the tcgen05 GEMM
+    of the replayed graph; fallback: an eager pass (launch gaps then contaminate small kernels).  The dominant kernel is the wgmma GEMM
     (mmg_linear / mmg_conv* / the fused logits-sampling GEMM): algorithmic FLOPs / its summed duration vs the measured bf16 peak."""
     from muse_maskgit_pytorch_b200 import _lib
     rec = []
@@ -279,25 +298,16 @@ def kernel_roofline(mg, texts, te_dev, pk):
         d = tot.setdefault(name, [0.0, 0.0, 0])
         d[0] += e0.elapsed_time(e1); d[1] += fl; d[2] += 1
     all_ms = sum(v[0] for v in tot.values())
-    traffic, tsrc, fused_share = None, None, 1.0
-    tp = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(tp):                                      # dram bytes per launch of the dominant kernel, from the committed ncu capture
-        tj = json.load(open(tp))
-        traffic, tsrc = tj.get("tc_gemm_dram_bytes_per_launch"), tj.get("source")
-        fused_share = float(tj.get("logits_fused_gemm_share", 1.0))
-    # mmg_logits_fused is one entry point = GEMMs + threshold / finisher kernels: only its GEMM share (ncu launch list of the same build) counts as
-    # tcgen05 GEMM time; its FLOPs are the logits GEMM's (the 1/16 sample GEMM is not counted)
-    if "mmg_logits_fused" in tot:
-        tot["mmg_logits_fused (GEMM share)"] = [tot["mmg_logits_fused"][0] * fused_share, tot["mmg_logits_fused"][1], tot["mmg_logits_fused"][2]]
-    gemm = [tot[k] for k in ("mmg_linear", "mmg_conv2d", "mmg_conv_transpose2d", "mmg_logits_fused (GEMM share)") if k in tot]
+    # mmg_logits_fused is one entry point = its two GEMMs + the threshold / finishing kernels: its events cannot separate the GEMM share, so
+    # the GEMM rate below covers the stand-alone products only and the fused entry point is listed on its own in by_entry_point_ms
+    gemm = [tot[k] for k in ("mmg_linear", "mmg_conv2d", "mmg_conv_transpose2d") if k in tot]
     g_ms, g_fl, g_n = sum(v[0] for v in gemm), sum(v[1] for v in gemm), sum(v[2] for v in gemm)
-    tot.pop("mmg_logits_fused (GEMM share)", None)
     achieved = g_fl / (g_ms * 1e-3) / 1e12 if g_ms > 0 else 0.0
-    return {"bound": "tensor", "kernel": "tc_gemm_kernel (tcgen05; mmg_linear + mmg_conv2d + mmg_conv_transpose2d + fused logits/sampling GEMM)",
+    return {"bound": "tensor", "kernel": "tc_gemm_kernel (wgmma; mmg_linear + mmg_conv2d + mmg_conv_transpose2d)",
             "achieved": round(achieved, 1), "peak": pk["tflops"], "unit": "TFLOP/s", "frac": round(achieved / pk["tflops"], 4),
-            "traffic": traffic, "traffic_source": tsrc, "flop_per_launch": round(g_fl / max(g_n, 1)),
+            "flop_per_launch": round(g_fl / max(g_n, 1)),
             "launches": g_n, "launches_per_step_all_kernels": len(rec), "avg_launch_us": round(1e3 * g_ms / max(g_n, 1), 2),
-            "share_of_step": round(g_ms / max(all_ms, 1e-9), 3), "timing": how, "logits_fused_gemm_share": fused_share,
+            "share_of_step": round(g_ms / max(all_ms, 1e-9), 3), "timing": how,
             "by_entry_point_ms": {k: round(v[0], 3) for k, v in sorted(tot.items(), key=lambda kv: -kv[1][0])}, "peak_source": pk["src"]}
 
 
@@ -346,7 +356,7 @@ def hbm_kernels(mg, pk):
 
 
 def teacher_forced_flip_rate(mg, b=2):
-    """Token-id parity of the timed (bf16, tcgen05) path at the C3 model config: every decode step is fed the fp32 oracle's ids and noise;
+    """Token-id parity of the timed (bf16, wgmma) path at the C3 model config: every decode step is fed the fp32 oracle's ids and noise;
     flip = a sampled token that differs from the oracle's.  (The oracle is the CHECKER here, tests/test_gpu_full_config.py holds the same test.)"""
     from oracle import muse_oracle as O
     tr = mg.transformer
@@ -387,7 +397,7 @@ def cpu_threads():
 
 
 def build_reference(device="cpu", flash=True):
-    """The UNMODIFIED reference package (baseline/_ref, pip-installed from /root/reference in the build container) with its own default
+    """The UNMODIFIED reference package (oracle/_ref, installed by build() from the reference checkout) with its own default
     init under torch.manual_seed(0) at the C3 config; four absent third-party packages are stood in for by tests/golden/_shims."""
     from baseline import ref_loader
     ref = ref_loader.load(512)
@@ -429,7 +439,7 @@ def cpu_baseline():
 
 
 def cpu_baseline_port(cores):
-    """Fallback when baseline/_ref is absent: the oracle port, 2 of 18 decode steps + the VAE decode of one image."""
+    """Fallback when oracle/_ref is absent: the oracle port, 2 of 18 decode steps + the VAE decode of one image."""
     from oracle import muse_oracle as O
     import muse_maskgit_pytorch_b200 as M
     from muse_maskgit_pytorch_b200 import t5
@@ -450,16 +460,16 @@ def cpu_baseline_port(cores):
         t2 = time.perf_counter()
     total = TIMESTEPS * (t1 - t0) / 2 + (t2 - t1)
     return {"value": round(1.0 / total, 5), "unit": "images/s", "cores": cores, "kind": "port",
-            "sample": "baseline/_ref missing: oracle port, 1 image, 2 of 18 decode steps + VAE decode timed, images/s = 1 / (18 x step + decode)"}
+            "sample": "oracle/_ref missing: oracle port, 1 image, 2 of 18 decode steps + VAE decode timed, images/s = 1 / (18 x step + decode)"}
 
 
 def gpu_eager_baseline(device):
-    """The unmodified reference modules on this B200 in eager PyTorch (SURVEY.md 8d, BASELINE.md 4.4): fp32 and autocast(bf16), both through
+    """The unmodified reference modules on this GPU in eager PyTorch (SURVEY.md 8d, BASELINE.md 4.4): fp32 and autocast(bf16), both through
     the reference-owned attention branch (flash=False, attend.py:123-138; the flash branch belongs to an un-vendored third-party package), global
     batch 64, one warm-up + one timed generate() each.  None of this repo's kernels run here."""
     out = {}
     if not reference_available():
-        return {"unavailable": "baseline/_ref missing"}
+        return {"unavailable": "oracle/_ref missing"}
     te = text_embeddings(GLOBAL_BATCH).to(device)
     for name, flash, autocast in (("fp32", False, False), ("autocast_bf16", False, True)):
         try:
@@ -480,14 +490,14 @@ def gpu_eager_baseline(device):
         except Exception as ex:
             out[name] = {"error": f"{type(ex).__name__}: {str(ex)[:160]}"}
         torch.cuda.empty_cache()
-    out["note"] = "unmodified reference (baseline/_ref + stand-ins for its 4 absent third-party packages), eager PyTorch on one B200"
+    out["note"] = "unmodified reference (oracle/_ref + stand-ins for its 4 absent third-party packages), eager PyTorch on one GPU"
     return out
 
 
 def run_reference(args):
     """`--impl reference`: the unmodified reference's own MaskGit.generate() (stock code path: its Transformer / Attend / VQGanVAE modules,
     its sampling tail) on the host cores.  One bench step = one full generate() of REF_BATCH images (18 steps, CFG = 3), a bounded sample of the
-    64-image workload (BASELINE.md section 4).  A wall budget (MMG_REF_BUDGET_S, default 270 s) caps the number of timed steps."""
+    64-image workload (BASELINE.md section 4).  Exactly --steps calls are timed."""
     rank = int(os.environ.get("RANK", 0))
     if rank != 0:
         return
@@ -496,32 +506,33 @@ def run_reference(args):
     base = {"impl": "reference", "metric": METRIC, "unit": "images/s", "n_gpus": args.gpus, "higher_is_better": True, "scaling": "strong",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic"}
     if not reference_available():
-        cb = cpu_baseline_port(cores)
-        base.update({"value": cb["value"], "steps": 1, "warmup": 0, "ms_per_step": round(1e3 / cb["value"], 1), "cpu_baseline": cb,
-                     "config": {"workload": "C3 on host cores: oracle port (baseline/_ref missing)", "global_batch": 1, "parallelism": "cpu"},
+        if args.dump_outputs:
+            sys.exit("--dump-outputs with --impl reference needs the reference installed in oracle/_ref (see oracle/reference_install.py)")
+        runs = [cpu_baseline_port(cores) for _ in range(args.steps)]      # exactly --steps timed samples of the port
+        cb = dict(runs[-1], value=round(sum(r["value"] for r in runs) / len(runs), 5))
+        base.update({"value": cb["value"], "steps": args.steps, "warmup": 0, "ms_per_step": round(1e3 / cb["value"], 1), "cpu_baseline": cb,
+                     "config": {"workload": "C3 on host cores: oracle port (oracle/_ref missing)", "global_batch": 1, "parallelism": "cpu"},
                      "e2e": {"value": cb["value"], "unit": "images/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}})
         print(json.dumps(base))
         return
-    budget = float(os.environ.get("MMG_REF_BUDGET_S", "270"))
     mg = build_reference("cpu")
     te = text_embeddings(GLOBAL_BATCH)[:REF_BATCH]
     torch.manual_seed(2)
-    t_start = time.perf_counter()
     warm = 1 if args.warmup > 0 else 0
     if warm:
         reference_generate(mg, te, timesteps=2)                      # allocator / thread-pool warm-up (2 of the 18 steps)
     times = []
     for i in range(args.steps):
         t0 = time.perf_counter()
-        reference_generate(mg, te)
+        images = reference_generate(mg, te)
         times.append(time.perf_counter() - t0)
-        if time.perf_counter() - t_start + times[-1] > budget:      # the next step would overrun the wall budget
-            break
+    if args.dump_outputs:
+        dump_output(args.dump_outputs, "images", images)                # the [REF_BATCH, 3, 256, 256] images of the last timed call
     dt = sum(times) / len(times)
     v = REF_BATCH / dt
-    sample = (f"unmodified reference MaskGit.generate() (baseline/_ref), {REF_BATCH} images per step, full config (18 steps, CFG=3, V=65536, 256x256, fp32), "
-              f"{len(times)} timed calls of {dt:.1f} s on {cores} torch threads" + ("" if len(times) == args.steps else f" (of {args.steps} requested: wall budget {budget:.0f} s)"))
-    base.update({"value": round(v, 5), "steps": len(times), "steps_requested": args.steps, "warmup": warm, "ms_per_step": round(1e3 * dt, 1),
+    sample = (f"unmodified reference MaskGit.generate() (oracle/_ref), {REF_BATCH} images per step, full config (18 steps, CFG=3, V=65536, 256x256, fp32), "
+              f"{len(times)} timed calls of {dt:.1f} s on {cores} torch threads")
+    base.update({"value": round(v, 5), "steps": len(times), "warmup": warm, "ms_per_step": round(1e3 * dt, 1),
                  "config": {"workload": "C3: MaskGit.generate() 256x256, 18 steps, cond_scale=3, top-k 0.9 — the reference's own implementation on the host cores; "
                                         "transformer dim512 depth8 V65536, VQGanVAE dim256; random-init weights, pre-computed T5 embeddings (32 positions); "
                                         f"batch {REF_BATCH} per call (a bounded sample of the 64-image workload; CPU throughput is flat in the batch size)",
@@ -552,8 +563,11 @@ def run_c2(args):
     fn = lambda: tr(ids, text_embeds=te)
     for _ in range(max(args.warmup, 3)):
         fn()
-    ms, launches = timed_loop(dist, world, device, fn, args.steps)
+    last = {}
+    ms, launches = timed_loop(dist, world, device, lambda: last.update(logits=fn()), args.steps)
     if rank == 0:
+        if args.dump_outputs:
+            dump_output(args.dump_outputs, "logits", last["logits"])    # [B, 256, 65536] fp32: a fixed sample of 4 Mi logits
         v = B * world / (ms / 1e3)
         pk = peaks()
         print(json.dumps(_secondary_line("sequences/sec MaskGitTransformer forward (n=256, V=65536)", "sequences/s", v, ms, world, args,
@@ -578,8 +592,11 @@ def run_c4(args):
     fn = lambda: parallel.generate_sharded(mg, texts, text_embeds_shard=te, cond_images_shard=cond, seed=2, timesteps=TIMESTEPS, cond_scale=COND_SCALE)
     for _ in range(max(args.warmup, 3)):
         fn()
-    ms, launches = timed_loop(dist, world, device, fn, args.steps)
+    last = {}
+    ms, launches = timed_loop(dist, world, device, lambda: last.update(images=fn()), args.steps)
     if rank == 0:
+        if args.dump_outputs:
+            dump_output(args.dump_outputs, "images", last["images"])    # [G, 3, 512, 512]: a fixed sample of 4 Mi pixels at G = 32
         v = G / (ms / 1e3)
         pk = peaks()
         print(json.dumps(_secondary_line("images/sec super-res MaskGit.generate() 512x512 18-step CFG=3", "images/s", v, ms, world, args,
@@ -602,8 +619,11 @@ def run_c5(args):
     fn = lambda: vae(img)
     for _ in range(max(args.warmup, 3)):
         fn()
-    ms, launches = timed_loop(dist, world, device, fn, args.steps)
+    last = {}
+    ms, launches = timed_loop(dist, world, device, lambda: last.update(recons=fn()), args.steps)
     if rank == 0:
+        if args.dump_outputs:
+            dump_output(args.dump_outputs, "recons", last["recons"])    # the [B, 3, 512, 512] reconstructions (48 MB at B = 16)
         v = B * world / (ms / 1e3)
         pk = peaks()
         print(json.dumps(_secondary_line("images/sec VQGanVAE encode+VQ+decode 512x512", "images/s", v, ms, world, args,
@@ -626,6 +646,9 @@ if __name__ == "__main__":
     ap.add_argument("--no-extras", "--no-cpu-baseline", dest="no_extras", action="store_true",
                     help="skip cpu_baseline / parity / gpu_eager_baseline / hbm_kernels (N=1 extras)")
     ap.add_argument("--global-batch", type=int, default=GLOBAL_BATCH, help="experiments only; the benchmark config is 64")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned to DIR/<name>.npy (float32; a fixed seeded sample above 48 MB), "
+                         "for output-by-output comparison of builds")
     args = ap.parse_args()
     GLOBAL_BATCH = args.global_batch
     if args.impl == "reference":

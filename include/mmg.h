@@ -1,5 +1,5 @@
 /*
- * mmg.h — C-ABI of libmmg.so: hand-written sm_100a kernels for the MaskGit.generate() hot path.
+ * mmg.h — C-ABI of libmmg.so: hand-written sm_90a kernels for the MaskGit.generate() hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b, "lower face").  Every entry point is
  *     extern "C" int mmg_<op>(const mmg_<op>_args* a, void* cuda_stream);
@@ -9,7 +9,7 @@
  *   - no ownership transfer; the caller (PyTorch) owns all buffers;
  *   - mmg_last_error() returns a thread-local, human readable description of the last failure;
  *   - activations are row-major "token-major" matrices [rows, channels] (images: NHWC); `dtype` selects the
- *     operand type of a matrix product: MMG_BF16 -> tcgen05 tensor-core path (fp32 accumulate in TMEM),
+ *     operand type of a matrix product: MMG_BF16 -> wgmma tensor-core path (fp32 accumulate),
  *     MMG_F32 -> fp32 CUDA-core path ("parity precision").  There is no CPU path in this library.
  *
  * Each function cites the reference code it replaces (paths relative to /root/reference/muse_maskgit_pytorch/).
@@ -29,7 +29,7 @@ extern "C" {
 #define MMG_OK            0
 #define MMG_EINVAL       -1   /* bad argument / unsupported shape */
 #define MMG_ECUDA        -2   /* CUDA runtime / driver error (see mmg_last_error) */
-#define MMG_EUNSUPPORTED -3   /* device is not sm_100 */
+#define MMG_EUNSUPPORTED -3   /* device is not sm_90 */
 
 /* operand dtypes */
 #define MMG_F32  0
@@ -39,7 +39,7 @@ int         mmg_version(void);
 const char* mmg_last_error(void);
 /* Number of kernel launches issued through this library by the calling process (bench.py "gpu_launches"). */
 int64_t     mmg_launch_count(void);
-/* Number of bf16 matrix products / convolutions of this process that fell off the tcgen05 path onto the CUDA-core kernel because of their shape
+/* Number of bf16 matrix products / convolutions of this process that fell off the wgmma path onto the CUDA-core kernel because of their shape
  * or alignment (K or Cin % 64, N % 64, 16-byte rows, conv tile geometry).  MMG_VERBOSE=1 logs each one to stderr. */
 int64_t     mmg_simt_fallback_count(void);
 /* Number of launches of the CUDA-core matrix-product / attention kernels (any dtype) by this process.  precision="fp32" runs its products on the
@@ -109,7 +109,7 @@ typedef struct {
   const void* a;           /* [M, lda] operand dtype                                                             */
   const void* w;           /* [N, ldw] operand dtype (nn.Linear weight layout, K contiguous)                     */
   int64_t M, N, K, lda, ldw;
-  int32_t dtype;           /* MMG_BF16: tcgen05 path (K % 64 == 0, N % 64 == 0, 16B-aligned rows); MMG_F32: CUDA cores */
+  int32_t dtype;           /* MMG_BF16: wgmma path (K % 64 == 0, N % 64 == 0, 16B-aligned rows); MMG_F32: CUDA cores */
   int32_t epilogue;        /* enum mmg_epilogue                                                                   */
   mmg_epilogue_args epi;
 } mmg_linear_args;
@@ -257,7 +257,7 @@ typedef struct {
 int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream);
 
 /* to_logits + the sampling tail of a decode step in one call, WITHOUT a [rows, V] logits buffer (muse_maskgit_pytorch.py:576-609 on the rows
- * listed in s.masked_pos; bf16 operands, tcgen05): a 4096-column sample GEMM gives every row a candidate threshold, the logits GEMM's epilogue
+ * listed in s.masked_pos; bf16 operands, wgmma): a 4096-column sample GEMM gives every row a candidate threshold, the logits GEMM's epilogue
  * keeps online-softmax partials and emits only the candidates >= threshold (~12 % of the logits) as per-row lists, a finishing kernel runs the
  * exact-rank perturbed argmax of mmg_logits_sample on the lists.  Rows whose threshold missed are redone through materialised logits inside the
  * same call (<= 128 rows per call; beyond that status[1] is raised and the caller must repeat the step with mmg_linear + mmg_logits_sample).
@@ -303,7 +303,7 @@ typedef struct {
   int64_t* ids; int64_t T; int32_t D, bits;
   const void* w_split;                     /* optional, bf16 tokens: [64, D] bf16, rows [hi(bits) | mid(bits) | lo(bits) | 0...] = the 3-way bf16
                                               split of w_in (hi + mid + lo == w_in in fp32; 3 * bits <= 64, D % 64 == 0): the projection then
-                                              runs on the tcgen05 path (mmg_linear + MMG_EPI_LFQ_IDS), one TMA stream over the tokens      */
+                                              runs on the wgmma path (mmg_linear + MMG_EPI_LFQ_IDS), one TMA stream over the tokens      */
 } mmg_vq_lfq_encode_args;
 int mmg_vq_lfq_encode(const mmg_vq_lfq_encode_args* a, void* stream);
 

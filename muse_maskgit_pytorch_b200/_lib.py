@@ -5,7 +5,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("MMG_LIB") or os.path.join(_HERE, "libmmg.so")     # MMG_LIB: instrumented dev builds (scripts/trace_gemm.py)
+LIB_PATH = os.environ.get("MMG_LIB") or os.path.join(_HERE, "libmmg.so")     # MMG_LIB: an alternative build of the library
 
 F32, BF16 = 0, 1
 EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB, EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN = range(10)
@@ -204,7 +204,7 @@ def simt_launch_count():
 
 
 def simt_fallback_count():
-    """bf16 products that left the tcgen05 path for the CUDA-core kernel (shape / alignment): should stay 0 on the benchmark configs."""
+    """bf16 products that left the wgmma path for the CUDA-core kernel (shape / alignment): should stay 0 on the benchmark configs."""
     return int(lib().mmg_simt_fallback_count())
 
 

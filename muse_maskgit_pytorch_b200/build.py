@@ -1,4 +1,4 @@
-"""Build libmmg.so (hand-written sm_100a kernels + C-ABI) in-tree with nvcc.  No torch headers, no pybind:
+"""Build libmmg.so (hand-written sm_90a kernels + C-ABI) in-tree with nvcc.  No torch headers, no pybind:
 the library is a plain C-ABI shared object (include/mmg.h) loaded with ctypes."""
 import os
 import subprocess
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libmmg.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr"]
 
 
@@ -43,7 +43,7 @@ def build(verbose=False, force=False):
         list(ex.map(run, jobs))
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in srcs]
     if force or jobs or _newer(LIB, objs):
-        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

@@ -1,8 +1,8 @@
 // Attention core (dh = 64): out = softmax(scale * q k^T + mask) v over keys [0, Tk), key 0 = learned null key.
 // replaces Attend.forward / flash_attn (attend.py:66-140).
 //   * mmg_attention with dtype MMG_F32  -> fp32 CUDA-core kernel (parity precision)
-//   * mmg_attention with dtype MMG_BF16 -> tcgen05 kernel (mmg_attention_tc.cuh): S = Q K^T and O = P V on the tensor
-//     cores with S/P/O resident in TMEM.
+//   * mmg_attention with dtype MMG_BF16 -> wgmma kernel (mmg_attention_tc.cuh): S = Q K^T and O = P V on the tensor
+//     cores, S staged through shared memory, O accumulated in registers.
 #include "mmg_common.cuh"
 #include "mmg_attention_tc.cuh"
 #include "mmg_attention_split.cuh"
@@ -76,12 +76,13 @@ attention_simt_kernel(const T* __restrict__ q, const T* __restrict__ k, const T*
   }
 }
 
-template <uint32_t COLS>
-static int attn_launch_cols(const AttnTcParams& p, dim3 grid, size_t smem, cudaStream_t st) {
+template <int KB>
+static int attn_launch(const AttnTcParams& p, dim3 grid, cudaStream_t st) {
+  constexpr size_t smem = attn_smem_bytes(KB);
   static std::once_flag once; static cudaError_t err = cudaSuccess;
-  std::call_once(once, [] { err = cudaFuncSetAttribute(attention_tc_kernel<COLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); });
+  std::call_once(once, [] { err = cudaFuncSetAttribute(attention_tc_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); });
   if (err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(attention_tc): %s", cudaGetErrorString(err));
-  MMG_CUDA(launch_pdl(attention_tc_kernel<COLS>, grid, dim3(160), smem, st, p));
+  MMG_CUDA(launch_pdl(attention_tc_kernel<KB>, grid, dim3(160), smem, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -106,12 +107,10 @@ int attention_tc_launch(const mmg_attention_args* a, cudaStream_t st) {
     int rc = make_tmap_bf16(&p.tma_k, a->k, 2, dims, str, box); if (rc) return rc;
     rc = make_tmap_bf16(&p.tma_v, a->v, 2, dims, str, box); if (rc) return rc;
   }
-  const int kvb = (p.KB * 128 + 1023) & ~1023;
-  const size_t smem = 1024 + 16384 + 2 * (size_t)kvb + (size_t)((p.KB + 63) / 64) * 16384 + 128;
   dim3 grid((a->Tq + 127) / 128, (unsigned)BH);
-  if (p.KB <= 64) return attn_launch_cols<128>(p, grid, smem, st);
-  if (p.KB <= 192) return attn_launch_cols<256>(p, grid, smem, st);
-  return attn_launch_cols<512>(p, grid, smem, st);
+  if (p.KB == 32) return attn_launch<32>(p, grid, st);
+  if (p.KB == 64) return attn_launch<64>(p, grid, st);
+  return attn_launch<128>(p, grid, st);
 }
 
 // fp32 parity on the tensor cores: q / k / v arrive as 3-way bf16 splits (384 columns per row), see mmg_attention_split.cuh

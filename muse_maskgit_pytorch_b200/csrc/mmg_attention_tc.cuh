@@ -1,21 +1,21 @@
-// tcgen05 attention for dh = 64 (bf16 operands, fp32 softmax statistics).
+// wgmma attention for dh = 64 (bf16 operands, fp32 softmax statistics).
 //
 // One CTA = one (batch, head, 128-query tile).  Key 0 of every (batch, head) is the learned null key: it is never masked, and it is handled
 // OUTSIDE the tensor-core blocks — each softmax thread computes its row's q . k_null with 64 FMAs, its weight joins the row sum and
 // p_null * v_null is added to O in the epilogue — so that the n = 256 (1 024, 32) real keys are exactly 4 (8, 1) blocks instead of 4 + a block
-// that holds one key.  The real keys 1 .. Tk-1 are walked in nb blocks of KB (<= 256, multiple of 32) keys (the last block
+// that holds one key.  The real keys 1 .. Tk-1 are walked in nb blocks of KB (32, 64 or 128) keys (the last block
 // may be shorter: KB_tail), twice (or once, see single_pass):
-//   pass A:  S = Q K^T (tcgen05.mma, M=128, N=KB, 4 k-steps) -> TMEM -> per-row running max        (no P, no V traffic)
+//   pass A:  S = Q K^T (wgmma, 2 x m64nKBk16, 4 k-steps) -> shared-memory staging -> per-row running max        (no P, no V traffic)
 //   pass B:  S again -> p = exp2((s - max) * scale*log2e) in registers (masked / out-of-range keys -> 0), row sums in fp32,
-//            P (bf16) written to shared memory in the K-major SWIZZLE_128B operand layout, O += P V (tcgen05.mma, M=128,
-//            N=64, KB/16 k-steps, V consumed MN-major straight from its TMA tile) accumulating in TMEM across blocks.
+//            P (bf16) written to shared memory in the K-major SWIZZLE_128B operand layout, O += P V (wgmma, 2 x m64n64k16,
+//            KB_tail/16 k-steps, V consumed MN-major straight from its TMA tile) accumulating in registers across blocks.
 //   finally: O / rowsum -> bf16 -> out[b, t, h*64 : (h+1)*64].
 // The exact two-pass softmax (true row max, as attend.py:131) avoids the rescaling chain of an online softmax; the second
-// Q K^T costs 4 extra MMAs per block.  Warp 4 is the control warp (one elected lane: TMA loads + MMA issue); warps 0-3
-// own TMEM lane quarters 0-3 = query rows.
+// Q K^T costs 4 extra MMAs per block.  Warps 0-3 are one warpgroup: they issue the wgmma and own the query rows (thread = row once the
+// accumulators are staged); warp 4 (one elected lane) issues the TMA loads of the next block as soon as a block is done with K / V.
 #pragma once
 #include "mmg_common.cuh"
-#include "mmg_sm100.cuh"
+#include "mmg_sm90.cuh"
 #include <cudaTypedefs.h>
 #include <float.h>
 
@@ -33,131 +33,77 @@ struct alignas(64) AttnTcParams {
   int single_pass;
 };
 
-template <uint32_t TMEM_COLS>
+// Shared memory of one CTA (launcher and kernel agree on it): Q, K, V, P tiles and the fp32 staging of S / O
+__host__ __device__ constexpr int attn_stg_ld(int KB) { return (KB > 64 ? KB : 64) + 4; }
+__host__ __device__ constexpr size_t attn_smem_bytes(int KB) {
+  return 1024 + 16384 + 2 * (size_t)((KB * 128 + 1023) & ~1023) + (size_t)((KB + 63) / 64) * 16384 + (size_t)128 * attn_stg_ld(KB) * 4 + 128;
+}
+
+template <int KB>
 __global__ void __launch_bounds__(160, 1)
 attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
-  using namespace sm100;
+  using namespace sm90;
+  constexpr int LD = attn_stg_ld(KB);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  const int KB = p.KB;
-  const int kv_bytes = KB * 128;
+  constexpr int kv_bytes = KB * 128;
   uint8_t* sQ = smem;                         // 128 x 64 bf16
   uint8_t* sK = sQ + 16384;                   // KB x 64
   uint8_t* sV = sK + ((kv_bytes + 1023) & ~1023);
   uint8_t* sP = sV + ((kv_bytes + 1023) & ~1023);      // ceil(KB/64) sub-tiles of 128 x 64 bf16
-  const int p_tiles = (KB + 63) / 64;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + p_tiles * 16384);
-  uint64_t* bar_q = bars + 0; uint64_t* bar_kv = bars + 1; uint64_t* bar_s = bars + 2;
-  uint64_t* bar_sdone = bars + 3; uint64_t* bar_p = bars + 4; uint64_t* bar_pv = bars + 5; uint64_t* bar_k = bars + 6;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 7);
+  constexpr int p_tiles = (KB + 63) / 64;
+  float* stg = reinterpret_cast<float*>(sP + p_tiles * 16384);    // 128 x LD fp32: S of a block, finally O
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg + 128 * LD);
+  uint64_t* bar_q = bars + 0; uint64_t* bar_kv = bars + 1; uint64_t* bar_free = bars + 2;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // warpgroup index broadcast from lane 0: provably uniform, so the wgmma of the softmax warpgroup are not treated as divergent code
+  const int wg_role = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int bh = blockIdx.y, b = bh / p.heads, h = bh % p.heads;
   const int q0 = blockIdx.x * 128;
   const int kvh = p.kv_shared ? h : bh;
 
   if (warp == 4 && lane == 0) {
     prefetch_tmap(&p.tma_q); prefetch_tmap(&p.tma_k); prefetch_tmap(&p.tma_v);
-    mbar_init(bar_q, 1); mbar_init(bar_kv, 1); mbar_init(bar_s, 1); mbar_init(bar_sdone, 4); mbar_init(bar_p, 4); mbar_init(bar_pv, 1); mbar_init(bar_k, 1);
+    mbar_init(bar_q, 1); mbar_init(bar_kv, 1); mbar_init(bar_free, 4);
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc<TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_wait();
   pdl_trigger();
-  const uint32_t tS = tmem_base;                       // KB fp32 columns
-  const uint32_t tO = tmem_base + TMEM_COLS - 64;      // 64 fp32 columns
 
-  if (warp == 4) {
+  if (wg_role == 1) {
     if (elect_one()) {
-      const uint32_t idesc_s = idesc_bf16_f32(128, (uint32_t)KB, false, false);
-      const uint32_t idesc_s_tail = idesc_bf16_f32(128, (uint32_t)p.KB_tail, false, false);
-      const uint32_t idesc_o = idesc_bf16_f32(128, 64, false, true);          // B (= V) is MN-major
-      const uint64_t qdesc = smem_desc_kmajor_sw128(smem_u32(sQ));
-      const uint64_t kdesc = smem_desc_kmajor_sw128(smem_u32(sK));
-      auto issue_s = [&](int blk) {
-        const uint32_t id = blk == p.nb - 1 ? idesc_s_tail : idesc_s;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(tS, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), id, k ? 1u : 0u);
-        umma_commit(bar_s);
-      };
-      auto issue_pv = [&](int blk) {
-        const int ksteps = (blk == p.nb - 1 ? p.KB_tail : KB) / 16;
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint32_t pa = smem_u32(sP) + (ks >> 2) * 16384 + (ks & 3) * 32;
-          umma_f16(tO, smem_desc_kmajor_sw128(pa), smem_desc_mnmajor_sw128(smem_u32(sV) + ks * 2048, 1024), idesc_o, (blk | ks) ? 1u : 0u);
-        }
-        umma_commit(bar_pv);
-      };
-      if (p.single_pass) {
-        // K(blk+1) is fetched as soon as S(blk) has retired and V(blk) while the softmax of S(blk) runs: loads are off the
-        // critical path, which is  S-MMA -> softmax -> PV-MMA  per key block.
-        uint32_t ph_s = 0, ph_p = 0, ph_pv = 0, ph_v = 0, ph_k = 0;
-        const int krow0 = kvh * p.Tk_alloc + 1;                  // real keys start at row 1
-        mbar_expect_tx(bar_q, 16384 + kv_bytes);
-        tma_load_2d(sQ, &p.tma_q, bar_q, 0, bh * p.Tq + q0);
-        tma_load_2d(sK, &p.tma_k, bar_q, 0, krow0);
-        mbar_expect_tx(bar_kv, kv_bytes);
-        tma_load_2d(sV, &p.tma_v, bar_kv, 0, krow0);
-        mbar_wait(bar_q, 0);
-        tc_fence_after();
-        issue_s(0);
-        for (int blk = 0; blk < p.nb; ++blk) {
-          const bool more = blk + 1 < p.nb;
-          mbar_wait(bar_s, ph_s); ph_s ^= 1;                     // S(blk) retired: K smem reusable
-          if (more) { mbar_expect_tx(bar_k, kv_bytes); tma_load_2d(sK, &p.tma_k, bar_k, 0, krow0 + (blk + 1) * KB); }
-          mbar_wait(bar_p, ph_p); ph_p ^= 1;                     // P(blk) staged, S(blk) consumed
-          mbar_wait(bar_kv, ph_v); ph_v ^= 1;                    // V(blk) landed
-          tc_fence_after();
-          issue_pv(blk);
-          if (more) { mbar_wait(bar_k, ph_k); ph_k ^= 1; tc_fence_after(); issue_s(blk + 1); }
-          mbar_wait(bar_pv, ph_pv); ph_pv ^= 1;                  // P / V smem reusable; after the last block O is final
-          if (more) { mbar_expect_tx(bar_kv, kv_bytes); tma_load_2d(sV, &p.tma_v, bar_kv, 0, krow0 + (blk + 1) * KB); }
-        }
-      } else {
+      // one K (pass A) or K + V (pass B) load per block, each after the softmax warpgroup is done with the previous block's tiles
       mbar_expect_tx(bar_q, 16384);
       tma_load_2d(sQ, &p.tma_q, bar_q, 0, bh * p.Tq + q0);
-      mbar_wait(bar_q, 0);
-      uint32_t ph_kv = 0, ph_sdone = 0, ph_p = 0, ph_pv = 0;
-      for (int pass = 0; pass < 2; ++pass) {
-        for (int blk = 0; blk < p.nb; ++blk) {
-          const int krow = kvh * p.Tk_alloc + 1 + blk * KB;
+      uint32_t ph_free = 0;
+      int loads = 0;
+      for (int pass = p.single_pass ? 1 : 0; pass < 2; ++pass) {
+        for (int blk = 0; blk < p.nb; ++blk, ++loads) {
+          if (loads) { mbar_wait(bar_free, ph_free); ph_free ^= 1; }
+          const int krow = kvh * p.Tk_alloc + 1 + blk * KB;                 // real keys start at row 1
           mbar_expect_tx(bar_kv, pass == 0 ? kv_bytes : 2 * kv_bytes);
           tma_load_2d(sK, &p.tma_k, bar_kv, 0, krow);
           if (pass == 1) tma_load_2d(sV, &p.tma_v, bar_kv, 0, krow);
-          mbar_wait(bar_kv, ph_kv); ph_kv ^= 1;
-          tc_fence_after();
-          issue_s(blk);
-          if (pass == 0) {
-            mbar_wait(bar_sdone, ph_sdone); ph_sdone ^= 1;      // softmax warps consumed S; K smem is free (MMA retired before S was readable)
-          } else {
-            mbar_wait(bar_p, ph_p); ph_p ^= 1;                  // P staged in smem (and S consumed)
-            tc_fence_after();
-            issue_pv(blk);
-            mbar_wait(bar_pv, ph_pv); ph_pv ^= 1;               // K/V/P smem free again; on the last block: O complete
-          }
         }
-      }
       }
     }
     __syncwarp();
   } else {
-    // ===================== softmax warps: thread = query row =====================
+    // ===================== softmax warpgroup: wgmma, then thread = query row =====================
     const int r = warp * 32 + lane;
     const int qi = q0 + r;
-    const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
+    const float* srow = stg + r * LD;
     const uint8_t* km = p.key_mask ? p.key_mask + (int64_t)b * (p.Tk - 1) : nullptr;   // one byte per REAL key
     const int Tr = p.Tk - 1;                                     // real keys
-    uint32_t ph_s = 0, ph_pv = 0;
+    uint32_t ph_kv = 0;
     float row_sum = 0.f;
     float mneg = 0.f;
     // the null key: s0 = q_r . k_null (Q tile: row r at r * 128 bytes, 16-byte chunk c at position c ^ (r & 7))
     const bf16* knull = p.k + (int64_t)kvh * p.Tk_alloc * 64;
     float s0 = 0.f;
-    mbar_wait(bar_q, 0);                                        // Q has landed (the control warp waits on the same phase)
+    mbar_wait(bar_q, 0);
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
       const uint4 qv = *reinterpret_cast<const uint4*>(sQ + r * 128 + ((c ^ (r & 7)) * 16));
@@ -169,6 +115,11 @@ attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
     }
     float row_max = s0;                                         // the null key is always live
     float p_null = 0.f;
+    float o_acc[2][32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { o_acc[0][i] = 0.f; o_acc[1][i] = 0.f; }
+    const uint64_t qdesc = smem_desc_kmajor_sw128(smem_u32(sQ));
+    const uint64_t kdesc = smem_desc_kmajor_sw128(smem_u32(sK));
     for (int pass = p.single_pass ? 1 : 0; pass < 2; ++pass) {
       if (pass == 1) {
         mneg = (p.single_pass ? p.smax : row_max) * p.scale_log2e;
@@ -176,13 +127,26 @@ attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
         row_sum = p_null;
       }
       for (int blk = 0; blk < p.nb; ++blk) {
-        mbar_wait(bar_s, ph_s); ph_s ^= 1;
-        tc_fence_after();
+        mbar_wait(bar_kv, ph_kv); ph_kv ^= 1;
+        {   // S = Q K^T for the 128 query rows (two m64 halves), staged row-major
+          float s_acc[2][KB / 2];
+          wgmma_fence();
+#pragma unroll
+          for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) Wgmma<KB>::template mma<0>(s_acc[mh], qdesc + (uint64_t)(mh * 512 + k * 2), kdesc + (uint64_t)(k * 2), k ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(s_acc[0]); reg_fence(s_acc[1]);
+          named_sync(1, 128);                                    // every row of the previous block's S has been read
+          stage_acc<KB / 2, LD>(s_acc[0], stg, 0, KB);
+          stage_acc<KB / 2, LD>(s_acc[1], stg + 64 * LD, 0, KB);
+          named_sync(1, 128);
+        }
         const int kb_cur = blk == p.nb - 1 ? p.KB_tail : KB;
         for (int c = 0; c < kb_cur; c += 32) {
           float s[32];
-          tmem_ld_32x32b_x32(tS + lane_base + c, s);
-          tmem_ld_wait();
+          stage_ld32(srow + c, s);
           const int j0 = blk * KB + c;
           // liveness of the 32 keys of this chunk as one ballot word (lane l tests key j0 + l: ONE coalesced mask byte per lane instead of 32
           // byte loads per thread; key 0, the null key, is never masked)
@@ -234,31 +198,36 @@ attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
             }
           }
         }
-        tc_fence_before();
-        if (pass == 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_sdone);
-        } else {
-          fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core (async proxy)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_p);
-          mbar_wait(bar_pv, ph_pv); ph_pv ^= 1;  // this block's P.V retired (P smem reusable; after the last block O is final)
+        if (pass == 1) {
+          fence_proxy_async();                 // generic-proxy smem writes of P -> visible to the tensor core (async proxy)
+          named_sync(1, 128);
+          const int ksteps = (blk == p.nb - 1 ? p.KB_tail : KB) / 16;
+          for (int ks = 0; ks < ksteps; ++ks) {
+            wgmma_fence();
+            const uint32_t pa = smem_u32(sP) + (ks >> 2) * 16384 + (ks & 3) * 32;
+            const uint64_t vdesc = smem_desc_mnmajor_sw128(smem_u32(sV) + ks * 2048, 1024);
+            Wgmma<64>::template mma<1>(o_acc[0], smem_desc_kmajor_sw128(pa), vdesc, 1u);
+            Wgmma<64>::template mma<1>(o_acc[1], smem_desc_kmajor_sw128(pa + 8192), vdesc, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(o_acc[0]); reg_fence(o_acc[1]);
         }
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_free);                    // K / V / P of this block are no longer needed
       }
     }
-    tc_fence_after();
+    named_sync(1, 128);
+    stage_acc<32, LD>(o_acc[0], stg, 0, 64);
+    stage_acc<32, LD>(o_acc[1], stg + 64 * LD, 0, 64);
+    named_sync(1, 128);
     const float inv = 1.f / row_sum;
     const bf16* vnull = p.v + (int64_t)kvh * p.Tk_alloc * 64;
 #pragma unroll
     for (int c = 0; c < 64; c += 32) {
       float o[32];
-      if (p.nb > 0) {
-        tmem_ld_32x32b_x32(tO + lane_base + c, o);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = 0.f;                  // no real key at all: the output is the null value
-      }
+      stage_ld32(srow + c, o);                                     // no real key at all (nb == 0): zero, the output is the null value
 #pragma unroll
       for (int i = 0; i < 32; i += 8) {                          // + p_null * v_null (fp32; p_null unrounded in numerator and denominator)
         const uint4 vv = __ldg(reinterpret_cast<const uint4*>(vnull + c + i));
@@ -280,9 +249,6 @@ attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) { tc_fence_after(); tmem_dealloc<TMEM_COLS>(tmem_base); }
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------
@@ -291,13 +257,12 @@ inline bool attention_tc_supported(const mmg_attention_args* a) {
   return al(a->q) && al(a->k) && al(a->v) && al(a->out) && (a->ldo % 8 == 0) && a->Tk >= 2 && a->Tk <= 4096;
 }
 
-// Key blocking: nb-1 blocks of KB keys and a last block of KB_tail keys (multiple of 32).  KB = 64 keeps S (64 fp32 columns) + O (64)
-// inside a 128-column TMEM allocation and ~50 KB of shared memory, so four CTAs share an SM and hide each other's
-// MMA -> softmax -> MMA round trips; long sequences use 128-key blocks (fewer round trips per CTA, two CTAs per SM).
+// Key blocking: nb-1 blocks of KB keys and a last block of KB_tail keys (multiple of 32).  KB = 64 keeps a CTA at ~84 KB of shared memory,
+// so two CTAs share an SM and hide each other's MMA -> softmax -> MMA round trips; long sequences use 128-key blocks (fewer round trips per CTA).
 inline void attn_blocks(int Tk, int* nb, int* KB, int* KB_tail) {
   static const int forced = [] { const char* e = getenv("MMG_ATTN_KB"); return e ? atoi(e) : 0; }();
   int kb = forced ? forced : (Tk <= 640 ? 64 : 128);
-  if (kb != 32 && kb != 64 && kb != 128 && kb != 160 && kb != 256) kb = 64;
+  if (kb != 32 && kb != 64 && kb != 128) kb = 64;
   const int full = Tk / kb, rem = Tk - full * kb;
   *KB = kb;
   if (rem == 0) { *nb = full; *KB_tail = kb; }

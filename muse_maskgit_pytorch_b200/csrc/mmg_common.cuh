@@ -1,4 +1,4 @@
-// Shared host/device helpers for libmmg (sm_100a only).
+// Shared host/device helpers for libmmg (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -21,7 +21,7 @@ inline int fail(int code, const char* fmt, ...) {
   return code;
 }
 inline std::atomic<int64_t>& launch_counter() { static std::atomic<int64_t> c{0}; return c; }
-// bf16 matrix products / convolutions that could not take the tcgen05 path (K or Cin % 64, N % 64, alignment, tile geometry) and ran on the
+// bf16 matrix products / convolutions that could not take the wgmma path (K or Cin % 64, N % 64, alignment, tile geometry) and ran on the
 // CUDA-core kernel instead: a >100x performance cliff, so it is counted (mmg_simt_fallback_count) and, with MMG_VERBOSE=1, logged once per shape
 inline std::atomic<int64_t>& simt_fallback_counter() { static std::atomic<int64_t> c{0}; return c; }
 // every launch of the CUDA-core matrix-product / attention kernels (any dtype): the fp32 parity mode is expected to keep this at zero on
@@ -30,7 +30,7 @@ inline std::atomic<int64_t>& simt_launch_counter() { static std::atomic<int64_t>
 inline void note_simt_fallback(const char* what, long long M, long long N, long long K) {
   simt_fallback_counter()++;
   static const bool verbose = [] { const char* e = getenv("MMG_VERBOSE"); return e && e[0] == '1'; }();
-  if (verbose) fprintf(stderr, "[libmmg] %s M=%lld N=%lld K=%lld (bf16) runs on the CUDA-core kernel: shape / alignment outside the tcgen05 path\n", what, M, N, K);
+  if (verbose) fprintf(stderr, "[libmmg] %s M=%lld N=%lld K=%lld (bf16) runs on the CUDA-core kernel: shape / alignment outside the wgmma path\n", what, M, N, K);
 }
 
 #define MMG_CHECK_ARG(cond, ...) do { if (!(cond)) return ::mmg::fail(MMG_EINVAL, __VA_ARGS__); } while (0)
@@ -42,7 +42,7 @@ inline void note_simt_fallback(const char* what, long long M, long long N, long 
 
 inline int num_sms() {
   static int n = 0;
-  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
   return n;
 }
 
@@ -50,7 +50,7 @@ inline int num_sms() {
 // Hot-loop kernels are launched with cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs become
 // resident (and run their prologue) while the previous grid drains, then block in griddepcontrol.wait until that grid has
 // completed and flushed.  Every kernel launched this way calls pdl_wait() before its first global access.  Opt-in with MMG_PDL=1:
-// measured on B200 it is a wash under CUDA-graph replay (+1 % at batch 8, -2 % at batch 64), so the default is off.
+// under CUDA-graph replay the launch gaps it hides are already small, so the default is off.
 inline bool pdl_enabled() { static int v = -1; if (v < 0) { const char* e = getenv("MMG_PDL"); v = (e && e[0] == '1') ? 1 : 0; } return v != 0; }
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
@@ -88,17 +88,19 @@ __device__ __forceinline__ float warp_max(float v) {
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float leaky01(float x) { return x > 0.f ? x : 0.1f * x; }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per lane
+// one full 32-byte sector per lane as two adjacent 16-byte accesses (p 32-byte aligned)
 __device__ __forceinline__ void st256(void* p, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t a4, uint32_t a5, uint32_t a6, uint32_t a7) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" :: "l"(p), "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(a4), "r"(a5), "r"(a6), "r"(a7) : "memory");
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.v4.b32 [%0+16], {%5,%6,%7,%8};"
+               :: "l"(p), "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(a4), "r"(a5), "r"(a6), "r"(a7) : "memory");
 }
 __device__ __forceinline__ void ld256(const void* p, uint32_t (&a)[8]) {
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]) : "l"(p));
+  asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%8];\n\tld.global.v4.b32 {%4,%5,%6,%7}, [%8+16];"
+               : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]) : "l"(p));
 }
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) { __nv_bfloat162 t = __floats2bfloat162_rn(a, b); return *reinterpret_cast<uint32_t*>(&t); }
 __device__ __forceinline__ bool aligned32(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 31) == 0; }
 
-// load/store 64 consecutive elements of T from/to a 16B-aligned row chunk (256-bit accesses when 32B-aligned)
+// load/store 64 consecutive elements of T from/to a 16B-aligned row chunk (whole 32-byte sectors per access pair when 32B-aligned)
 template <typename T> struct Vec64;
 template <> struct Vec64<float> {
   static __device__ __forceinline__ void store(float* p, const float (&v)[64]) {

@@ -527,7 +527,7 @@ extern "C" int mmg_cast(const mmg_cast_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->src && a->dst, "mmg_cast: NULL pointer");
   if (a->n == 0) return MMG_OK;
-  const unsigned grid = (unsigned)((a->n + 255) / 256 < 148 * 16 ? (a->n + 255) / 256 : 148 * 16);
+  const unsigned grid = (unsigned)((a->n + 255) / 256 < num_sms() * 16 ? (a->n + 255) / 256 : num_sms() * 16);
   if (a->src_dtype == MMG_F32 && a->dst_dtype == MMG_BF16) cast_kernel<float, bf16><<<grid, 256, 0, st>>>((const float*)a->src, (bf16*)a->dst, a->n);
   else if (a->src_dtype == MMG_BF16 && a->dst_dtype == MMG_F32) cast_kernel<bf16, float><<<grid, 256, 0, st>>>((const bf16*)a->src, (float*)a->dst, a->n);
   else return fail(MMG_EINVAL, "mmg_cast: unsupported dtype pair");
@@ -543,7 +543,7 @@ extern "C" int mmg_split3(const mmg_split3_args* a, void* stream) {
   MMG_CHECK_ARG((reinterpret_cast<uintptr_t>(a->src) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->dst) & 15) == 0, "mmg_split3: 16-byte alignment");
   if (a->rows == 0) return MMG_OK;
   const int64_t work = a->rows * (a->K / 8);
-  const unsigned grid = (unsigned)((work + 255) / 256 < 148 * 16 ? (work + 255) / 256 : 148 * 16);
+  const unsigned grid = (unsigned)((work + 255) / 256 < num_sms() * 16 ? (work + 255) / 256 : num_sms() * 16);
   split3_kernel<<<grid, 256, 0, st>>>(a->src, reinterpret_cast<bf16*>(a->dst), a->rows, a->K, a->lds, a->side);
   MMG_LAUNCHED();
   return MMG_OK;

@@ -1,4 +1,4 @@
-// Fused GEMM epilogues, shared by the tcgen05 kernel (mmg_gemm_tc.cu) and the fp32 CUDA-core kernel
+// Fused GEMM epilogues, shared by the wgmma kernel (mmg_gemm_tc.cuh) and the fp32 CUDA-core kernel
 // (mmg_gemm_simt.cu).  One thread owns one output row and walks it in chunks of 64 accumulator columns.
 #pragma once
 #include "mmg_common.cuh"

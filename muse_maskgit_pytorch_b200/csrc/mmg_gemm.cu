@@ -1,4 +1,4 @@
-// mmg_linear / mmg_conv2d / mmg_conv_transpose2d: launchers for the tcgen05 GEMM (bf16) and the fp32 CUDA-core GEMM.
+// mmg_linear / mmg_conv2d / mmg_conv_transpose2d: launchers for the wgmma GEMM (bf16) and the fp32 CUDA-core GEMM.
 #include "mmg_gemm_tc.cuh"
 #include "mmg_tmap.cuh"
 #include <mutex>
@@ -27,11 +27,11 @@ template <int BN>
 static int launch_tc_red(const TcGemmParams& p, cudaStream_t st) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
   if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_red<%d>): %s", BN, cudaGetErrorString(attr_err));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, false, 2>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
+  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, 2>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -41,11 +41,11 @@ template <int BN>
 static int launch_tc_tstore(const TcGemmParams& p, cudaStream_t st) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
   if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_tstore<%d>): %s", BN, cudaGetErrorString(attr_err));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, false, 3>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
+  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, 3>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -55,11 +55,11 @@ template <int BN, int MODE = 4>
 static int launch_tc_qkvt(const TcGemmParams& p, cudaStream_t st) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, false, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
   if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_tiles<%d, %d>): %s", BN, MODE, cudaGetErrorString(attr_err));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, false, MODE>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
+  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, MODE>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -83,68 +83,15 @@ static int launch_tc_lnf(const TcGemmParams& p, cudaStream_t st) {
   return MMG_OK;
 }
 
-// CTA-pair variant (cta_group::2): clusters of two CTAs, one 256 x BN tile per pair and step
-template <int BN, int EPI_MODE = 0>
-static int launch_tc_pair(const TcGemmParams& p, cudaStream_t st) {
-  constexpr int SMEM = EPI_MODE ? TcCfg<BN>::PAIR_SMEM_BYTES_RED : TcCfg<BN>::PAIR_SMEM_BYTES;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  static int max_clusters = 0;
-  std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, true, EPI_MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (attr_err != cudaSuccess) return;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * (num_sms() / 2)); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = SMEM;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    attr_err = cudaOccupancyMaxActiveClusters(&max_clusters, tc_gemm_kernel<BN, false, true, EPI_MODE>, &cfg);
-  });
-  if (attr_err != cudaSuccess || max_clusters < 1) return fail(MMG_ECUDA, "tc_gemm pair<%d> setup: %s (clusters %d)", BN, cudaGetErrorString(attr_err), max_clusters);
-  const int tiles = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-  const int clusters = tiles < max_clusters ? tiles : max_clusters;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * clusters); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = SMEM; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  MMG_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_kernel<BN, false, true, EPI_MODE>, p));
-  MMG_LAUNCHED();
-  return MMG_OK;
-}
-
-// CTA pairs (cta_group::2) cut the L2->SM operand traffic by a third and deepen the ring to six stages: 8192^3 788 -> 732 us (88 % of the
-// measured cuBLAS rate), the VAE 3x3 convolutions (K = 9 Cin) -10 %, FF2 (K = 1408) 57 -> 51 us.  Round 2: the epilogue warps used to hand
-// the TMEM stage back to the leader CTA with mbarrier.arrive.release.cluster, which compiles to MEMBAR.ALL.GPU + ERRBAR and made every
-// warp wait, once per tile, for all of its global stores; with the plain remote arrive (mbar_arrive_remote) pairs also win for the K = 512
-// GEMMs with register epilogues (QKV 54 -> 48 us, GEGLU FF1 101 -> 89 us, fp32 logits 741 -> 640 us) and are the default for every dense
-// product with 256-column tiles; the short residual GEMM (N = 512, two column tiles) stays on single CTAs.  MMG_GEMM_PAIR = 0 / 1 forces the choice.
-static bool use_pair(const TcGemmParams& p, int bn, int epi_mode) {
-  static const int forced = [] { const char* e = getenv("MMG_GEMM_PAIR"); return e ? atoi(e) : -1; }();
-  if (bn != 256 || forced == 0 || p.num_m_tiles < 2) return false;
-  if (forced == 1) return true;
-  if (((p.num_m_tiles + 1) / 2) * p.num_n_tiles < 64) return false;
-  if (epi_mode == 3) return true;
-  if (epi_mode == 2) return p.num_kb >= 16;
-  if (p.mode == 0) return true;                                  // dense products: QKV, GEGLU, plain stores
-  return p.num_kb >= 64 && p.epi.kind != MMG_EPI_CONVT && p.epi.kind != MMG_EPI_CONVT_RGB;
-}
-
 static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
   if (epilogue == MMG_EPI_CONVT_RGB) return (int)N;             // whole row in one tile
-  if (N % 256 == 0 && M_tiles * (N / 256) >= 2 * 148) return 256;
-  if (N % 128 == 0 && M_tiles * (N / 128) >= 148) return 128;
+  if (N % 256 == 0 && M_tiles * (N / 256) >= 2 * num_sms()) return 256;
+  if (N % 128 == 0 && M_tiles * (N / 128) >= num_sms()) return 128;
   if (N % 128 == 0 && N >= 1024) return 128;
   return (N % 64 == 0 && N % 128 != 0) ? 64 : ((M_tiles * ((N + 127) / 128) >= 96) ? 128 : 64);
 }
 
 static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
-  p.num_n_tiles = (int)((N + bn - 1) / bn);
-  {
-    static const int nfast_forced = [] { const char* e = getenv("MMG_GEMM_NFAST"); return e ? atoi(e) : -1; }();
-    p.n_fast = nfast_forced >= 0 ? nfast_forced : ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
-  }
   const mmg_epilogue_args& e = p.epi.p;
   const bool in_place = (p.epi.kind == MMG_EPI_LNFOLD_RESIDUAL || (p.epi.kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
                         e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && !e.ln_out && p.mode == 0;
@@ -158,8 +105,15 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
   const bool geglu_tiles = p.epi.kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && bn == 256 && (e.ldo % 8) == 0 && aligned16(e.out);
   const int epi_mode = (in_place && red_forced != 0) ? 2 : (plain_f32 && tstore_forced != 0 && (bn == 256 || bn == 128)) ? 3 : (qkv_tiles && qkvt_forced != 0) ? 4 :
                        (geglu_tiles && geglut_forced != 0) ? 5 : 0;
-  const bool pair = use_pair(p, bn, epi_mode >= 4 ? 0 : epi_mode);
-  uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)(pair ? bn / 2 : bn)};
+  // the register epilogue (EPI_MODE 0) keeps 128 accumulator registers per thread at BN = 256 next to its 64-column chunk and spills; the
+  // tile epilogues at BN = 256 and every epilogue at BN = 128 fit the consumer warpgroups' registers
+  if (epi_mode == 0 && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
+  p.num_n_tiles = (int)((N + bn - 1) / bn);
+  {
+    static const int nfast_forced = [] { const char* e = getenv("MMG_GEMM_NFAST"); return e ? atoi(e) : -1; }();
+    p.n_fast = nfast_forced >= 0 ? nfast_forced : ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
+  }
+  uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
   int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
   if (epi_mode == 4) {
     const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads;
@@ -170,19 +124,17 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
       rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
       rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
     }
-    if (!pair) return bn == 256 ? launch_tc_qkvt<256>(p, st) : launch_tc_qkvt<128>(p, st);
-    return launch_tc_pair<256, 4>(p, st);
+    return bn == 256 ? launch_tc_qkvt<256>(p, st) : launch_tc_qkvt<128>(p, st);
   }
   if (epi_mode == 5) {
     uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 32};
     rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
-    return pair ? launch_tc_pair<256, 5>(p, st) : launch_tc_qkvt<256, 5>(p, st);
+    return launch_tc_qkvt<256, 5>(p, st);
   }
   if (epi_mode) {
     uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 32};
     rc = make_tmap_f32(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
   }
-  if (pair) return epi_mode == 2 ? launch_tc_pair<256, 2>(p, st) : epi_mode == 3 ? launch_tc_pair<256, 3>(p, st) : launch_tc_pair<256>(p, st);
   if (epi_mode == 3) return bn == 256 ? launch_tc_tstore<256>(p, st) : launch_tc_tstore<128>(p, st);   // 128: the sample GEMM of the fused tail at small batch
   if (epi_mode == 2) {
     switch (bn) { case 64: return launch_tc_red<64>(p, st); case 128: return launch_tc_red<128>(p, st); case 256: return launch_tc_red<256>(p, st); }
@@ -190,7 +142,7 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
   switch (bn) {
     case 64: return launch_tc<64>(p, st);
     case 128: return launch_tc<128>(p, st);
-    case 256: return launch_tc<256>(p, st);
+    case 256: return launch_tc<256>(p, st);       // CONVT_RGB: the whole 256-column row in one tile
   }
   return fail(MMG_EINVAL, "unsupported tile width %d", bn);
 }
@@ -435,13 +387,3 @@ extern "C" int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* st
   return MMG_OK;
 }
 
-#ifdef MMG_GEMM_TRACE
-extern "C" int mmg_trace_clear(void) {
-  void* p = nullptr;
-  if (cudaGetSymbolAddress(&p, mmg::g_gemm_trace) != cudaSuccess) return -1;
-  return (int)cudaMemset(p, 0, sizeof(mmg::g_gemm_trace));
-}
-extern "C" int mmg_trace_read(void* dst, size_t bytes) {
-  return (int)cudaMemcpyFromSymbol(dst, mmg::g_gemm_trace, bytes < sizeof(mmg::g_gemm_trace) ? bytes : sizeof(mmg::g_gemm_trace));
-}
-#endif

@@ -1,30 +1,32 @@
-// tcgen05 / TMA / TMEM GEMM for sm_100a:  C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulation in TMEM.
+// wgmma / TMA GEMM for sm_90a:  C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulation in registers.
 //
-//   warp 0      : TMA producer  (one elected lane) — A tile 128x64 and W tile BNx64 per k-block, SWIZZLE_128B
-//   warp 1      : TMEM allocator + MMA issuer (one elected lane) — 4 x tcgen05.mma (K=16) per k-block, M=128, N=BN
-//   warps 4..11 : epilogue — tcgen05.ld (32 lanes x 32 cols) -> registers -> fused Epilogue -> global (directly, or through a per-warp
-//                 shared-memory tile and a TMA store / TMA reduction, see EPI_MODE below); two warps share a TMEM lane quarter and
-//                 take alternate 64-column chunks.  setmaxnreg moves registers from warpgroup 0 (40/thread) to the epilogue
-//                 warpgroups (232/thread).
-//   persistent grid (<= #SM CTAs), static tile schedule (M- or N-fastest), STAGES-deep smem ring, 2 accumulator stages in TMEM so
-//   the epilogue of tile i overlaps the main loop of tile i+1.  Variants: LNF (LayerNorm of the output row through a 2-CTA
-//   cluster), PAIR (tcgen05 cta_group::2: one 256 x BN tile per CTA pair).
+//   warp 0      : TMA producer  (one elected lane) — A tile 128x64 and W tile BNx64 per k-block, SWIZZLE_128B, STAGES-deep ring
+//   warps 4..11 : two consumer warpgroups.  Warpgroup g multiplies rows [64 g, 64 g + 64) of the tile (wgmma m64nBNk16, 4 per k-block,
+//                 accumulators in registers), then runs the fused Epilogue on those rows: the accumulators go through a shared-memory
+//                 staging buffer (128 columns at a time) so that one thread owns one output row, 64 columns per chunk; two warps share a
+//                 32-row quarter and take alternate 64-column chunks.  Results leave directly, or through a per-warp shared-memory tile and
+//                 a TMA store / TMA reduction (EPI_MODE below).  setmaxnreg moves registers from warpgroup 0 (40/thread) to the consumers
+//                 (232/thread).
+//   persistent grid (<= #SM CTAs), static tile schedule (M- or N-fastest); the producer runs ahead into the next tile while the consumers
+//   finish the epilogue of the current one.  Variant: LNF (LayerNorm of the output row through a 2-CTA cluster).
 //
 // A is either a dense [M,K] matrix (2-D tensor map) or an NHWC activation addressed as an implicit-GEMM
 // convolution: the k-block (tap, channel-chunk) is fetched with a 4-D tensor map at shifted (x+dx, y+dy)
 // coordinates and TMA's out-of-bounds zero fill provides the padding — no im2col buffer.
 #pragma once
 #include "mmg_common.cuh"
-#include "mmg_sm100.cuh"
+#include "mmg_sm90.cuh"
 #include "mmg_epilogue.cuh"
 
 namespace mmg {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;
-constexpr int TC_THREADS = 384;          // warpgroup 0: warp 0 TMA, warp 1 MMA (2, 3 idle); warpgroups 1-2: 8 epilogue warps
+constexpr int TC_THREADS = 384;          // warpgroup 0: warp 0 TMA (1-3 idle); warpgroups 1-2: wgmma + epilogue
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_MAX_TAPS = 16;
+constexpr int TC_STG_LD = 132;           // staging row stride (floats): 128 columns + 4, conflict-free 16-byte row reads
+constexpr int TC_SMEM_LIMIT = 227 * 1024;
 
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
@@ -45,67 +47,53 @@ struct alignas(64) TcGemmParams {
   Epilogue epi;
 };
 
-// -DMMG_GEMM_TRACE (scripts/trace_gemm.py only): per-CTA, per-tile clock64() stamps of the three roles, to see which of
-// TMA / MMA issue / epilogue a tile period is made of.  Compiles to nothing in the product build.
-#ifdef MMG_GEMM_TRACE
-__device__ long long g_gemm_trace[160 * 32 * 10];
-#define MMG_TR(slot, val) do { if (tile_i < 32) g_gemm_trace[((size_t)blockIdx.x * 32 + tile_i) * 10 + (slot)] = (val); } while (0)
-#define MMG_CLK() clock64()
-#else
-#define MMG_TR(slot, val) do {} while (0)
-#define MMG_CLK() 0ll
-#endif
-
+// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][per-warp output tiles, 32 KB (tile epilogues only)][staging, 2 x 64 x 132 fp32]
 template <int BN> struct TcCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  // in-place reduction epilogue (EPI_MODE 2): one 32-row x 128-byte tile per epilogue warp (1024-byte aligned for the TMA swizzle)
-  static constexpr int SMEM_BYTES_RED = STAGES * STAGE_BYTES + 1024 + 1024 + TC_EPI_WARPS * 4096;
-  static constexpr uint32_t TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  // CTA pair (cta_group::2, M = 256 over two SMs): each CTA stages its own 128 rows of A and HALF of the W tile, so a k-block costs
-  // 32 KB of L2->SM traffic per SM instead of 48 KB and six stages fit where four did
-  static constexpr int PAIR_STAGES = 6;
-  static constexpr int PAIR_STAGE_BYTES = A_BYTES + B_BYTES / 2;
-  static constexpr int PAIR_SMEM_BYTES = PAIR_STAGES * PAIR_STAGE_BYTES + 1024 + 256;
-  static constexpr int PAIR_SMEM_BYTES_RED = PAIR_STAGES * PAIR_STAGE_BYTES + 1024 + 1024 + TC_EPI_WARPS * 4096;
+  static constexpr int STG_BYTES = 2 * 64 * TC_STG_LD * 4;
+  static constexpr int TILE_BYTES = TC_EPI_WARPS * 4096;
+  static constexpr int stages(int extra) {
+    return (TC_SMEM_LIMIT - 1024 - 1024 - STG_BYTES - extra) / STAGE_BYTES < 6 ? (TC_SMEM_LIMIT - 1024 - 1024 - STG_BYTES - extra) / STAGE_BYTES : 6;
+  }
+  // LNF keeps 8 KB of static shared memory for the statistics exchange
+  static constexpr int STAGES = stages(BN == 256 ? 8192 : 0);
+  static constexpr int STAGES_RED = stages(TILE_BYTES);
+  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 1024 + STG_BYTES;
+  static constexpr int SMEM_BYTES_RED = 1024 + STAGES_RED * STAGE_BYTES + 1024 + TILE_BYTES + STG_BYTES;
+  static_assert(STAGES >= 2 && STAGES_RED >= 2, "operand ring too shallow");
 };
 
 // LNF: the epilogue additionally emits LayerNorm(out row) as bf16 (see mmg_epilogue_args::ln_out).  Launched as clusters of two
 // CTAs that own the two column halves (N == 2 * BN) of the same 128 rows; per-row (sum, sumsq) partials cross through DSMEM.
-// PAIR: launched as clusters of two CTAs that form one tcgen05 CTA pair: a 256 x BN output tile per pair, the leader (rank 0) issues
-// the MMAs for both SMs, TMA completions of both CTAs are counted on the leader's barriers, MMA commits are multicast to both.
-// One thread owns one output ROW, so a direct 32-byte store / load touches 32 different 128-byte lines per instruction and the L1
-// pipeline retires it at ~2 cycles per line: 16.7 B/clk/SM measured (scripts/stbench.cu) — 7 850 cycles for a 128 KB fp32 tile whose
-// MMAs take ~4 100.  The fp32 epilogues therefore leave through shared memory and the TMA engine instead:
+// One thread owns one output ROW, so a direct 32-byte store / load touches 32 different 128-byte lines per instruction, and the L1
+// retires such row-strided accesses slowly.  The fp32 epilogues therefore leave through shared memory and the TMA engine instead:
 // EPI_MODE 2 (RED): in-place residual epilogues (out == resid, fp32) write the term they add into a per-warp
 // 32 x 32 tile and push it with ONE TMA reduction (cp.reduce.async.bulk.tensor .add): the residual is never read, the adds happen
 // in L2, and the L1 sees 8 conflict-free shared-memory stores per thread instead of 16 row-strided global accesses.
-// (Per-thread 128-byte bulk reductions were measured first: 52 -> 41 us on the wo GEMM, limited by the bulk-operation rate.)
 // EPI_MODE 3: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same tiles with a TMA store.
 // EPI_MODE 4: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 32 rows are 32 consecutive tokens of one
 // sequence and land on 32 consecutive rows of one head of q / k / v): head chunk -> tile -> one TMA store per warp and chunk.
 // EPI_MODE 5: the GEGLU epilogue (bf16 out, BN == 256): the two warps of a lane quarter take ADJACENT chunk pairs (0,1 | 2,3), so a
-// warp's 2 x 32 outputs per row are 128 contiguous bytes -> one 32-row x 128-byte tile -> one TMA store per warp and tile instead of
-// 8 row-strided 32-byte global stores per thread (which the L1 retires at 16.7 B/clk/SM, see above).
-template <int BN, bool LNF = false, bool PAIR = false, int EPI_MODE = 0>
+// warp's 2 x 32 outputs per row are 128 contiguous bytes -> one 32-row x 128-byte tile -> one TMA store per warp and tile.
+template <int BN, bool LNF = false, int EPI_MODE = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
-  using namespace sm100;
+  using namespace sm90;
   using Cfg = TcCfg<BN>;
   constexpr bool RED = EPI_MODE == 2 || EPI_MODE == 3, RED_ADD = EPI_MODE == 2;   // 3: same tiles, plain TMA store
   constexpr bool QKVT = EPI_MODE == 4;
   constexpr bool GEGLUT = EPI_MODE == 5;
+  constexpr bool TILES = EPI_MODE != 0;
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
-  static_assert(!(LNF && PAIR), "LayerNorm fusion and CTA pairs both claim the cluster");
   static_assert(!(LNF && EPI_MODE != 0), "the LayerNorm-fused kernel has no room for the epilogue tiles");
-  // QKV tile epilogue in pair mode: TWO 4 KB tiles per warp (a warp issues two TMA stores per output tile; with one tile the second chunk
-  // waited ~1 500 cycles for the first store's shared-memory read, queued behind the operand loads in the TMA unit) paid for with one ring stage
-  constexpr int EPI_BUFS = (QKVT && PAIR && BN == 256) ? 2 : 1;
-  constexpr int STAGES = PAIR ? (EPI_BUFS == 2 ? Cfg::PAIR_STAGES - 1 : Cfg::PAIR_STAGES) : Cfg::STAGES;
-  constexpr int STAGE_BYTES = PAIR ? Cfg::PAIR_STAGE_BYTES : Cfg::STAGE_BYTES;
+  constexpr int STAGES = TILES ? Cfg::STAGES_RED : Cfg::STAGES;
+  constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
+  constexpr int ROUNDS = (BN + 127) / 128;
+  // residual rows are fetched one chunk ahead (the first one during the main loop) only at BN <= 128: at BN = 256 the 128 accumulator
+  // registers leave no room for a 64-register residual buffer next to them, so each chunk loads its residual when it needs it
+  constexpr bool EARLY_RESID = BN <= 128;
 
   if (p.skip_if_zero) { pdl_wait(); if (*p.skip_if_zero == 0) return; }       // uniform over the grid: nothing has been set up yet
 
@@ -113,17 +101,14 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint8_t* tiles = smem + STAGES * STAGE_BYTES + 1024;
+  float* staging = reinterpret_cast<float*>(tiles + (TILES ? Cfg::TILE_BYTES : 0));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_pm = PAIR ? (p.num_m_tiles + 1) / 2 : p.num_m_tiles;             // PAIR: tiles are 256 rows tall, CTA `rank` owns rows [128 * rank, +128)
-  const int num_tiles = LNF ? p.num_m_tiles : num_pm * p.num_n_tiles;             // LNF: this CTA walks m-blocks, n-block = cluster rank
-  const int tile0 = (LNF || PAIR) ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = (LNF || PAIR) ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int num_tiles = LNF ? p.num_m_tiles : p.num_m_tiles * p.num_n_tiles;   // LNF: this CTA walks m-blocks, n-block = cluster rank
+  const int tile0 = LNF ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+  const int tile_step = LNF ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   const int my_rank = LNF ? (int)(blockIdx.x & 1) : 0;
-  const int pair_rank = PAIR ? (int)cluster_ctarank() : 0;
   __shared__ float s_part[LNF ? 2 : 1][2][LNF ? 128 : 1][2][2];                    // [buffer][cta rank][row][column half][sum, sumsq]
   __shared__ uint64_t s_bar_stats;
   __shared__ float s_scale[128];               // QKV epilogue: q_scale | k_scale staged once per CTA
@@ -135,56 +120,34 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&p.tma_b);
     prefetch_tmap(&p.tma_a[0]);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(tmem_full + i, 1); mbar_init(tmem_empty + i, PAIR ? 2 * TC_EPI_WARPS : TC_EPI_WARPS); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, TC_EPI_WARPS); }
     if (LNF) mbar_init(&s_bar_stats, 2 * TC_EPI_WARPS * 32);      // every epilogue thread of both CTAs arrives once per tile
     fence_barrier_init();
   }
-  if (warp == 1) { if (PAIR) tmem_alloc_pair<Cfg::TMEM_COLS>(tmem_ptr); else tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  if (LNF || PAIR) cluster_sync_all();          // the peer's barriers must exist before the first remote arrive / TMA completion
+  if (LNF) cluster_sync_all();                  // the peer's barriers must exist before the first remote arrive
   pdl_wait();                                   // everything above overlapped the previous kernel's tail
   pdl_trigger();
 
   if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && elect_one()) {
+      // ===================== TMA producer =====================
       int stage = 0; uint32_t phase = 0;
-      [[maybe_unused]] int tile_i = 0;
-      const uint32_t full0 = PAIR ? mapa_shared(smem_u32(full_bar), 0) : 0u;      // the leader's full barriers, as seen from this CTA
-      for (int tile = tile0; tile < num_tiles; tile += tile_step, ++tile_i) {
-        const int t_m = p.n_fast ? tile / p.num_n_tiles : tile % num_pm, t_n = p.n_fast ? tile % p.num_n_tiles : tile / num_pm;
-        const int m_blk = LNF ? tile : PAIR ? 2 * t_m + pair_rank : t_m;
+      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+        const int t_m = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, t_n = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
+        const int m_blk = LNF ? tile : t_m;
         const int n_blk = LNF ? my_rank : t_n;
-        [[maybe_unused]] long long w_empty = 0;
         int x0 = 0, y0 = 0, b0 = 0;
         if (p.mode == 1) {
           const int xt = m_blk % p.tiles_x, yt = (m_blk / p.tiles_x) % p.tiles_y, bt = m_blk / (p.tiles_x * p.tiles_y);
           x0 = xt * p.TW; y0 = yt * p.TH; b0 = bt * p.TB;
         }
         for (int kb = 0; kb < p.num_kb; ++kb) {
-          { [[maybe_unused]] const long long t0 = MMG_CLK(); mbar_wait(empty_bar + stage, phase ^ 1); w_empty += MMG_CLK() - t0; }
+          mbar_wait(empty_bar + stage, phase ^ 1);
           uint8_t* sa = smem + stage * STAGE_BYTES;
           uint8_t* sb = sa + Cfg::A_BYTES;
-          if (PAIR) {
-            // both CTAs' bytes complete on the leader's barrier, which alone arms it (a completion that lands before the leader
-            // armed the phase only drives the transaction count negative for a moment)
-            const uint32_t fb = full0 + (uint32_t)stage * 8u;
-            if (pair_rank == 0) mbar_expect_tx(full_bar + stage, 2 * STAGE_BYTES);
-            if (p.mode == 0) {
-              tma_load_2d_pair(sa, &p.tma_a[0], fb, kb * TC_BK, m_blk * TC_BM);
-            } else {
-              const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
-              tma_load_4d_pair(sa, &p.tma_a[p.tap_map[tap]], fb, cc * TC_BK, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], b0);
-            }
-            tma_load_2d_pair(sb, &p.tma_b, fb, kb * TC_BK, n_blk * BN + pair_rank * (BN / 2));
-          } else {
-          mbar_expect_tx(full_bar + stage, Cfg::STAGE_BYTES);
+          mbar_expect_tx(full_bar + stage, STAGE_BYTES);
           if (p.mode == 0) {
             tma_load_2d(sa, &p.tma_a[0], full_bar + stage, kb * TC_BK, m_blk * TC_BM);
           } else {
@@ -192,72 +155,31 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
             tma_load_4d(sa, &p.tma_a[p.tap_map[tap]], full_bar + stage, cc * TC_BK, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], b0);
           }
           tma_load_2d(sb, &p.tma_b, full_bar + stage, kb * TC_BK, n_blk * BN);
-          }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        MMG_TR(8, w_empty); MMG_TR(9, MMG_CLK());
       }
     }
-  } else if (warp == 1 && pair_rank == 0) {
-    // ===================== MMA issuer (PAIR: the leader CTA issues for both SMs) =====================
-    constexpr uint32_t idesc = idesc_bf16_f32(PAIR ? 2 * TC_BM : TC_BM, BN, false, false);
-    int stage = 0; uint32_t phase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
-    [[maybe_unused]] int tile_i = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step, ++tile_i) {
-      if (lane == 0) MMG_TR(0, MMG_CLK());
-      if (PAIR) mbar_wait_cluster(tmem_empty + acc, acc_phase ^ 1);    // released by the epilogue warps of BOTH CTAs
-      else mbar_wait(tmem_empty + acc, acc_phase ^ 1);
-      tc_fence_after();
-      if (lane == 0) MMG_TR(1, MMG_CLK());
-      [[maybe_unused]] long long w_full = 0;
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < p.num_kb; ++kb) {
-        { [[maybe_unused]] const long long t0 = MMG_CLK(); mbar_wait(full_bar + stage, phase); w_full += MMG_CLK() - t0; }
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint64_t adesc = smem_desc_kmajor_sw128(sa);
-          const uint64_t bdesc = smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
-          if (PAIR) {
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k)
-              umma_f16_pair(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-            umma_commit_pair(empty_bar + stage, 3);                       // the slot is free in both CTAs once these MMAs retire
-            if (kb == p.num_kb - 1) umma_commit_pair(tmem_full + acc, 3); // each CTA's epilogue reads its own half of the accumulator
-          } else {
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)
-            umma_f16(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-          umma_commit(empty_bar + stage);                         // smem slot free once these MMAs retire
-          if (kb == p.num_kb - 1) umma_commit(tmem_full + acc);   // accumulator ready for the epilogue
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (lane == 0) { MMG_TR(2, w_full); MMG_TR(3, MMG_CLK()); }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;                 // TMEM lane quarter this warp may access (warp id % 4)
-    const int half = (warp - 4) >> 2;             // 0: even 64-column chunks, 1: odd chunks
+    // ===================== consumer warpgroups: wgmma main loop, then the epilogue of their 64 rows =====================
+    const int wg = (warp - 4) >> 2, wq = warp & 3;
+    const int quarter = 2 * wg + (wq & 1);        // this warp's 32 rows of the tile, inside its warpgroup's 64
+    const int half = wq >> 1;                     // 0: even 64-column chunks, 1: odd chunks
     const int r_in_tile = quarter * 32 + lane;
+    float* stg = staging + wg * 64 * TC_STG_LD;
+    const float* my_row = stg + ((wq & 1) * 32 + lane) * TC_STG_LD;
     Epilogue epi = p.epi;
     if (epi.kind == MMG_EPI_QKV) { epi.p.q_scale = s_scale; epi.p.k_scale = s_scale + 64; }
     const bool whole_row = (epi.kind == MMG_EPI_CONVT_RGB);      // needs every chunk of a row in one thread
     const bool prefetch_resid = epi.can_prefetch_resid();
-    int acc = 0; uint32_t acc_phase = 0;
+    int stage = 0; uint32_t phase = 0;
     uint32_t stats_phase = 0; int stats_buf = 0;
-    [[maybe_unused]] int tile_i = 0;
-    [[maybe_unused]] const bool tr = (warp == 4 && lane == 0);
-    const uint32_t tmem_empty0 = PAIR ? mapa_shared(smem_u32(tmem_empty), 0) : 0u;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step, ++tile_i) {
-      const int t_m = p.n_fast ? tile / p.num_n_tiles : tile % num_pm, t_n = p.n_fast ? tile % p.num_n_tiles : tile / num_pm;
-      const int m_blk = LNF ? tile : PAIR ? 2 * t_m + pair_rank : t_m;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+      const int t_m = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, t_n = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
+      const int m_blk = LNF ? tile : t_m;
       const int n_blk = LNF ? my_rank : t_n;
       int64_t row; bool valid;
       if (p.mode == 0) {
@@ -272,24 +194,33 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
       const bool mine = !whole_row || half == 0;
       const int c_first = GEGLUT ? 2 * half : whole_row ? 0 : half, c_step = (GEGLUT || whole_row) ? 1 : 2;
       const int c_end = GEGLUT ? c_first + 2 : BN / 64;
-      const bool pre = !RED && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
+      const bool pre = EARLY_RESID && !RED && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
       float rbuf[64];
       float ln_sum = 0.f, ln_sq = 0.f;
-      if (pre) epi.load_resid(row, n_blk * BN + c_first * 64, rbuf);      // in flight while the MMA of this tile completes
+      if (pre) epi.load_resid(row, n_blk * BN + c_first * 64, rbuf);      // in flight during the main loop
       if (valid && mine) epi.begin_row(row);                               // row geometry / folded-LayerNorm statistics: independent of the accumulator
-      if (tr) MMG_TR(4, MMG_CLK());
-      mbar_wait(tmem_full + acc, acc_phase);
-      tc_fence_after();
-      if (tr) MMG_TR(5, MMG_CLK());
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
-      bool released = false;
-      auto release = [&]() {                       // hand the accumulator stage back to the MMA issuer (all of this warp's chunks are in registers)
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { if (PAIR) mbar_arrive_remote(tmem_empty0 + (uint32_t)acc * 8u); else mbar_arrive(tmem_empty + acc); }
-        if (tr) MMG_TR(6, MMG_CLK());
-        released = true;
-      };
+
+      // ---- main loop: 4 wgmma (K = 16) per k-block; a ring slot goes back to the producer once the wgmma group after it was issued ----
+      int prev_stage = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(full_bar + stage, phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+        const uint64_t adesc = smem_desc_kmajor_sw128(sa + (uint32_t)wg * 8192u);
+        const uint64_t bdesc = smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k)
+          Wgmma<BN>::template mma<0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
+
       // the epilogue of one 64-column accumulator chunk held in v
       auto chunk = [&](const int c, float (&v)[64]) {
         const int col0 = n_blk * BN + c * 64;
@@ -297,7 +228,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
           // columns past N are zero accumulators (TMA zero-fills the missing W rows) and are clipped by the tensor map, rows past M too
           float o[32];
           epi.template geglu_chunk<true>(v, o, row, col0, valid && col0 < p.N);
-          const uint32_t wtile = smem_u32(smem + STAGES * STAGE_BYTES + 1024) + (uint32_t)(warp - 4) * 4096u;
+          const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
           const int cc = c - c_first;                       // 0 / 1: left / right 64 bytes of the warp's 128-byte rows
           if (cc == 0) { if (lane == 0) bulk_wait_read0(); __syncwarp(); }     // this warp's previous store has left the tile
 #pragma unroll
@@ -313,13 +244,12 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         } else if (QKVT && col0 < p.N) {
           int h;
           const int which = epi.template qkv_chunk<true>(col0, v, h);
-          const uint32_t wtile = smem_u32(smem + STAGES * STAGE_BYTES + 1024) + (uint32_t)(warp - 4) * (4096u * EPI_BUFS) +
-                                 (EPI_BUFS == 2 ? (uint32_t)((c - c_first) / c_step) * 4096u : 0u);
+          const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
           const uint32_t rw = (uint32_t)(m_blk * TC_BM + quarter * 32), tok = (uint32_t)epi.p.tokens;
           const uint32_t bq = rw / tok, t0 = rw - bq * tok;                       // warp-uniform: the 32 rows are tokens t0 .. t0+31 of sequence bq
           const int64_t drow = which == 0 ? ((int64_t)bq * epi.p.heads + h) * epi.p.q_rows + t0
                                           : ((int64_t)bq * epi.p.heads + h) * epi.p.kv_rows + epi.p.key_off + t0;
-          if (lane == 0) { if (EPI_BUFS == 2) bulk_wait_read1(); else bulk_wait_read0(); }      // the store that last used this tile has read it
+          if (lane == 0) bulk_wait_read0();          // the store that last used this tile has read it
           __syncwarp();
 #pragma unroll
           for (int j = 0; j < 8; ++j)
@@ -333,7 +263,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         } else if (RED && col0 < p.N) {
           // rows past M hold garbage here and are clipped by the tensor map; the tile layout is the TMA 128-byte swizzle
           if (RED_ADD) epi.resid_term(col0, v);
-          const uint32_t wtile = smem_u32(smem + STAGES * STAGE_BYTES + 1024) + (uint32_t)(warp - 4) * 4096u;
+          const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (lane == 0) bulk_wait_read0();             // this warp's previous push has left the tile
@@ -352,9 +282,10 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
           }
         } else if (valid && col0 < p.N) {
           if (prefetch_resid) {
+            if (!EARLY_RESID) epi.load_resid(row, col0, rbuf);
             epi.fuse_resid(col0, v, rbuf);
             const int cn = col0 + c_step * 64;
-            if (c + c_step < BN / 64 && cn < p.N) epi.load_resid(row, cn, rbuf);   // next chunk's residual overlaps the stores
+            if (EARLY_RESID && c + c_step < BN / 64 && cn < p.N) epi.load_resid(row, cn, rbuf);   // next chunk's residual overlaps the stores
             if (LNF) {
               if (row >= epi.p.ln_split && epi.p.ln_add) {
 #pragma unroll
@@ -369,42 +300,23 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
           }
         }
       };
-      if constexpr ((QKVT || GEGLUT) && BN == 256) {
-        // two chunks per warp and an epilogue that needs no residual registers: BOTH chunks leave TMEM first (128 registers) and the stage goes
-        // back ~700 cycles after tmem_full instead of after the first chunk's arithmetic and store (QKV: 2 550 cycles, during which the MMA
-        // issuer sat waiting for the stage, scripts/trace_gemm.py)
-        if (mine) {
-          float va[64], vb[64];
-          const int ca = c_first, cb = c_first + c_step;
-          tmem_ld_32x32b_x32(t_row + ca * 64, va);
-          tmem_ld_32x32b_x32(t_row + ca * 64 + 32, va + 32);
-          tmem_ld_32x32b_x32(t_row + cb * 64, vb);
-          tmem_ld_32x32b_x32(t_row + cb * 64 + 32, vb + 32);
-          tmem_ld_wait();
-          release();
-          chunk(ca, va);
-          chunk(cb, vb);
-        }
-      } else {
+#pragma unroll
+      for (int rd = 0; rd < ROUNDS; ++rd) {
+        // columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread
+        named_sync(1 + wg, 128);                   // the previous round's (tile's) readers are done with the staging buffer
+        stage_acc<BN / 2, TC_STG_LD>(acc, stg, 128 * rd, BN - 128 * rd < 128 ? BN - 128 * rd : 128);
+        named_sync(1 + wg, 128);
 #pragma unroll 1
         for (int c = c_first; c < c_end; c += c_step) {
           if (!mine) break;
+          if ((c >> 1) != rd) continue;
           float v[64];
-          tmem_ld_32x32b_x32(t_row + c * 64, v);
-          tmem_ld_32x32b_x32(t_row + c * 64 + 32, v + 32);
-          tmem_ld_wait();
-          if (c + c_step >= c_end) release();        // last chunk is in registers: hand the accumulator stage back before the math
+          stage_ld32(my_row + (c & 1) * 64, v);
+          stage_ld32(my_row + (c & 1) * 64 + 32, v + 32);
           chunk(c, v);
         }
       }
       if (valid && mine) epi.end_row(row);
-      if (tr) MMG_TR(7, MMG_CLK());
-      if (!released) {                             // warps that own no chunk of this tile
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { if (PAIR) mbar_arrive_remote(tmem_empty0 + (uint32_t)acc * 8u); else mbar_arrive(tmem_empty + acc); }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       if (LNF) {
         // ---- LayerNorm of the freshly written row: exchange (sum, sumsq) partials with the CTA that owns the other column half ----
         const uint32_t slot = smem_u32(&s_part[stats_buf][my_rank][r_in_tile][half][0]);
@@ -440,11 +352,9 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
     }
   }
 
-  if ((RED || QKVT || GEGLUT) && warp >= 4 && lane == 0) bulk_wait0();   // every pushed tile has landed before the CTA (and its shared memory) goes away
-  tc_fence_before();
+  if (TILES && warp >= 4 && lane == 0) bulk_wait0();   // every pushed tile has landed before the CTA (and its shared memory) goes away
   __syncthreads();
-  if (LNF || PAIR) cluster_sync_all();          // no CTA may exit while its peer can still write its shared memory / read its operands
-  if (warp == 1) { tc_fence_after(); if (PAIR) tmem_dealloc_pair<Cfg::TMEM_COLS>(tmem_base); else tmem_dealloc<Cfg::TMEM_COLS>(tmem_base); }
+  if (LNF) cluster_sync_all();                  // no CTA may exit while its peer can still write its shared memory
 }
 
 }  // namespace mmg

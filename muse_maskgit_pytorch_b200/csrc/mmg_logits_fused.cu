@@ -1,12 +1,12 @@
 // mmg_logits_fused: to_logits + top-k filter + gumbel argmax + confidence of one decode step WITHOUT materialising the
 // [rows, V] fp32 logits (muse_maskgit_pytorch.py:576-609; SURVEY.md 7.5).
 //
-//   1. sample GEMM     S[r, j] = e_r . W[j * stride]      ns = min(V, 4096) evenly spaced vocabulary rows (the tcgen05 GEMM on a strided view of W)
+//   1. sample GEMM     S[r, j] = e_r . W[j * stride]      ns = min(V, 4096) evenly spaced vocabulary rows (the wgmma GEMM on a strided view of W)
 //   2. threshold       t_lo[r] = sample quantile whose expected exceedance count in the full row is k + 4 sigma (exact k-th value when ns == V)
-//   3. fused GEMM      the tcgen05 logits GEMM, 128 x 256 tiles, whose epilogue keeps per-row online-softmax partials (max, sum exp) in registers
+//   3. fused GEMM      the wgmma logits GEMM, 128 x 128 tiles, whose epilogue keeps per-row online-softmax partials (max, sum exp) in registers
 //                      and appends the candidates {x >= t_lo[r]} (12 % of the logits) to per-(row, split, chunk) lists: each epilogue thread owns
 //                      one row for a whole work item (an M-tile x a contiguous range of N-tiles), compacts its candidates through a private
-//                      shared-memory FIFO and writes them as full 32-byte sectors.  The logits themselves never leave TMEM / registers.
+//                      shared-memory FIFO and writes them as full 32-byte sectors.  The logits themselves never leave the SM.
 //   4. finish          per row: merge the partials, gather the lists (n candidates; the exact top-k is inside iff n >= k), then the same exact-rank
 //                      perturbed argmax as the materialised-logits sampler (mmg_sampler.cuh: sample_from_list) -> ids, scores.
 //   5./6. fallback     rows whose sampled threshold missed (n < k: ~3e-5 of the rows) or whose lists overflowed are redone through the
@@ -15,7 +15,7 @@
 //
 // HBM traffic per row: ~62 KB of candidates written + read instead of 2 x 256 KB of logits; the Philox / gumbel work happens on the lists only.
 #include <cuda_fp16.h>
-#include "mmg_sm100.cuh"
+#include "mmg_sm90.cuh"
 #include "mmg_tmap.cuh"
 #include "mmg_sampler.cuh"
 #include <mutex>
@@ -24,158 +24,103 @@ namespace mmg {
 
 int linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* stream);      // mmg_gemm.cu
 
-constexpr int LF_BM = 128, LF_BN = 256, LF_BK = 64;
-constexpr int LF_EPI_WARPS = 8, LF_THREADS = 128 + 32 * LF_EPI_WARPS;   // warpgroup 0: TMA / MMA; 2 epilogue warpgroups
-constexpr int LF_SEGS = 2;                  // list segments per (row, split): epilogue warpgroup h owns the 64-column chunks h and h + 2 of every tile
+constexpr int LF_BM = 128, LF_BN = 128, LF_BK = 64;
+constexpr int LF_EPI_WARPS = 8, LF_THREADS = 128 + 32 * LF_EPI_WARPS;   // warpgroup 0: TMA; 2 consumer warpgroups (wgmma + epilogue)
+constexpr int LF_SEGS = 2;                  // list segments per (row, split): warps of column half h take the 64-column chunk h of every tile
 constexpr int LF_FIFO = 32;                 // candidate entries of the per-thread shared-memory FIFO (drained 4 at a time after every 64 columns)
 constexpr int LF_FB_CAP = 128;              // rows per step that may take the materialised fallback
 constexpr int LF_MAX_SPLITS = 64;
 constexpr int LF_A_BYTES = LF_BM * LF_BK * 2, LF_B_BYTES = LF_BN * LF_BK * 2;
+constexpr int LF_STG_LD = LF_BN + 4;        // accumulator staging row stride (floats)
 
-// What bounds this kernel (ncu, 16 384 rows, profiles/r2_fused_tail.md): with the epilogue reduced to draining TMEM the CTA-pair main loop keeps
-// the tensor pipe 98.6 % busy (621 us), with the softmax statistics 98.3 % (636 us) — the operand feed is not the limit, and keeping A resident
-// in shared memory (half the L2 -> SM traffic) changed nothing.  The candidate emission is (913 us, 67 %): it is issue cost in the epilogue warps
-// (a predicated append per logit + the sector flushes; two warps per scheduler use 52 % of the issue slots), so the FIFO is deep enough to be
-// drained once per 64 columns by most lanes at once.
-template <bool PAIR> struct LfCfg {
-  static constexpr int STAGES = PAIR ? 4 : 3;
-  static constexpr int STAGE_BYTES = LF_A_BYTES + (PAIR ? LF_B_BYTES / 2 : LF_B_BYTES);
+// Shared memory: the candidate FIFOs (64 KB) and the accumulator staging (2 x 64 x 132 fp32) leave room for two 32 KB operand stages
+// within the 227 KB of a block: the tile is 128 x 128.
+struct LfCfg {
+  static constexpr int STAGE_BYTES = LF_A_BYTES + LF_B_BYTES;
   static constexpr int FIFO_BYTES = LF_EPI_WARPS * LF_FIFO * 32 * 8;
-  // [<= 1 KB to align][operand ring][barriers + padding up to the next 8 KB boundary][FIFO region, 8 KB aligned like its per-warp stride]
-  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 8192 + FIFO_BYTES;
+  static constexpr int STG_BYTES = 2 * 64 * LF_STG_LD * 4;
+  static constexpr int STAGES = 2;
+  // [<= 1 KB to align][operand ring][barriers + padding up to the next 8 KB boundary][FIFO region, 8 KB aligned like its per-warp stride][staging]
+  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 8192 + FIFO_BYTES + STG_BYTES;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
 struct alignas(64) LfParams {
   CUtensorMap tma_a, tma_b;
   int64_t R;                      // rows (sampled positions of the step)
   int num_kb, num_m_tiles, num_pm, S, npt, cap;
-  int dbg;                        // MMG_LOGITS_DBG (measurement only): 1 = epilogue without the candidate lists, 2 = epilogue only drains TMEM
+  int dbg;                        // MMG_LOGITS_DBG (measurement only): 1 = epilogue without the candidate lists, 2 = epilogue only reads the accumulators
   const float* thr;               // [R] candidate threshold per row
   float4* parts;                  // [R][S][2]: (running max, sum of exp(x - max), candidate count as int bits, overflow flag as int bits)
   uint2* lists;                   // [R][S][2][cap]: (logit bits, vocabulary index)
 };
 
-template <bool PAIR>
 __global__ void __launch_bounds__(LF_THREADS, 1)
 tc_logits_kernel(const __grid_constant__ LfParams p) {
-  using namespace sm100;
-  using Cfg = LfCfg<PAIR>;
+  using namespace sm90;
+  using Cfg = LfCfg;
   constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   // FIFO region: aligned (in the shared-memory window) to its 8 KB per-warp stride, so that a thread's slot address is base | slot << 8
   uint8_t* fifo_all = smem + STAGES * STAGE_BYTES + 256;
   fifo_all += (8192u - (smem_u32(fifo_all) & 8191u)) & 8191u;
+  float* staging = reinterpret_cast<float*>(fifo_all + Cfg::FIFO_BYTES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_items = p.num_pm * p.S;
-  const int unit0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int unit_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int pair_rank = PAIR ? (int)cluster_ctarank() : 0;
+  const int unit0 = (int)blockIdx.x, unit_step = (int)gridDim.x;
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&p.tma_a); prefetch_tmap(&p.tma_b);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(tmem_full + i, 1); mbar_init(tmem_empty + i, PAIR ? 2 * LF_EPI_WARPS : LF_EPI_WARPS); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, LF_EPI_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) { if (PAIR) tmem_alloc_pair<512>(tmem_ptr); else tmem_alloc<512>(tmem_ptr); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  if (PAIR) cluster_sync_all();
   pdl_wait();
   pdl_trigger();
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (warp == 0) {
+    if (warp == 0 && elect_one()) {
       // ===================== TMA producer =====================
-      if (elect_one()) {
-        int stage = 0; uint32_t phase = 0;
-        const uint32_t full0 = PAIR ? mapa_shared(smem_u32(full_bar), 0) : 0u;
-        for (int item = unit0; item < num_items; item += unit_step) {
-          const int pm = item % p.num_pm, sp = item / p.num_pm;
-          const int m_blk = PAIR ? 2 * pm + pair_rank : pm;
-          for (int j = 0; j < p.npt; ++j) {
-            const int n_blk = sp * p.npt + j;
-            for (int kb = 0; kb < p.num_kb; ++kb) {
-              mbar_wait(empty_bar + stage, phase ^ 1);
-              uint8_t* sa = smem + stage * STAGE_BYTES;
-              uint8_t* sb = sa + LF_A_BYTES;
-              if (PAIR) {
-                const uint32_t fb = full0 + (uint32_t)stage * 8u;
-                if (pair_rank == 0) mbar_expect_tx(full_bar + stage, 2 * STAGE_BYTES);
-                tma_load_2d_pair(sa, &p.tma_a, fb, kb * LF_BK, m_blk * LF_BM);
-                tma_load_2d_pair(sb, &p.tma_b, fb, kb * LF_BK, n_blk * LF_BN + pair_rank * (LF_BN / 2));
-              } else {
-                mbar_expect_tx(full_bar + stage, STAGE_BYTES);
-                tma_load_2d(sa, &p.tma_a, full_bar + stage, kb * LF_BK, m_blk * LF_BM);
-                tma_load_2d(sb, &p.tma_b, full_bar + stage, kb * LF_BK, n_blk * LF_BN);
-              }
-              if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
-    } else if (warp == 1 && pair_rank == 0) {
-      // ===================== MMA issuer (PAIR: the leader CTA issues for both SMs) =====================
-      constexpr uint32_t idesc = idesc_bf16_f32(PAIR ? 2 * LF_BM : LF_BM, LF_BN, false, false);
       int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
       for (int item = unit0; item < num_items; item += unit_step) {
+        const int m_blk = item % p.num_pm, sp = item / p.num_pm;
         for (int j = 0; j < p.npt; ++j) {
-          if (PAIR) mbar_wait_cluster(tmem_empty + acc, acc_phase ^ 1); else mbar_wait(tmem_empty + acc, acc_phase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * LF_BN;
+          const int n_blk = sp * p.npt + j;
           for (int kb = 0; kb < p.num_kb; ++kb) {
-            mbar_wait(full_bar + stage, phase);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-              const uint64_t adesc = smem_desc_kmajor_sw128(sa);
-              const uint64_t bdesc = smem_desc_kmajor_sw128(sa + LF_A_BYTES);
-              if (PAIR) {
-#pragma unroll
-                for (int k = 0; k < LF_BK / 16; ++k)
-                  umma_f16_pair(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-                umma_commit_pair(empty_bar + stage, 3);
-                if (kb == p.num_kb - 1) umma_commit_pair(tmem_full + acc, 3);
-              } else {
-#pragma unroll
-                for (int k = 0; k < LF_BK / 16; ++k)
-                  umma_f16(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-                umma_commit(empty_bar + stage);
-                if (kb == p.num_kb - 1) umma_commit(tmem_full + acc);
-              }
-            }
-            __syncwarp();
+            mbar_wait(empty_bar + stage, phase ^ 1);
+            uint8_t* sa = smem + stage * STAGE_BYTES;
+            uint8_t* sb = sa + LF_A_BYTES;
+            mbar_expect_tx(full_bar + stage, STAGE_BYTES);
+            tma_load_2d(sa, &p.tma_a, full_bar + stage, kb * LF_BK, m_blk * LF_BM);
+            tma_load_2d(sb, &p.tma_b, full_bar + stage, kb * LF_BK, n_blk * LF_BN);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
       }
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    // ===================== epilogue warps: one thread = one row of the work item x every other 64-column chunk =====================
+    // ===================== consumer warpgroups: wgmma on 64 rows each, then one thread = one row x one 64-column chunk per tile =====================
     constexpr float LOG2E = 1.4426950408889634f;
-    const int quarter = warp & 3;                 // TMEM lane quarter this warp may access (warp id % 4)
-    const int half = (warp - 4) >> 2;             // 0: 64-column chunks 0 and 2 of a tile, 1: chunks 1 and 3
+    const int wg = (warp - 4) >> 2, wq = warp & 3;
+    const int quarter = 2 * wg + (wq & 1);        // this warp's 32 rows of the tile, inside its warpgroup's 64
+    const int half = wq >> 1;                     // the 64-column chunk of every tile this warp takes
     const int r_in_tile = quarter * 32 + lane;
+    float* stg = staging + wg * 64 * LF_STG_LD;
+    const float* my_row = stg + ((wq & 1) * 32 + lane) * LF_STG_LD + half * 64;
     // FIFO slot s of this thread lives at fifo | s << 8 (the warp's 8 KB region is 8 KB aligned, a slot row is 32 lanes x 8 bytes)
     const uint32_t fifo = smem_u32(fifo_all) + (uint32_t)(warp - 4) * (LF_FIFO * 256) + (uint32_t)lane * 8u;
-    const uint32_t tmem_empty0 = PAIR ? mapa_shared(smem_u32(tmem_empty), 0) : 0u;
-    int acc = 0; uint32_t acc_phase = 0;
+    int stage = 0; uint32_t phase = 0;
+    float acc[LF_BN / 2];
+#pragma unroll
+    for (int i = 0; i < LF_BN / 2; ++i) acc[i] = 0.f;
     for (int item = unit0; item < num_items; item += unit_step) {
-      const int pm = item % p.num_pm, sp = item / p.num_pm;
-      const int m_blk = PAIR ? 2 * pm + pair_rank : pm;
+      const int m_blk = item % p.num_pm, sp = item / p.num_pm;
       const int64_t row = (int64_t)m_blk * LF_BM + r_in_tile;
       const bool valid = row < p.R;
       const float tlo = valid ? __ldg(p.thr + row) : FLT_MAX;            // rows past R never produce a candidate
@@ -185,21 +130,34 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
       int flushed = 0, ovf = 0;
       for (int j = 0; j < p.npt; ++j) {
         const int n_blk = sp * p.npt + j;
-        mbar_wait(tmem_full + acc, acc_phase);
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * LF_BN;
-#pragma unroll 1
-        for (int c = half; c < LF_BN / 64; c += 2) {
+        int prev_stage = -1;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(full_bar + stage, phase);
+          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+          const uint64_t adesc = smem_desc_kmajor_sw128(sa + (uint32_t)wg * 8192u);
+          const uint64_t bdesc = smem_desc_kmajor_sw128(sa + LF_A_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < LF_BK / 16; ++k)
+            Wgmma<LF_BN>::template mma<0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
+          prev_stage = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
+        named_sync(1 + wg, 128);                   // the previous tile's readers are done with the staging buffer
+        stage_acc<LF_BN / 2, LF_STG_LD>(acc, stg, 0, LF_BN);
+        named_sync(1 + wg, 128);
+        {
+          const int c = half;
           float v[64];
-          tmem_ld_32x32b_x32(t_row + c * 64, v);
-          tmem_ld_32x32b_x32(t_row + c * 64 + 32, v + 32);
-          tmem_ld_wait();
-          if (c + 2 >= LF_BN / 64) {               // last chunk is in registers: hand the accumulator stage back before the math
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (PAIR) mbar_arrive_remote(tmem_empty0 + (uint32_t)acc * 8u); else mbar_arrive(tmem_empty + acc); }
-          }
-          if (p.dbg == 2) { if (v[0] == 123.456f) m_run = v[5]; continue; }
+          stage_ld32(my_row, v);
+          stage_ld32(my_row + 32, v + 32);
+          if (p.dbg == 2) { if (v[0] == 123.456f) m_run = v[5]; goto next_tile; }
           // ---- online softmax statistics of the row ----
           float lm = fmaxf(v[0], v[1]);
 #pragma unroll
@@ -210,7 +168,7 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
 #pragma unroll
           for (int i = 0; i < 64; i += 2) { s0 += ex2_approx(fmaf(v[i], LOG2E, -mb)); s1 += ex2_approx(fmaf(v[i + 1], LOG2E, -mb)); }
           s_run += s0 + s1;
-          if (p.dbg == 1) continue;
+          if (p.dbg == 1) goto next_tile;
           // ---- candidates >= t_lo -> private FIFO (predicated, no branch) ----
           const uint32_t col0 = (uint32_t)(n_blk * LF_BN + c * 64);
           const uint32_t pos8_before = pos8;
@@ -239,7 +197,7 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
             flushed += 4;
           }
         }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      next_tile:;
       }
       // ---- end of the work item: the last (< 4) entries as one padded sector, then the partial record ----
       const int pos = (int)(pos8 >> 8);
@@ -264,10 +222,7 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();
-  if (warp == 1) { tc_fence_after(); if (PAIR) tmem_dealloc_pair<512>(tmem_base); else tmem_dealloc<512>(tmem_base); }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -525,16 +480,15 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
 // ---------------------------------------------------------------------------------------------------------------------------
 static inline uint64_t up256(uint64_t x) { return (x + 255) & ~uint64_t(255); }
 
-struct LfPlan { int pair, num_m_tiles, num_pm, S, npt, cap, ns, stride; };
+struct LfPlan { int num_m_tiles, num_pm, S, npt, cap, ns, stride; };
 
 // Splits of the N range: the static schedule hands item i to unit i % units; pick the smallest power-of-two S (npt = NT / S >= 2 tiles per
 // item) whose makespan ceil(items / units) * npt is within 4 % of the best one.
 static LfPlan lf_plan(int64_t R, int V, int k) {
   LfPlan pl{};
   pl.num_m_tiles = (int)((R + LF_BM - 1) / LF_BM);
-  pl.pair = pl.num_m_tiles >= 2;
-  pl.num_pm = pl.pair ? (pl.num_m_tiles + 1) / 2 : pl.num_m_tiles;
-  const int units = pl.pair ? num_sms() / 2 : num_sms();
+  pl.num_pm = pl.num_m_tiles;
+  const int units = num_sms();
   const int NT = V / LF_BN;
   long best = -1;
   auto span_of = [&](int s) { const long items = (long)pl.num_pm * s; return ((items + units - 1) / units) * (long)(NT / s); };
@@ -555,7 +509,7 @@ static LfPlan lf_plan(int64_t R, int V, int k) {
   // segments, plus 6 binomial sigmas, as whole 32-byte sectors
   const double per = (double)SMP_CAP / ((double)LF_SEGS * pl.S);
   int cap = (int)(per + 6.0 * sqrt(per) + 8.0);
-  if (cap > 128 * pl.npt) cap = 128 * pl.npt;                  // a segment cannot hold more than the columns it sees (128 per tile)
+  if (cap > 64 * pl.npt) cap = 64 * pl.npt;                    // a segment cannot hold more than the columns it sees (64 per tile)
   pl.cap = (cap + 3) / 4 * 4;
   (void)k;
   return pl;
@@ -597,37 +551,15 @@ static bool lf_supported(int V, int K, int k) {
   return n_exp + 4.0 * sd <= SMP_CAP;
 }
 
-template <bool PAIR>
 static int launch_lf(const LfParams& p, cudaStream_t st) {
-  constexpr int SMEM = LfCfg<PAIR>::SMEM_BYTES;
+  constexpr int SMEM = LfCfg::SMEM_BYTES;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  static int max_units = 0;
-  std::call_once(once, [] {
-    attr_err = cudaFuncSetAttribute(tc_logits_kernel<PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (attr_err != cudaSuccess) return;
-    if (PAIR) {
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3(2 * (num_sms() / 2)); cfg.blockDim = dim3(LF_THREADS); cfg.dynamicSmemBytes = SMEM;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr; cfg.numAttrs = 1;
-      attr_err = cudaOccupancyMaxActiveClusters(&max_units, tc_logits_kernel<PAIR>, &cfg);
-    } else {
-      max_units = num_sms();
-    }
-  });
-  if (attr_err != cudaSuccess || max_units < 1) return fail(MMG_ECUDA, "tc_logits<%d> setup: %s (units %d)", (int)PAIR, cudaGetErrorString(attr_err), max_units);
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_logits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); });
+  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "tc_logits setup: %s", cudaGetErrorString(attr_err));
   const int items = p.num_pm * p.S;
-  const int units = items < max_units ? items : max_units;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(PAIR ? 2 * units : units); cfg.blockDim = dim3(LF_THREADS); cfg.dynamicSmemBytes = SMEM; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (PAIR) { attr[na].id = cudaLaunchAttributeClusterDimension; attr[na].val.clusterDim.x = 2; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1; ++na; }
-  if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  MMG_CUDA(cudaLaunchKernelEx(&cfg, tc_logits_kernel<PAIR>, p));
+  const int units = items < num_sms() ? items : num_sms();
+  MMG_CUDA(launch_pdl(tc_logits_kernel, dim3(units), dim3(LF_THREADS), SMEM, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -685,9 +617,9 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
     { const char* e = getenv("MMG_LOGITS_DBG"); p.dbg = e ? atoi(e) : 0; }
     uint64_t da[2] = {(uint64_t)a->K, (uint64_t)R}; uint64_t sa[1] = {(uint64_t)a->K * 2}; uint32_t ba[2] = {LF_BK, LF_BM};
     if ((rc = make_tmap_bf16(&p.tma_a, a->e, 2, da, sa, ba))) return rc;
-    uint64_t db[2] = {(uint64_t)a->K, (uint64_t)s.V}; uint64_t sb[1] = {(uint64_t)a->K * 2}; uint32_t bb[2] = {LF_BK, (uint32_t)(pl.pair ? LF_BN / 2 : LF_BN)};
+    uint64_t db[2] = {(uint64_t)a->K, (uint64_t)s.V}; uint64_t sb[1] = {(uint64_t)a->K * 2}; uint32_t bb[2] = {LF_BK, (uint32_t)LF_BN};
     if ((rc = make_tmap_bf16(&p.tma_b, a->w, 2, db, sb, bb))) return rc;
-    if ((rc = pl.pair ? launch_lf<true>(p, st) : launch_lf<false>(p, st))) return rc;
+    if ((rc = launch_lf(p, st))) return rc;
   }
   float t = s.temperature; if (t < 1e-10f) t = 1e-10f;      // max(temperature, 1e-10): muse_maskgit_pytorch.py:411
   {   // 4. finish

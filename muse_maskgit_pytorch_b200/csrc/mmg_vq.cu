@@ -5,7 +5,7 @@
 namespace mmg {
 
 // LFQ encode: the nearest code of the implicit {+-1}^bits codebook is the sign pattern of the projected token.
-// CUDA-core path (fp32 "parity" precision; bf16 inputs normally take the tcgen05 route below).  The projection [bits, D] sits in
+// CUDA-core path (fp32 "parity" precision; bf16 inputs normally take the wgmma route below).  The projection [bits, D] sits in
 // shared memory; a warp owns LFQ_TOK tokens at a time and a lane 4 channels of each (one 128-bit / 64-bit load per token), so one
 // 128-bit shared-memory read of a weight quad feeds 4 x LFQ_TOK FMAs (0.06 shared reads per FMA instead of 1) and the token
 // stream is fully coalesced.  Warp-shuffle reduction, then bit-pack (MSB first; x == 0 -> bit 0).
@@ -238,7 +238,7 @@ extern "C" int mmg_vq_lfq_encode(const mmg_vq_lfq_encode_args* a, void* stream) 
   MMG_CHECK_ARG(a->w_in || a->D == a->bits, "mmg_vq_lfq_encode: identity projection needs D == bits");
   if (a->T == 0) return MMG_OK;
   if (a->dtype == MMG_BF16 && a->w_split && a->D % 64 == 0 && 3 * a->bits <= 64) {
-    // bf16 tokens: the projection runs on tcgen05 as ONE HBM-bound TMA stream of the tokens against the 3-way bf16 split of project_in
+    // bf16 tokens: the projection runs on wgmma as ONE HBM-bound TMA stream of the tokens against the 3-way bf16 split of project_in
     // ([hi | mid | lo] rows, hi + mid + lo == the fp32 weight), recombined in fp32 by the LFQ_IDS epilogue
     mmg_linear_args l{};
     l.a = a->x; l.w = a->w_split; l.M = a->T; l.N = 64; l.K = a->D; l.lda = a->D; l.ldw = a->D; l.dtype = MMG_BF16; l.epilogue = MMG_EPI_LFQ_IDS;

@@ -2,8 +2,8 @@
 (ref: muse_maskgit_pytorch.py:199-386, 427-791) over libmmg.so.
 
 The nn.Modules here only HOLD parameters under the reference's state_dict keys (SURVEY.md 8b); the arithmetic of
-`forward`, `forward_with_cond_scale` and `MaskGit.generate` is issued as sm_100a kernels through the C-ABI:
-  tcgen05 GEMMs with fused epilogues (QKV split + l2norm/scale, residual, GEGLU), tcgen05 attention, LayerNorm,
+`forward`, `forward_with_cond_scale` and `MaskGit.generate` is issued as sm_90a kernels through the C-ABI:
+  wgmma GEMMs with fused epilogues (QKV split + l2norm/scale, residual, GEGLU), wgmma attention, LayerNorm,
   the masked-row final-LN + CFG combine, the logits GEMM on masked rows only, and the fused sampling tail.
 Both CFG branches of a decode step run as one batch of 2B sequences; the null branch's cross-attention is the
 constant to_out(null_v) (every text key masked -> softmax puts weight exactly 1 on the null key, SURVEY.md 8a T3).
@@ -59,7 +59,7 @@ class Attention(nn.Module):
 class TransformerBlocks(nn.Module):
     def __init__(self, *, dim, depth, dim_head=64, heads=8, ff_mult=4, flash=True):
         super().__init__()
-        assert dim_head == 64, ("dim_head must be 64 here: the tcgen05 attention kernel (S and O tiles in TMEM, one 128-byte swizzled row per head "
+        assert dim_head == 64, ("dim_head must be 64 here: the wgmma attention kernel (one 128-byte swizzled row per head "
                                 "vector) and the QKV epilogue are specialised for the head size every Muse config uses; the reference accepts "
                                 "any value (muse_maskgit_pytorch.py:95-110, 164-172)")
         self.dim, self.depth, self.heads, self.dim_head, self.ff_mult = dim, depth, heads, dim_head, ff_mult

@@ -30,7 +30,7 @@ def _epi(out=None, ldo=0, bias=None, act=0, resid=None, ldr=0, row_stats=None, l
 
 
 # ---- fp32 on the tensor cores ---------------------------------------------------------------------------------------------
-# precision="fp32" (the token-identical parity mode) runs its matrix products and convolutions on the SAME tcgen05 kernels as the bf16 path:
+# precision="fp32" (the token-identical parity mode) runs its matrix products and convolutions on the SAME wgmma kernels as the bf16 path:
 # both operands are split into three bf16 terms (mmg_split3) and one bf16 product over 6K columns accumulates the six significant cross
 # terms in fp32.  Shapes the TMA path cannot take (K or N not a multiple of 64) stay on the CUDA-core kernel.  MMG_FP32_TC=0 / fp32_tc(False)
 # forces the CUDA-core kernel everywhere (the round-1 behaviour).
@@ -71,11 +71,11 @@ def _split_weight(w, rows, K):
 
 def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, N=None, epi=None, row_stats=None, ln_width=0,
            ln_out=None, ln_gamma=None, ln_gamma_b=None, ln_add=None, ln_split=None):
-    """out = a @ w.T (+ epilogue).  a [M, K], w [N, K] same dtype (bf16 -> tcgen05, fp32 -> CUDA cores)."""
+    """out = a @ w.T (+ epilogue).  a [M, K], w [N, K] same dtype (bf16 -> wgmma, fp32 -> CUDA cores)."""
     _chk(a, "a"); _chk(w, "w")
     assert w.shape[1] == a.shape[1] and a.dtype == w.dtype
     if a.dtype == torch.float32 and _FP32_TC[0] and a.shape[1] % 64 == 0 and (w.shape[0] if N is None else N) % 64 == 0 and a.shape[0] > 0:
-        a, w = split3(a, 0), _split_weight(w, w.shape[0], w.shape[1])          # same product, 6K bf16 columns, fp32 accumulation in TMEM
+        a, w = split3(a, 0), _split_weight(w, w.shape[0], w.shape[1])          # same product, 6K bf16 columns, fp32 accumulation on the tensor cores
     args = L.LinearArgs()
     args.a = a.data_ptr(); args.w = w.data_ptr()
     args.M = a.shape[0] if M is None else M
@@ -284,7 +284,7 @@ def ff_geglu(x, ln_gamma, w1, w2f, cvec, F, xn, h, stats, add=None, add_from=0):
 
 
 def vq_lfq_encode(x, w_in, b_in, ids, bits, w_split=None):
-    """w_split: [64, D] bf16 3-way split of w_in -> bf16 tokens take the tcgen05 route (one TMA stream over the tokens)."""
+    """w_split: [64, D] bf16 3-way split of w_in -> bf16 tokens take the wgmma route (one TMA stream over the tokens)."""
     a = L.LfqEncodeArgs()
     a.x = _chk(x).data_ptr(); a.dtype = L.dt(x); a.w_in = L.ptr(w_in); a.b_in = L.ptr(b_in); a.ids = ids.data_ptr()
     a.w_split = L.ptr(w_split)

@@ -2,8 +2,8 @@
 
 Same constructor keywords, attribute names, state_dict keys and method signatures as the reference for the inference
 surface (encode / decode / decode_from_ids / forward without losses / get_encoded_fmap_size / copy_for_eval / save / load).
-The modules below only HOLD parameters under the reference's key names; all arithmetic happens in the sm_100a kernels:
-convolutions are implicit GEMMs over NHWC activations (tcgen05 + TMA in bf16 precision), the quantizer is the LFQ sign
+The modules below only HOLD parameters under the reference's key names; all arithmetic happens in the sm_90a kernels:
+convolutions are implicit GEMMs over NHWC activations (wgmma + TMA in bf16 precision), the quantizer is the LFQ sign
 scan / explicit L2 argmin scan.  Training losses (GAN, VGG; vqgan_vae.py:350-385, 465-534) are out of scope.
 """
 import copy
@@ -242,7 +242,7 @@ class VQGanVAE(nn.Module):
             P["pin_w3"] = None
             if lin and adt == torch.bfloat16 and 3 * q.bits <= 64 and self.enc_dec.encoded_dim % 64 == 0:
                 # project_in split into three bf16 terms (hi + mid + lo reproduces the fp32 weight to 24 bits) stacked as the 64 rows of
-                # one tcgen05 GEMM; the LFQ_IDS epilogue recombines them, adds the bias, takes signs and packs the id
+                # one wgmma GEMM; the LFQ_IDS epilogue recombines them, adds the bias, takes signs and packs the id
                 w = P["pin_w"]
                 hi = w.to(adt); r1 = w - hi.float(); mid = r1.to(adt); lo = (r1 - mid.float()).to(adt)
                 w3 = torch.zeros((64, w.shape[1]), device=dev, dtype=adt)
@@ -333,7 +333,7 @@ class VQGanVAE(nn.Module):
         P = self._packed()
         ids = torch.empty((x.shape[0],), device=x.device, dtype=torch.int64)
         if self.lookup_free_quantization:
-            # bf16 fmap + split projection: tcgen05 route inside mmg_vq_lfq_encode (HBM-bound TMA stream of the fmap); else CUDA cores
+            # bf16 fmap + split projection: wgmma route inside mmg_vq_lfq_encode (HBM-bound TMA stream of the fmap); else CUDA cores
             ops.vq_lfq_encode(x, P["pin_w"], P["pin_b"], ids, self.quantizer.bits, w_split=P["pin_w3"] if x.dtype == torch.bfloat16 else None)
         else:
             ids.fill_(-1)                                   # all-ones keys for the packed (distance, code) atomicMin
@@ -391,7 +391,7 @@ class VQGanVAE(nn.Module):
             assert size % self.dim_divisor == 0, f"{name} must be divisible by {self.dim_divisor}"
         assert C == self.channels, "number of channels on image or sketch is not equal to the channels set on this VQGanVAE"
         if return_loss or return_discr_loss:
-            raise NotImplementedError("VQGanVAE training losses are outside the scope of the B200 inference path")
+            raise NotImplementedError("VQGanVAE training losses are outside the scope of this inference path")
         x, h, w = self._encode_nhwc(img)
         ids = self._quantize_nhwc(x)
         return self._decode_nhwc(self._codes_nhwc(ids), B, h, w)

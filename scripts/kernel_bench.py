@@ -152,7 +152,7 @@ if want("vq"):
     report("vq_lfq_encode T=16384 D=2048 bits=16 (bf16 fmap)", timeit(lambda: ops.vq_lfq_encode(x, w, bb, ids, bits)), bytes_=T * (D * 2 + 8))
     hi = w.to(bf); r1 = w - hi.float(); mid = r1.to(bf); lo = (r1 - mid.float()).to(bf)
     w3 = torch.zeros((64, D), device="cuda", dtype=bf); w3[:16], w3[16:32], w3[32:48] = hi, mid, lo
-    report("vq LFQ via tcgen05 GEMM + LFQ_IDS epilogue (bf16 fmap)", timeit(lambda: ops.linear(x, w3, ids, epilogue=ops.EPI_LFQ_IDS, bias=bb, ln_width=bits)), bytes_=T * (D * 2 + 8))
+    report("vq LFQ via wgmma GEMM + LFQ_IDS epilogue (bf16 fmap)", timeit(lambda: ops.linear(x, w3, ids, epilogue=ops.EPI_LFQ_IDS, bias=bb, ln_width=bits)), bytes_=T * (D * 2 + 8))
     xf = x.float(); report("vq_lfq_encode T=16384 D=2048 bits=16 (fp32 fmap)", timeit(lambda: ops.vq_lfq_encode(xf, w, bb, ids, bits)), bytes_=T * (D * 4 + 8))
     T2, K2, D2 = 256, 8192, 256
     x2 = torch.randn((T2, D2), device="cuda"); cb = torch.randn((K2, D2), device="cuda"); ids2 = torch.empty((T2,), device="cuda", dtype=torch.long)

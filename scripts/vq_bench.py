@@ -1,4 +1,4 @@
-"""VQ codebook lookup (LFQ, bf16 tokens, tcgen05 route) at the C5 per-GPU size and 8x that: the bench.py `hbm_kernels` measurement alone.
+"""VQ codebook lookup (LFQ, bf16 tokens, wgmma route) at the C5 per-GPU size and 8x that: the bench.py `hbm_kernels` measurement alone.
 usage: python scripts/vq_bench.py        (MMG_PDL=1 to overlap consecutive launches' prologues)"""
 import json, os, sys
 import torch

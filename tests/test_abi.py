@@ -1,4 +1,4 @@
-"""CPU: libmmg.so builds for sm_100a, loads without a GPU/driver, exports every symbol include/mmg.h declares, and the
+"""CPU: libmmg.so builds for sm_90a, loads without a GPU/driver, exports every symbol include/mmg.h declares, and the
 ctypes mirror of every argument block has the C struct's size.  No compute calls here."""
 import ctypes
 import os
@@ -69,13 +69,15 @@ def test_decode_step_workspace_query_is_host_only():
 
 
 def test_baseline_ref_is_the_unmodified_reference():
-    """baseline/_ref (the reference arm of bench.py) is byte-identical to /root/reference wherever both exist (build container)."""
+    """oracle/_ref (the reference arm of bench.py) is byte-identical to the reference checkout wherever both exist."""
     import filecmp
     import pytest
-    ref = "/root/reference/muse_maskgit_pytorch"
-    inst = os.path.join(ROOT, "baseline", "_ref", "muse_maskgit_pytorch")
-    if not (os.path.isdir(ref) and os.path.isdir(inst)):
-        pytest.skip("needs /root/reference and baseline/_ref")
+    from oracle import reference_install as RI
+    src = RI.source_dir()
+    inst = os.path.join(RI.DEST, RI.PACKAGE)
+    if src is None or not RI.installed():
+        pytest.skip("needs the reference checkout and oracle/_ref")
+    ref = os.path.join(src, RI.PACKAGE)
     names = sorted(f for f in os.listdir(ref) if f.endswith(".py"))
     assert names and names == sorted(f for f in os.listdir(inst) if f.endswith(".py"))
     match, mismatch, errors = filecmp.cmpfiles(ref, inst, names, shallow=False)

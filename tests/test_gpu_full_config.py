@@ -1,4 +1,4 @@
-"""GPU parity tests ON THE BENCHMARKED PATH at the BASELINE configs (bf16 / tcgen05, the kernels bench.py times):
+"""GPU parity tests ON THE BENCHMARKED PATH at the BASELINE configs (bf16 / wgmma, the kernels bench.py times):
 
   C2  MaskGitTransformer dim 512, depth 8, seq 256, V = 65536: full forward with CFG vs the fp32 CPU oracle;
   C3  MaskGit.generate() decode steps, teacher forced with the oracle's ids and noise, at the full model config: sampled-token flip rate;
@@ -157,8 +157,8 @@ def test_c3_teacher_forced_flip_rate_full_config():
 
 
 def test_c3_teacher_forced_token_identical_fp32_on_tensor_cores():
-    """precision='fp32' at the SAME full C3 config, on the SAME tcgen05 GEMM / attention kernels (operands as 3-way bf16 splits, six cross terms
-    per product, fp32 accumulation in TMEM; no CUDA-core GEMM or attention launch): every one of the 5 782 sampled tokens of the 18 teacher-forced
+    """precision='fp32' at the SAME full C3 config, on the SAME wgmma GEMM / attention kernels (operands as 3-way bf16 splits, six cross terms
+    per product, fp32 accumulation; no CUDA-core GEMM or attention launch): every one of the 5 782 sampled tokens of the 18 teacher-forced
     steps equals the fp32 oracle's token.  (A token could still differ where the oracle's own top-2 margin is below fp32 summation noise.)"""
     from muse_maskgit_pytorch_b200 import _lib
     bf_tr, _ = base_transformer()
@@ -169,7 +169,7 @@ def test_c3_teacher_forced_token_identical_fp32_on_tensor_cores():
     assert ops().fp32_tc()
     fb0 = _lib.simt_launch_count()
     flips, total, per_step, worst_score = _c3_teacher_forced(tr)
-    print(f"C3 full-config teacher-forced, fp32 on tcgen05 (3-way bf16 split): {flips}/{total} tokens differ (per step {per_step}); "
+    print(f"C3 full-config teacher-forced, fp32 on wgmma (3-way bf16 split): {flips}/{total} tokens differ (per step {per_step}); "
           f"max |score diff| {worst_score:.2e}; CUDA-core GEMM / attention launches {_lib.simt_launch_count() - fb0}")
     assert flips <= 1 and worst_score < 5e-5
     assert _lib.simt_launch_count() == fb0
@@ -246,8 +246,8 @@ def _fp32_reference_math():
 
 @pytest.mark.parametrize("q_only", [False, True], ids=["self_qkv_32768x1536x512", "cross_q_16384x512x512"])
 def test_gemm_generate_shape_qkv(q_only):
-    """tc_gemm_kernel<256,0,0,4> / <128,...>: the self-attention QKV product of a batch-64 CFG step (128 sequences x 256 tokens) and
-    the cross-attention q product of its 64 conditional sequences."""
+    """The QKV tile epilogue: the self-attention QKV product of a batch-64 CFG step (128 sequences x 256 tokens; tc_gemm_kernel<256, false, 4>)
+    and the cross-attention q product of its 64 conditional sequences (tc_gemm_kernel<128, false, 4>)."""
     o = ops()
     b, n, heads, dim = (64 if q_only else 128), 256, 8, 512
     inner, nsec = heads * 64, (1 if q_only else 3)
@@ -274,8 +274,8 @@ def test_gemm_generate_shape_qkv(q_only):
 
 
 def test_gemm_generate_shape_ff_geglu_lnfold():
-    """FF1 32768 x 2816 x 512 with the GEGLU epilogue + row statistics (tc_gemm_kernel<256,0,0,0>) and FF2 32768 x 512 x 1408 as CTA
-    pairs with the LayerNorm fold and the in-place TMA reduction (tc_gemm_kernel<256,0,1,2>), i.e. x += LN(gate * gelu(a Wx)) W2^T."""
+    """FF1 32768 x 2816 x 512 with the GEGLU tile epilogue + row statistics (tc_gemm_kernel<256, false, 5>) and FF2 32768 x 512 x 1408 with
+    the LayerNorm fold and the in-place TMA reduction (tc_gemm_kernel<256, false, 2>), i.e. x += LN(gate * gelu(a Wx)) W2^T."""
     o = ops()
     M_, K, Fu, Fp, dim = 32768, 512, 1365, 1408, 512
     a = grand((M_, K), 11)
@@ -309,7 +309,7 @@ def test_gemm_generate_shape_ff_geglu_lnfold():
 
 @pytest.mark.parametrize("M_", [32768, 16384 + 128 * 3], ids=["32768", "16768"])
 def test_gemm_generate_shape_wo_residual(M_):
-    """attention to_out: x += a Wo^T, 32768 x 512 x 512, in place through the TMA reduction (tc_gemm_kernel<.,0,0,2>)."""
+    """attention to_out: x += a Wo^T, 32768 x 512 x 512, in place through the TMA reduction (tc_gemm_kernel<256, false, 2>)."""
     o = ops()
     a, w = grand((M_, 512), 21), grand((512, 512), 22, 512 ** -0.5)
     x = grand((M_, 512), 23, dtype=torch.float32)
@@ -321,7 +321,7 @@ def test_gemm_generate_shape_wo_residual(M_):
 
 @pytest.mark.parametrize("rows", [64 * 229, 64 * 47 + 5], ids=["14656", "3013_ragged"])
 def test_gemm_generate_shape_logits(rows):
-    """to_logits on the masked rows of a step: rows x 65536 x 512, fp32 out, CTA pairs + TMA-store tiles (tc_gemm_kernel<256,0,1,3>)."""
+    """to_logits on the masked rows of a step: rows x 65536 x 512, fp32 out through the TMA-store tiles (tc_gemm_kernel<256, false, 3>)."""
     o = ops()
     a, w = grand((rows, 512), 31), grand((65536, 512), 32, 512 ** -0.5)
     out = torch.empty((rows + 3, 65536), device="cuda")
@@ -340,8 +340,9 @@ def _nhwc(t):
     return t.permute(0, 2, 3, 1).contiguous()
 
 
-def test_gemm_generate_shape_conv3x3_glu_pair():
-    """VAE decoder GLU res-block conv: 3x3, 2048 -> 4096 on 16 x 16 maps, batch 64, K = 18432 (CTA-pair implicit GEMM, tc_gemm_kernel<256,0,1,0>)."""
+def test_gemm_generate_shape_conv3x3_glu():
+    """VAE decoder GLU res-block conv: 3x3, 2048 -> 4096 on 16 x 16 maps, batch 64, K = 18432: implicit GEMM (4-D tensor-map A operand)
+    with the register epilogue in 128-column tiles, tc_gemm_kernel<128, false, 0>."""
     o = ops()
     B, H, W, C = 64, 16, 16, 2048
     x = grand((B, C, H, W), 41)

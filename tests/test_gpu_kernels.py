@@ -430,9 +430,10 @@ def test_groupnorm_and_conv_in(dtype):
     assert ok, msg
 
 
-def test_linear_geglu_lnfold_pair():
+def test_linear_geglu_lnfold():
     """inner LayerNorm folded through FF2: GEGLU epilogue accumulates per-row (sum, sumsq); LNFOLD_RESIDUAL applies
-    rstd * (acc - mean * cvec) + resid  ==  resid + LN(h) W2^T   (ref: muse_maskgit_pytorch.py:83-89)."""
+    rstd * (acc - mean * cvec) + resid  ==  resid + LN(h) W2^T   (ref: muse_maskgit_pytorch.py:83-89).  At M = 300 both products take 64-column
+    tiles: FF1 tc_gemm_kernel<64, false, 0> (register epilogue), FF2 tc_gemm_kernel<64, false, 2> (in-place TMA reduction)."""
     M, K, Fu, Fp, dim = 300, 128, 341, 384, 128
     bf = torch.bfloat16
     a = rnd("a", (M, K), bf)
@@ -462,7 +463,7 @@ def test_linear_geglu_lnfold_pair():
 
 
 def test_lfq_ids_gemm_epilogue_bit_exact():
-    """tcgen05 path of the LFQ lookup: 3-way bf16 split of project_in + LFQ_IDS epilogue; dyadic data -> bit-identical ids."""
+    """wgmma path of the LFQ lookup: 3-way bf16 split of project_in + LFQ_IDS epilogue; dyadic data -> bit-identical ids."""
     T, D, bits = 1000, 2048, 16
     bf = torch.bfloat16
     x = torch.from_numpy(synth.dyadic("vx", (T, D), bits=4, span=2.0))
@@ -509,8 +510,9 @@ def test_logits_sample_philox_matches_oracle_stream():
 
 
 def test_ff_geglu_lnfold_bitwise_reproducible_at_block_width():
-    """dim 512 / inner 1365 (44 statistic chunks per row, 11 column tiles, CTA pairs): the folded-LayerNorm FeedForward gives the same bits on
-    every run — the row statistics are per-chunk partials added in a fixed order, not atomics."""
+    """dim 512 / inner 1365 (44 statistic chunks per row, 11 column tiles; FF1 tc_gemm_kernel<256, false, 5>, FF2 tc_gemm_kernel<128, false, 2>):
+    the folded-LayerNorm FeedForward gives the same bits on every run — the row statistics are per-chunk partials added in a fixed order,
+    not atomics."""
     M, K, Fu, Fp, dim = 4096, 512, 1365, 1408, 512
     bf = torch.bfloat16
     g = torch.Generator(device="cuda").manual_seed(3)
@@ -680,7 +682,7 @@ def test_split3_terms_reconstruct_fp32():
 
 @pytest.mark.parametrize("M,N,K", [(256, 512, 512), (300, 192, 128), (1024, 2816, 512), (512, 512, 1408)])
 def test_linear_fp32_tensor_core_split_vs_fp64(M, N, K):
-    """precision='fp32' products run as 6K-wide bf16 products on tcgen05: error vs an fp64 reference at the level of the fp32 CUDA-core kernel."""
+    """precision='fp32' products run as 6K-wide bf16 products on wgmma: error vs an fp64 reference at the level of the fp32 CUDA-core kernel."""
     a, w = rnd(f"a{M}{K}", (M, K)), rnd(f"w{N}{K}", (N, K), std=K ** -0.5)
     ref = (a.double() @ w.double().t())
     o = ops()
