@@ -550,7 +550,7 @@ class MaskGit(nn.Module):
             self.train(was_training)
 
     def _generate(self, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
-                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids):
+                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, seed=None):
         tr = self.transformer
         if negative_texts is not None:
             raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
@@ -581,7 +581,8 @@ class MaskGit(nn.Module):
         if self.sampler_rng == "aten" and self.sampler_noise_fn is None:
             aten = self._aten_plan(device, b, fmap_size ** 2, tr.num_tokens, timesteps, use_critic)
         elif self.sampler_noise_fn is None:      # (injected noise: the host generator is the caller's stream — nothing is drawn from it here)
-            seed = self.sampler_seed if self.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+            if seed is None:                     # (a rerun on the materialised path keeps the seed of the attempt it repeats)
+                seed = self.sampler_seed if self.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
             self._seed_dev.fill_(seed)
         body = partial(self._generate_body, fmap_size=fmap_size, temperature=temperature, topk_filter_thres=topk_filter_thres,
                        timesteps=timesteps, cond_scale=cond_scale, b=b, use_critic=use_critic, critic_noise_scale=critic_noise_scale,
@@ -590,7 +591,7 @@ class MaskGit(nn.Module):
         if not self.use_cuda_graph or self.sampler_noise_fn is not None:
             images, ids, status = body(text_embeds, cond_images)
             if self._fused_tail_overflowed(status):
-                return self._generate_unfused(texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
+                return self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
                                               force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids)
             return (images, ids) if return_ids else images
         # ---- whole-call CUDA graph: 18 decode steps + VAE decode replayed as one launch (no per-kernel host work) ----
@@ -627,7 +628,7 @@ class MaskGit(nn.Module):
         graph.replay()
         images, ids = out_images.clone(), out_ids.clone()
         if self._fused_tail_overflowed(out_status):
-            return self._generate_unfused(texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
+            return self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
                                           force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids)
         return (images, ids) if return_ids else images
 
@@ -639,14 +640,16 @@ class MaskGit(nn.Module):
         self.last_fused_fallback_rows, overflow = (int(v) for v in status.tolist())
         return overflow != 0
 
-    def _generate_unfused(self, *args):
+    def _generate_unfused(self, seed, *args):
+        """Repeats a generate() call whose fused tail overflowed on the materialised path, with the same noise: the same libmmg seed, or the
+        ATen generator position the failed attempt started from."""
         saved = self.use_fused_tail
         self.use_fused_tail = False
         try:
             if self.sampler_rng == "aten" and self.sampler_noise_fn is None:       # re-read the generator position the failed attempt consumed
                 gen = torch.cuda.default_generators[next(self.parameters()).device.index or 0]
                 gen.set_offset(self._aten_start_offset)
-            return self._generate(*args)
+            return self._generate(*args, seed=seed)
         finally:
             self.use_fused_tail = saved
 

@@ -68,6 +68,26 @@ def test_decode_step_workspace_query_is_host_only():
     assert f(8, 2, 256, 512, 8, 1408, 65536, 256) < c3 and f(0, 2, 256, 512, 8, 1408, 65536, 256) == 0
 
 
+def test_fused_logits_planner_restatement_matches_workspace_query():
+    """oracle/fused_tail.py's restatement of mmg_logits_fused's planner (split count S and list capacity per row count, on the SM count the
+    library sees: the device's, or 132 without one) gives the library's workspace size everywhere: the GPU tests choose their row counts
+    from it to reach given plans."""
+    import math
+    import torch
+    from muse_maskgit_pytorch_b200 import ops
+    from oracle import fused_tail as FT
+    units = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
+    for V in (1024, 1280, 4096, 8192, 12288, 65536):
+        for K in (64, 512, 1024):
+            for k in (math.ceil(0.1 * V), math.ceil(0.2 * V)):
+                for R in (1, 77, 128, 129, 300, 1000, 2048, 4097, 6912, 8192, 8300, 13952, 16384, 16385, 25000, 40000):
+                    assert FT.workspace_bytes(R, V, K, k, units) == ops.logits_fused_workspace_bytes(R, V, K, k), (R, V, K, k, units)
+    assert FT.workspace_bytes(300, 65536, 512, math.ceil(0.2 * 65536), units) == 0
+    assert FT.lf_plan(16384, 65536, 132)["S"] == 1 and FT.lf_plan(8192, 65536, 132)["S"] == 2
+    for sms in (132, 114):                 # H100 SXM / PCIe: the GPU tests reach the shared-segment plans S = 1, 2 at V = 65536 on both
+        assert FT.rows_for_plan(65536, 1, sms) and FT.rows_for_plan(65536, 2, sms)
+
+
 def test_baseline_ref_is_the_unmodified_reference():
     """oracle/_ref (the reference arm of bench.py) is byte-identical to the reference checkout wherever both exist."""
     import filecmp

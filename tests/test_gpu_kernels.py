@@ -8,6 +8,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import synth, muse_oracle as O
+from tests import util
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
@@ -221,19 +222,6 @@ def _sample_case(b, n, nm, V, temp, logits, u=None, seed=5):
     return mp, idd.cpu(), sd.cpu(), k
 
 
-def _oracle_rows(logits, u_rows, temp, k):
-    """per-row reference: top-k filter (exactly k kept, ties by lowest index) + gumbel argmax + confidence."""
-    R, V = logits.shape
-    order = torch.argsort(-logits, dim=-1, stable=True)[:, :k]
-    keep = torch.zeros((R, V), dtype=torch.bool).scatter_(1, order, True)
-    filt = torch.where(keep, logits, torch.tensor(float("-inf")))
-    pert = filt / max(temp, 1e-10) + O.gumbel_from_uniform(u_rows)
-    pred = pert.argmax(-1)
-    top2 = pert.topk(2, dim=-1).values
-    p = logits.softmax(-1).gather(1, pred[:, None])[:, 0]
-    return pred, 1 - p, top2[:, 0] - top2[:, 1]
-
-
 @pytest.mark.parametrize("V,temp", [(65536, 1.0), (65536, 0.0), (1024, 0.5), (8192, 17 / 18), (512, 1.0)])
 def test_logits_sample_injected_noise(V, temp):
     b, n, nm = 2, 16, 5
@@ -241,7 +229,7 @@ def test_logits_sample_injected_noise(V, temp):
     u = torch.from_numpy(synth.uniform(f"u{V}", (b, n, V), 7))
     mp, ids, scores, k = _sample_case(b, n, nm, V, temp, logits, u)
     rows_u = torch.stack([u[bi, mp[bi, j]] for bi in range(b) for j in range(nm)])
-    pred, sc, margin = _oracle_rows(logits.reshape(-1, V), rows_u, temp, k)
+    pred, sc, margin = util.oracle_rows(logits.reshape(-1, V), rows_u, temp, k)
     got = torch.stack([ids[bi, mp[bi, j]] for bi in range(b) for j in range(nm)])
     gsc = torch.stack([scores[bi, mp[bi, j]] for bi in range(b) for j in range(nm)])
     bad = (got != pred) & (margin > 1e-4)
@@ -264,7 +252,7 @@ def test_logits_sample_adversarial_rows():
     u = torch.from_numpy(synth.uniform("uadv", (b, n, V), 9))
     mp, ids, scores, _ = _sample_case(b, n, nm, V, 1.0, logits, u)
     rows_u = torch.stack([u[0, mp[0, j]] for j in range(nm)])
-    pred, sc, margin = _oracle_rows(logits.reshape(-1, V), rows_u, 1.0, k)
+    pred, sc, margin = util.oracle_rows(logits.reshape(-1, V), rows_u, 1.0, k)
     got = torch.stack([ids[0, mp[0, j]] for j in range(nm)])
     assert torch.equal(got[margin > 1e-5], pred[margin > 1e-5]), (got.tolist(), pred.tolist())
 
@@ -503,7 +491,7 @@ def test_logits_sample_philox_matches_oracle_stream():
     ids = torch.full((b, n), V, dtype=torch.long, device="cuda"); sc = torch.full((b, n), -1e5, device="cuda")
     ops().logits_sample(dev(logits.reshape(-1, V).contiguous()), dev(mp), ids, sc, nm, k, 0.7, seed=seed, step=step, row_offset=off)
     rows_u = torch.stack([torch.from_numpy(philox.uniform(seed, step, off + bi * n + int(mp[bi, j]), V)) for bi in range(b) for j in range(nm)])
-    pred, score, margin = _oracle_rows(logits.reshape(-1, V), rows_u, 0.7, k)
+    pred, score, margin = util.oracle_rows(logits.reshape(-1, V), rows_u, 0.7, k)
     got = torch.stack([ids.cpu()[bi, mp[bi, j]] for bi in range(b) for j in range(nm)])
     assert torch.equal(got[margin > 1e-3], pred[margin > 1e-3]), (got.tolist(), pred.tolist())
     assert (got == pred).float().mean() > 0.9
@@ -659,7 +647,7 @@ def test_logits_sample_any_topk_threshold(thres, temp):
     ids = torch.full((b, n), V, dtype=torch.long, device="cuda"); sc = torch.full((b, n), -1e5, device="cuda")
     ops().logits_sample(dev(logits.reshape(nm, V).contiguous()), dev(mp), ids, sc, nm, k, temp, u=dev(u))
     rows_u = torch.stack([u[0, mp[0, j]] for j in range(nm)])
-    pred, score, margin = _oracle_rows(logits.reshape(-1, V), rows_u, temp, k)
+    pred, score, margin = util.oracle_rows(logits.reshape(-1, V), rows_u, temp, k)
     got = torch.stack([ids.cpu()[0, mp[0, j]] for j in range(nm)])
     gsc = torch.stack([sc.cpu()[0, mp[0, j]] for j in range(nm)])
     ok = margin > 1e-4

@@ -3,7 +3,7 @@ import os
 import numpy as np
 import torch
 
-from oracle import synth, shapes
+from oracle import synth, shapes, muse_oracle
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -44,6 +44,20 @@ def text_embeds(name, b, m, d, seed):
     te = torch.from_numpy(synth.normal(name, (b, m, d), seed))
     te[1::2, (3 * m) // 4:] = 0.
     return te
+
+
+def oracle_rows(logits, u_rows, temp, k):
+    """per-row reference of the sampling tail: top-k filter (exactly k kept, ties by lowest index) + gumbel argmax + confidence, in the
+    dtype of `logits` (float64 for the fused-tail tests).  Returns (token, 1 - softmax[token], top-2 margin of the perturbed values)."""
+    R, V = logits.shape
+    order = torch.argsort(-logits, dim=-1, stable=True)[:, :k]
+    keep = torch.zeros((R, V), dtype=torch.bool).scatter_(1, order, True)
+    filt = torch.where(keep, logits, torch.tensor(float("-inf"), dtype=logits.dtype))
+    pert = filt / max(temp, 1e-10) + muse_oracle.gumbel_from_uniform(u_rows)
+    pred = pert.argmax(-1)
+    top2 = pert.topk(2, dim=-1).values
+    p = logits.softmax(-1).gather(1, pred[:, None])[:, 0]
+    return pred, 1 - p, top2[:, 0] - top2[:, 1]
 
 
 def torch_noise_fn(seed):
