@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMG_VERSION 100
+#define MMG_VERSION 101
 
 /* error codes */
 #define MMG_OK            0
@@ -88,12 +88,6 @@ typedef struct {
   int32_t      heads, tokens, q_rows, kv_rows, key_off, nq_heads, nk_heads, nv_heads;
   /* CONVT(_RGB): input geometry of the GEMM rows (b, y, x) and the output parity                                  */
   int32_t      H, W, py, px;
-  /* Fused LayerNorm of the OUTPUT row (RESIDUAL / LNFOLD_RESIDUAL with N == 2 tile widths, bf16 tensor-core path): besides
-   * out = epilogue(acc) + resid the kernel also writes ln_out[r, :] = LN(out[r, :]) * gamma as bf16 for the next matrix product.
-   * Rows >= ln_split first get out += ln_add[:] and use ln_gamma_b (null-CFG rows whose cross-attention is the constant
-   * to_out(null_v)).  The two CTAs that own the halves of a row exchange (sum, sumsq) through distributed shared memory.  */
-  void*        ln_out; int64_t ld_ln;
-  const float* ln_gamma; const float* ln_gamma_b; const float* ln_add; int64_t ln_split;
   float*       row_stats;  /* [M, stats_slots, 2] fp32 (sum, sum of squares) partials.  GEGLU: the epilogue WRITES the statistics of each
                               64-column accumulator chunk (32 outputs, as rounded to out_dtype) to slot col / 64 (stats_slots >= N / 64;
                               every slot of every row is written exactly once, no atomics); LNFOLD_RESIDUAL: adds the stats_slots partials

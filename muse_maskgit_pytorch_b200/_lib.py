@@ -19,7 +19,6 @@ class EpilogueArgs(C.Structure):
                 ("heads", i32), ("tokens", i32), ("q_rows", i32), ("kv_rows", i32), ("key_off", i32),
                 ("nq_heads", i32), ("nk_heads", i32), ("nv_heads", i32),
                 ("H", i32), ("W", i32), ("py", i32), ("px", i32),
-                ("ln_out", vp), ("ld_ln", i64), ("ln_gamma", vp), ("ln_gamma_b", vp), ("ln_add", vp), ("ln_split", i64),
                 ("row_stats", vp), ("ln_width", i32), ("stats_slots", i32),
                 ("rgb_w", vp), ("rgb_b", vp), ("rgb_channels", i32), ("_pad", i32)]
 

@@ -108,7 +108,6 @@ int attention_tc_launch(const mmg_attention_args* a, cudaStream_t st) {
     rc = make_tmap_bf16(&p.tma_v, a->v, 2, dims, str, box); if (rc) return rc;
   }
   dim3 grid((a->Tq + 127) / 128, (unsigned)BH);
-  if (p.KB == 32) return attn_launch<32>(p, grid, st);
   if (p.KB == 64) return attn_launch<64>(p, grid, st);
   return attn_launch<128>(p, grid, st);
 }

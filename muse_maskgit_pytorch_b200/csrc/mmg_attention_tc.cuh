@@ -3,7 +3,7 @@
 // One CTA = one (batch, head, 128-query tile).  Key 0 of every (batch, head) is the learned null key: it is never masked, and it is handled
 // OUTSIDE the tensor-core blocks — each softmax thread computes its row's q . k_null with 64 FMAs, its weight joins the row sum and
 // p_null * v_null is added to O in the epilogue — so that the n = 256 (1 024, 32) real keys are exactly 4 (8, 1) blocks instead of 4 + a block
-// that holds one key.  The real keys 1 .. Tk-1 are walked in nb blocks of KB (32, 64 or 128) keys (the last block
+// that holds one key.  The real keys 1 .. Tk-1 are walked in nb blocks of KB (64 or 128) keys (the last block
 // may be shorter: KB_tail), twice (or once, see single_pass):
 //   pass A:  S = Q K^T (wgmma, 2 x m64nKBk16, 4 k-steps) -> shared-memory staging -> per-row running max        (no P, no V traffic)
 //   pass B:  S again -> p = exp2((s - max) * scale*log2e) in registers (masked / out-of-range keys -> 0), row sums in fp32,
@@ -260,9 +260,7 @@ inline bool attention_tc_supported(const mmg_attention_args* a) {
 // Key blocking: nb-1 blocks of KB keys and a last block of KB_tail keys (multiple of 32).  KB = 64 keeps a CTA at ~84 KB of shared memory,
 // so two CTAs share an SM and hide each other's MMA -> softmax -> MMA round trips; long sequences use 128-key blocks (fewer round trips per CTA).
 inline void attn_blocks(int Tk, int* nb, int* KB, int* KB_tail) {
-  static const int forced = [] { const char* e = getenv("MMG_ATTN_KB"); return e ? atoi(e) : 0; }();
-  int kb = forced ? forced : (Tk <= 640 ? 64 : 128);
-  if (kb != 32 && kb != 64 && kb != 128) kb = 64;
+  const int kb = Tk <= 640 ? 64 : 128;
   const int full = Tk / kb, rem = Tk - full * kb;
   *KB = kb;
   if (rem == 0) { *nb = full; *KB_tail = kb; }

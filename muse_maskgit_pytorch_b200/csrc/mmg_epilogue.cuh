@@ -297,9 +297,6 @@ struct Epilogue {
       for (int i = 0; i < 64; ++i) v[i] += __ldg(p.bias + col0 + i);
     }
   }
-  __device__ __forceinline__ void load_out_f32(int64_t row, int col0, float (&v)[64]) const {
-    Vec64<float>::load(reinterpret_cast<const float*>(p.out) + row * p.ldo + col0, v);
-  }
   __device__ __forceinline__ void store_f32(int64_t row, int col0, const float (&v)[64]) const {
     Vec64<float>::store(reinterpret_cast<float*>(p.out) + row * p.ldo + col0, v);
   }

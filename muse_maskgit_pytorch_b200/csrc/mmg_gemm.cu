@@ -9,76 +9,17 @@ int linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* stream)
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int BN>
+// persistent grid of min(tiles, #SM) CTAs; the tile epilogues keep 32 KB of per-warp output tiles next to the operand ring
+template <int BN, int EPI_MODE>
 static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
+  constexpr int smem = EPI_MODE == TC_EPI_REGS ? TcCfg<BN>::SMEM_BYTES : TcCfg<BN>::SMEM_BYTES_RED;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES); });
-  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm<%d>): %s", BN, cudaGetErrorString(attr_err));
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, EPI_MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm<%d, %d>): %s", BN, EPI_MODE, cudaGetErrorString(attr_err));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES, st, p));
-  MMG_LAUNCHED();
-  return MMG_OK;
-}
-
-// in-place reduction epilogue (x += A W^T through cp.reduce.async.bulk): the residual GEMMs of the transformer blocks
-template <int BN>
-static int launch_tc_red(const TcGemmParams& p, cudaStream_t st) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
-  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_red<%d>): %s", BN, cudaGetErrorString(attr_err));
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, 2>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
-  MMG_LAUNCHED();
-  return MMG_OK;
-}
-
-// plain fp32 store through the per-warp tiles + TMA store (the logits GEMM)
-template <int BN>
-static int launch_tc_tstore(const TcGemmParams& p, cudaStream_t st) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
-  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_tstore<%d>): %s", BN, cudaGetErrorString(attr_err));
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, 3>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
-  MMG_LAUNCHED();
-  return MMG_OK;
-}
-
-// QKV (MODE 4) / GEGLU (MODE 5) epilogues through per-warp tiles + TMA stores
-template <int BN, int MODE = 4>
-static int launch_tc_qkvt(const TcGemmParams& p, cudaStream_t st) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, false, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES_RED); });
-  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_tiles<%d, %d>): %s", BN, MODE, cudaGetErrorString(attr_err));
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, false, MODE>, dim3(grid), dim3(TC_THREADS), TcCfg<BN>::SMEM_BYTES_RED, st, p));
-  MMG_LAUNCHED();
-  return MMG_OK;
-}
-
-// LayerNorm-fused variant: clusters of two CTAs (column halves of the same rows), grid = 2 * min(#m-tiles, #SM / 2)
-template <int BN>
-static int launch_tc_lnf(const TcGemmParams& p, cudaStream_t st) {
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BN>::SMEM_BYTES); });
-  if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm_lnf<%d>): %s", BN, cudaGetErrorString(attr_err));
-  const int pairs = p.num_m_tiles < num_sms() / 2 ? p.num_m_tiles : num_sms() / 2;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = TcCfg<BN>::SMEM_BYTES; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  MMG_CUDA(cudaLaunchKernelEx(&cfg, tc_gemm_kernel<BN, true>, p));
+  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, EPI_MODE>, dim3(grid), dim3(TC_THREADS), smem, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -94,28 +35,21 @@ static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
 static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
   const mmg_epilogue_args& e = p.epi.p;
   const bool in_place = (p.epi.kind == MMG_EPI_LNFOLD_RESIDUAL || (p.epi.kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
-                        e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && !e.ln_out && p.mode == 0;
+                        e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && p.mode == 0;
   const bool plain_f32 = p.epi.kind == MMG_EPI_STORE && e.out_dtype == MMG_F32 && p.mode == 0 && !e.bias && e.act == 0 && (e.ldo % 4) == 0 && aligned16(e.out);
-  static const int red_forced = [] { const char* ev = getenv("MMG_GEMM_RED"); return ev ? atoi(ev) : -1; }();
-  static const int tstore_forced = [] { const char* ev = getenv("MMG_GEMM_TSTORE"); return ev ? atoi(ev) : -1; }();
-  static const int qkvt_forced = [] { const char* ev = getenv("MMG_GEMM_QKVT"); return ev ? atoi(ev) : -1; }();
   const bool qkv_tiles = p.epi.kind == MMG_EPI_QKV && e.out_dtype == MMG_BF16 && p.mode == 0 && e.tokens % 32 == 0 && p.M % 128 == 0 && (bn == 128 || bn == 256) &&
                          (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out))) && e.nk_heads == e.nv_heads;
-  static const int geglut_forced = [] { const char* ev = getenv("MMG_GEMM_GEGLUT"); return ev ? atoi(ev) : -1; }();
   const bool geglu_tiles = p.epi.kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && bn == 256 && (e.ldo % 8) == 0 && aligned16(e.out);
-  const int epi_mode = (in_place && red_forced != 0) ? 2 : (plain_f32 && tstore_forced != 0 && (bn == 256 || bn == 128)) ? 3 : (qkv_tiles && qkvt_forced != 0) ? 4 :
-                       (geglu_tiles && geglut_forced != 0) ? 5 : 0;
-  // the register epilogue (EPI_MODE 0) keeps 128 accumulator registers per thread at BN = 256 next to its 64-column chunk and spills; the
+  const int epi_mode = in_place ? TC_EPI_REDUCE : (plain_f32 && (bn == 256 || bn == 128)) ? TC_EPI_TSTORE : qkv_tiles ? TC_EPI_QKV :
+                       geglu_tiles ? TC_EPI_GEGLU : TC_EPI_REGS;
+  // the register epilogue keeps 128 accumulator registers per thread at BN = 256 next to its 64-column chunk and spills; the
   // tile epilogues at BN = 256 and every epilogue at BN = 128 fit the consumer warpgroups' registers
-  if (epi_mode == 0 && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
+  if (epi_mode == TC_EPI_REGS && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
   p.num_n_tiles = (int)((N + bn - 1) / bn);
-  {
-    static const int nfast_forced = [] { const char* e = getenv("MMG_GEMM_NFAST"); return e ? atoi(e) : -1; }();
-    p.n_fast = nfast_forced >= 0 ? nfast_forced : ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
-  }
+  p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
   uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
   int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
-  if (epi_mode == 4) {
+  if (epi_mode == TC_EPI_QKV) {
     const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads;
     uint64_t str[1] = {128}; uint32_t box[2] = {64, 32};
     if (e.nq_heads) { uint64_t d[2] = {64, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
@@ -124,25 +58,25 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
       rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
       rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
     }
-    return bn == 256 ? launch_tc_qkvt<256>(p, st) : launch_tc_qkvt<128>(p, st);
+    return bn == 256 ? launch_tc<256, TC_EPI_QKV>(p, st) : launch_tc<128, TC_EPI_QKV>(p, st);
   }
-  if (epi_mode == 5) {
+  if (epi_mode == TC_EPI_GEGLU) {
     uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 32};
     rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
-    return launch_tc_qkvt<256, 5>(p, st);
+    return launch_tc<256, TC_EPI_GEGLU>(p, st);
   }
-  if (epi_mode) {
+  if (epi_mode != TC_EPI_REGS) {
     uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 32};
     rc = make_tmap_f32(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
   }
-  if (epi_mode == 3) return bn == 256 ? launch_tc_tstore<256>(p, st) : launch_tc_tstore<128>(p, st);   // 128: the sample GEMM of the fused tail at small batch
-  if (epi_mode == 2) {
-    switch (bn) { case 64: return launch_tc_red<64>(p, st); case 128: return launch_tc_red<128>(p, st); case 256: return launch_tc_red<256>(p, st); }
+  if (epi_mode == TC_EPI_TSTORE) return bn == 256 ? launch_tc<256, TC_EPI_TSTORE>(p, st) : launch_tc<128, TC_EPI_TSTORE>(p, st);   // 128: the sample GEMM of the fused tail at small batch
+  if (epi_mode == TC_EPI_REDUCE) {
+    switch (bn) { case 64: return launch_tc<64, TC_EPI_REDUCE>(p, st); case 128: return launch_tc<128, TC_EPI_REDUCE>(p, st); case 256: return launch_tc<256, TC_EPI_REDUCE>(p, st); }
   }
   switch (bn) {
-    case 64: return launch_tc<64>(p, st);
-    case 128: return launch_tc<128>(p, st);
-    case 256: return launch_tc<256>(p, st);       // CONVT_RGB: the whole 256-column row in one tile
+    case 64: return launch_tc<64, TC_EPI_REGS>(p, st);
+    case 128: return launch_tc<128, TC_EPI_REGS>(p, st);
+    case 256: return launch_tc<256, TC_EPI_REGS>(p, st);       // CONVT_RGB: the whole 256-column row in one tile
   }
   return fail(MMG_EINVAL, "unsupported tile width %d", bn);
 }
@@ -277,7 +211,6 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   if (!tc_ok) {
     MMG_CHECK_ARG(!skip_if_zero, "skippable GEMM requires the bf16 tensor-core path");
     if (a->dtype == MMG_BF16) note_simt_fallback("mmg_linear", a->M, a->N, a->K);
-    MMG_CHECK_ARG(!a->epi.ln_out, "fused LayerNorm output requires the bf16 tensor-core path (K %% 64, N %% 64, aligned operands)");
     ConvGeom g{};
     return launch_simt<false>(a->dtype, a->a, a->w, a->M, a->N, a->K, a->lda, a->ldw, g, epi, st);
   }
@@ -288,17 +221,6 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   p.epi = epi; p.epi.fast = 1;
   uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda * 2}; uint32_t box[2] = {TC_BK, TC_BM};
   rc = make_tmap_bf16(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc;
-  if (a->epi.ln_out) {
-    const int bn = (int)(a->N / 2);
-    MMG_CHECK_ARG(bn == 64 || bn == 128 || bn == 256, "fused LayerNorm output needs N in {128, 256, 512} (two column tiles), got %lld", (long long)a->N);
-    MMG_CHECK_ARG((a->epilogue == MMG_EPI_RESIDUAL && a->epi.out_dtype == MMG_F32 && a->epi.act == 0 && a->epi.ldr % 8 == 0) || a->epilogue == MMG_EPI_LNFOLD_RESIDUAL,
-                  "fused LayerNorm output is offered for the fp32 RESIDUAL / LNFOLD_RESIDUAL epilogues");
-    MMG_CHECK_ARG(a->epi.ln_gamma && a->epi.ld_ln % 8 == 0, "fused LayerNorm output: gamma / ld_ln");
-    uint64_t dimsb[2] = {(uint64_t)a->K, (uint64_t)a->N}; uint64_t strb[1] = {(uint64_t)a->ldw * 2}; uint32_t boxb[2] = {TC_BK, (uint32_t)bn};
-    rc = make_tmap_bf16(&p.tma_b, a->w, 2, dimsb, strb, boxb); if (rc) return rc;
-    p.num_n_tiles = 2;
-    switch (bn) { case 64: return launch_tc_lnf<64>(p, st); case 128: return launch_tc_lnf<128>(p, st); default: return launch_tc_lnf<256>(p, st); }
-  }
   const int bn = pick_bn(p.num_m_tiles, a->N, a->epilogue);
   MMG_CHECK_ARG(bn == 64 || bn == 128 || bn == 256, "mmg_linear: unsupported N=%lld for this epilogue", (long long)a->N);
   return dispatch_tc(p, bn, a->w, a->N, a->K, a->ldw, st);

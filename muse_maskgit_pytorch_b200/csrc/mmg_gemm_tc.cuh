@@ -8,7 +8,7 @@
 //                 a TMA store / TMA reduction (EPI_MODE below).  setmaxnreg moves registers from warpgroup 0 (40/thread) to the consumers
 //                 (232/thread).
 //   persistent grid (<= #SM CTAs), static tile schedule (M- or N-fastest); the producer runs ahead into the next tile while the consumers
-//   finish the epilogue of the current one.  Variant: LNF (LayerNorm of the output row through a 2-CTA cluster).
+//   finish the epilogue of the current one.
 //
 // A is either a dense [M,K] matrix (2-D tensor map) or an NHWC activation addressed as an implicit-GEMM
 // convolution: the k-block (tap, channel-chunk) is fetched with a 4-D tensor map at shifted (x+dx, y+dy)
@@ -28,11 +28,20 @@ constexpr int TC_MAX_TAPS = 16;
 constexpr int TC_STG_LD = 132;           // staging row stride (floats): 128 columns + 4, conflict-free 16-byte row reads
 constexpr int TC_SMEM_LIMIT = 227 * 1024;
 
+// How the epilogue's results leave the CTA (the EPI_MODE of tc_gemm_kernel; described above the kernel).  The launcher picks one per product.
+enum TcEpiMode : int {
+  TC_EPI_REGS = 0,      // from registers, one thread per row
+  TC_EPI_REDUCE = 2,    // in-place residual: per-warp tiles + TMA reduction
+  TC_EPI_TSTORE = 3,    // plain fp32: per-warp tiles + TMA store
+  TC_EPI_QKV = 4,       // QKV heads: per-warp tiles + TMA stores
+  TC_EPI_GEGLU = 5,     // GEGLU, BN = 256: per-warp tiles + TMA store
+};
+
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
   CUtensorMap tma_b;
-  CUtensorMap tma_out;      // EPI_MODE 2 / 3: the fp32 output [M, N] in boxes of 32 rows x 32 columns (128 B), SWIZZLE_128B; EPI_MODE 5: bf16 [M, N/2], 32 x 64
-  CUtensorMap tma_qkv[3];   // EPI_MODE 4: q / k / v as [rows, 64] bf16 matrices in boxes of 32 rows x 64 columns (128 B)
+  CUtensorMap tma_out;      // REDUCE / TSTORE: the fp32 output [M, N] in boxes of 32 rows x 32 columns (128 B), SWIZZLE_128B; GEGLU: bf16 [M, N/2], 32 x 64
+  CUtensorMap tma_qkv[3];   // QKV: q / k / v as [rows, 64] bf16 matrices in boxes of 32 rows x 64 columns (128 B)
   int64_t M, N;
   int num_kb, num_m_tiles, num_n_tiles;
   int mode;                 // 0 dense, 1 conv (4-D A maps)
@@ -57,37 +66,33 @@ template <int BN> struct TcCfg {
   static constexpr int stages(int extra) {
     return (TC_SMEM_LIMIT - 1024 - 1024 - STG_BYTES - extra) / STAGE_BYTES < 6 ? (TC_SMEM_LIMIT - 1024 - 1024 - STG_BYTES - extra) / STAGE_BYTES : 6;
   }
-  // LNF keeps 8 KB of static shared memory for the statistics exchange
-  static constexpr int STAGES = stages(BN == 256 ? 8192 : 0);
+  static constexpr int STAGES = stages(0);
   static constexpr int STAGES_RED = stages(TILE_BYTES);
   static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 1024 + STG_BYTES;
   static constexpr int SMEM_BYTES_RED = 1024 + STAGES_RED * STAGE_BYTES + 1024 + TILE_BYTES + STG_BYTES;
   static_assert(STAGES >= 2 && STAGES_RED >= 2, "operand ring too shallow");
 };
 
-// LNF: the epilogue additionally emits LayerNorm(out row) as bf16 (see mmg_epilogue_args::ln_out).  Launched as clusters of two
-// CTAs that own the two column halves (N == 2 * BN) of the same 128 rows; per-row (sum, sumsq) partials cross through DSMEM.
 // One thread owns one output ROW, so a direct 32-byte store / load touches 32 different 128-byte lines per instruction, and the L1
 // retires such row-strided accesses slowly.  The fp32 epilogues therefore leave through shared memory and the TMA engine instead:
-// EPI_MODE 2 (RED): in-place residual epilogues (out == resid, fp32) write the term they add into a per-warp
+// TC_EPI_REDUCE: in-place residual epilogues (out == resid, fp32) write the term they add into a per-warp
 // 32 x 32 tile and push it with ONE TMA reduction (cp.reduce.async.bulk.tensor .add): the residual is never read, the adds happen
 // in L2, and the L1 sees 8 conflict-free shared-memory stores per thread instead of 16 row-strided global accesses.
-// EPI_MODE 3: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same tiles with a TMA store.
-// EPI_MODE 4: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 32 rows are 32 consecutive tokens of one
+// TC_EPI_TSTORE: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same tiles with a TMA store.
+// TC_EPI_QKV: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 32 rows are 32 consecutive tokens of one
 // sequence and land on 32 consecutive rows of one head of q / k / v): head chunk -> tile -> one TMA store per warp and chunk.
-// EPI_MODE 5: the GEGLU epilogue (bf16 out, BN == 256): the two warps of a lane quarter take ADJACENT chunk pairs (0,1 | 2,3), so a
+// TC_EPI_GEGLU: the GEGLU epilogue (bf16 out, BN == 256): the two warps of a lane quarter take ADJACENT chunk pairs (0,1 | 2,3), so a
 // warp's 2 x 32 outputs per row are 128 contiguous bytes -> one 32-row x 128-byte tile -> one TMA store per warp and tile.
-template <int BN, bool LNF = false, int EPI_MODE = 0>
+template <int BN, int EPI_MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   using namespace sm90;
   using Cfg = TcCfg<BN>;
-  constexpr bool RED = EPI_MODE == 2 || EPI_MODE == 3, RED_ADD = EPI_MODE == 2;   // 3: same tiles, plain TMA store
-  constexpr bool QKVT = EPI_MODE == 4;
-  constexpr bool GEGLUT = EPI_MODE == 5;
-  constexpr bool TILES = EPI_MODE != 0;
+  constexpr bool RED = EPI_MODE == TC_EPI_REDUCE || EPI_MODE == TC_EPI_TSTORE, RED_ADD = EPI_MODE == TC_EPI_REDUCE;   // TSTORE: same tiles, plain TMA store
+  constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
+  constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
+  constexpr bool TILES = EPI_MODE != TC_EPI_REGS;
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
-  static_assert(!(LNF && EPI_MODE != 0), "the LayerNorm-fused kernel has no room for the epilogue tiles");
   constexpr int STAGES = TILES ? Cfg::STAGES_RED : Cfg::STAGES;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
   constexpr int ROUNDS = (BN + 127) / 128;
@@ -105,12 +110,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   float* staging = reinterpret_cast<float*>(tiles + (TILES ? Cfg::TILE_BYTES : 0));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = LNF ? p.num_m_tiles : p.num_m_tiles * p.num_n_tiles;   // LNF: this CTA walks m-blocks, n-block = cluster rank
-  const int tile0 = LNF ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = LNF ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int my_rank = LNF ? (int)(blockIdx.x & 1) : 0;
-  __shared__ float s_part[LNF ? 2 : 1][2][LNF ? 128 : 1][2][2];                    // [buffer][cta rank][row][column half][sum, sumsq]
-  __shared__ uint64_t s_bar_stats;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+  const int tile0 = (int)blockIdx.x, tile_step = (int)gridDim.x;
   __shared__ float s_scale[128];               // QKV epilogue: q_scale | k_scale staged once per CTA
   if (p.epi.kind == MMG_EPI_QKV && threadIdx.x < 128) {
     const float* src = threadIdx.x < 64 ? p.epi.p.q_scale : p.epi.p.k_scale;
@@ -121,11 +122,9 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
     prefetch_tmap(&p.tma_b);
     prefetch_tmap(&p.tma_a[0]);
     for (int i = 0; i < STAGES; ++i) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, TC_EPI_WARPS); }
-    if (LNF) mbar_init(&s_bar_stats, 2 * TC_EPI_WARPS * 32);      // every epilogue thread of both CTAs arrives once per tile
     fence_barrier_init();
   }
   __syncthreads();
-  if (LNF) cluster_sync_all();                  // the peer's barriers must exist before the first remote arrive
   pdl_wait();                                   // everything above overlapped the previous kernel's tail
   pdl_trigger();
 
@@ -135,9 +134,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
       // ===================== TMA producer =====================
       int stage = 0; uint32_t phase = 0;
       for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        const int t_m = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, t_n = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
-        const int m_blk = LNF ? tile : t_m;
-        const int n_blk = LNF ? my_rank : t_n;
+        const int m_blk = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, n_blk = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
         int x0 = 0, y0 = 0, b0 = 0;
         if (p.mode == 1) {
           const int xt = m_blk % p.tiles_x, yt = (m_blk / p.tiles_x) % p.tiles_y, bt = m_blk / (p.tiles_x * p.tiles_y);
@@ -173,14 +170,11 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
     const bool whole_row = (epi.kind == MMG_EPI_CONVT_RGB);      // needs every chunk of a row in one thread
     const bool prefetch_resid = epi.can_prefetch_resid();
     int stage = 0; uint32_t phase = 0;
-    uint32_t stats_phase = 0; int stats_buf = 0;
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-      const int t_m = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, t_n = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
-      const int m_blk = LNF ? tile : t_m;
-      const int n_blk = LNF ? my_rank : t_n;
+      const int m_blk = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, n_blk = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
       int64_t row; bool valid;
       if (p.mode == 0) {
         row = (int64_t)m_blk * TC_BM + r_in_tile; valid = row < p.M;
@@ -196,7 +190,6 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
       const int c_end = GEGLUT ? c_first + 2 : BN / 64;
       const bool pre = EARLY_RESID && !RED && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
       float rbuf[64];
-      float ln_sum = 0.f, ln_sq = 0.f;
       if (pre) epi.load_resid(row, n_blk * BN + c_first * 64, rbuf);      // in flight during the main loop
       if (valid && mine) epi.begin_row(row);                               // row geometry / folded-LayerNorm statistics: independent of the accumulator
 
@@ -286,14 +279,6 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
             epi.fuse_resid(col0, v, rbuf);
             const int cn = col0 + c_step * 64;
             if (EARLY_RESID && c + c_step < BN / 64 && cn < p.N) epi.load_resid(row, cn, rbuf);   // next chunk's residual overlaps the stores
-            if (LNF) {
-              if (row >= epi.p.ln_split && epi.p.ln_add) {
-#pragma unroll
-                for (int i = 0; i < 64; ++i) v[i] += __ldg(epi.p.ln_add + col0 + i);
-              }
-#pragma unroll
-              for (int i = 0; i < 64; ++i) { ln_sum += v[i]; ln_sq = fmaf(v[i], v[i], ln_sq); }
-            }
             epi.store_f32(row, col0, v);
           } else {
             epi.template apply<true>(row, col0, v, 64);
@@ -317,44 +302,11 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         }
       }
       if (valid && mine) epi.end_row(row);
-      if (LNF) {
-        // ---- LayerNorm of the freshly written row: exchange (sum, sumsq) partials with the CTA that owns the other column half ----
-        const uint32_t slot = smem_u32(&s_part[stats_buf][my_rank][r_in_tile][half][0]);
-        st_cluster_v2f32(mapa_shared(slot, my_rank), ln_sum, ln_sq);
-        st_cluster_v2f32(mapa_shared(slot, my_rank ^ 1), ln_sum, ln_sq);
-        const uint32_t bar = smem_u32(&s_bar_stats);
-        mbar_arrive_cluster(mapa_shared(bar, my_rank));
-        mbar_arrive_cluster(mapa_shared(bar, my_rank ^ 1));
-        mbar_wait_cluster(&s_bar_stats, stats_phase);
-        stats_phase ^= 1;
-        float ts = 0.f, tq = 0.f;
-#pragma unroll
-        for (int rk = 0; rk < 2; ++rk)
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) { ts += s_part[stats_buf][rk][r_in_tile][hf][0]; tq += s_part[stats_buf][rk][r_in_tile][hf][1]; }
-        stats_buf ^= 1;
-        if (valid) {
-          const float inv_n = 1.0f / (float)p.N;
-          const float mean = ts * inv_n;
-          const float rstd = rsqrtf(fmaxf(tq * inv_n - mean * mean, 0.f) + 1e-5f);
-          const float* gam = (row >= epi.p.ln_split && epi.p.ln_gamma_b) ? epi.p.ln_gamma_b : epi.p.ln_gamma;
-#pragma unroll 1
-          for (int c = c_first; c < BN / 64; c += c_step) {
-            const int col0 = n_blk * BN + c * 64;
-            float v[64];
-            epi.load_out_f32(row, col0, v);                                   // written by this very thread a moment ago (L1/L2 hit)
-#pragma unroll
-            for (int i = 0; i < 64; ++i) v[i] = (v[i] - mean) * rstd * __ldg(gam + col0 + i);
-            Vec64<bf16>::store(reinterpret_cast<bf16*>(epi.p.ln_out) + row * epi.p.ld_ln + col0, v);
-          }
-        }
-      }
     }
   }
 
   if (TILES && warp >= 4 && lane == 0) bulk_wait0();   // every pushed tile has landed before the CTA (and its shared memory) goes away
   __syncthreads();
-  if (LNF) cluster_sync_all();                  // no CTA may exit while its peer can still write its shared memory
 }
 
 }  // namespace mmg

@@ -49,7 +49,6 @@ struct alignas(64) LfParams {
   CUtensorMap tma_a, tma_b;
   int64_t R;                      // rows (sampled positions of the step)
   int num_kb, num_m_tiles, num_pm, S, npt, cap;
-  int dbg;                        // MMG_LOGITS_DBG (measurement only): 1 = epilogue without the candidate lists, 2 = epilogue only reads the accumulators
   const float* thr;               // [R] candidate threshold per row
   float4* parts;                  // [R][S][2]: (running max, sum of exp(x - max), candidate count as int bits, overflow flag as int bits)
   uint2* lists;                   // [R][S][2][cap]: (logit bits, vocabulary index)
@@ -157,7 +156,6 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
           float v[64];
           stage_ld32(my_row, v);
           stage_ld32(my_row + 32, v + 32);
-          if (p.dbg == 2) { if (v[0] == 123.456f) m_run = v[5]; goto next_tile; }
           // ---- online softmax statistics of the row ----
           float lm = fmaxf(v[0], v[1]);
 #pragma unroll
@@ -168,7 +166,6 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
 #pragma unroll
           for (int i = 0; i < 64; i += 2) { s0 += ex2_approx(fmaf(v[i], LOG2E, -mb)); s1 += ex2_approx(fmaf(v[i + 1], LOG2E, -mb)); }
           s_run += s0 + s1;
-          if (p.dbg == 1) goto next_tile;
           // ---- candidates >= t_lo -> private FIFO (predicated, no branch) ----
           const uint32_t col0 = (uint32_t)(n_blk * LF_BN + c * 64);
           const uint32_t pos8_before = pos8;
@@ -197,7 +194,6 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
             flushed += 4;
           }
         }
-      next_tile:;
       }
       // ---- end of the work item: the last (< 4) entries as one padded sector, then the partial record ----
       const int pos = (int)(pos8 >> 8);
@@ -614,7 +610,6 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
     LfParams p{};
     p.R = R; p.num_kb = a->K / LF_BK; p.num_m_tiles = pl.num_m_tiles; p.num_pm = pl.num_pm; p.S = pl.S; p.npt = pl.npt; p.cap = pl.cap;
     p.thr = thr; p.parts = parts; p.lists = lists;
-    { const char* e = getenv("MMG_LOGITS_DBG"); p.dbg = e ? atoi(e) : 0; }
     uint64_t da[2] = {(uint64_t)a->K, (uint64_t)R}; uint64_t sa[1] = {(uint64_t)a->K * 2}; uint32_t ba[2] = {LF_BK, LF_BM};
     if ((rc = make_tmap_bf16(&p.tma_a, a->e, 2, da, sa, ba))) return rc;
     uint64_t db[2] = {(uint64_t)a->K, (uint64_t)s.V}; uint64_t sb[1] = {(uint64_t)a->K * 2}; uint32_t bb[2] = {LF_BK, (uint32_t)LF_BN};

@@ -1,4 +1,4 @@
-// Inline-PTX wrappers for the Hopper (sm_90a) async machinery: mbarrier, clusters, TMA, wgmma.
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery: mbarrier, TMA, wgmma.
 #pragma once
 #include <stdint.h>
 #include <cuda.h>
@@ -34,30 +34,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "@P1 bra DONE;\n\t"
       "bra WAIT_LOOP;\n\t"
       "DONE:\n\t}\n" :: "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
-// ---- thread-block clusters / distributed shared memory ------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t cta_rank) {
-  uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank)); return r;
-}
-__device__ __forceinline__ void st_cluster_v2f32(uint32_t cluster_addr, float a, float b) {
-  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" :: "r"(cluster_addr), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "WAIT_LOOP_C:\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%0], %1;\n\t"
-      "@P1 bra DONE_C;\n\t"
-      "bra WAIT_LOOP_C;\n\t"
-      "DONE_C:\n\t}\n" :: "r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
 // ---- TMA ----------------------------------------------------------------------------------------------
@@ -108,18 +84,6 @@ __device__ __forceinline__ void named_sync(uint32_t id, uint32_t nthreads) {
 // warpgroup.  Thread t of the warpgroup (warp w = t / 32, lane l) holds d[i] = D[16 w + l / 4 + 8 ((i / 2) % 2)][8 (i / 4) + 2 (l % 4) + i % 2].
 // TB = 1: B is MN-major (e.g. V[keys, 64] for O = P V).
 template <int N> struct Wgmma;
-template <> struct Wgmma<32> {
-  template <int TB> static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
-        "}, %16, %17, p, 1, 1, 0, %19;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(a), "l"(b), "r"(accumulate), "n"(TB));
-  }
-};
 template <> struct Wgmma<64> {
   template <int TB> static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
     asm volatile(

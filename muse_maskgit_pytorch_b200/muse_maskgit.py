@@ -270,11 +270,7 @@ class Transformer(nn.Module):
                 x[j * bn:(j + 1) * bn].copy_(x[:bn])
         else:
             ops.embed(ids.contiguous(), P["tok"], P["pos"], x, n=n, copies=nb)
-        fused = (adt == torch.bfloat16 and self.dim in (128, 256, 512) and all("w2f" in l["ff"] for l in P["layers"])
-                 and os.environ.get("MMG_FUSE_LN", "0") == "1")   # opt-in: measured equal at batch 64 and slower at batch 8 (DESIGN.md)
         live = [j for j in range(nb) if not ctx["all_masked"][j]]
-        if fused and live == list(range(len(live))):
-            return self._run_blocks_fused(P, ws, ctx, nb, b, n, len(live))
         for li, lay in enumerate(P["layers"]):
             sa, ca, ff = lay["sa"], lay["ca"], lay["ff"]
             # --- self attention (all branches) ---
@@ -310,44 +306,6 @@ class Transformer(nn.Module):
                     else:
                         ops.layernorm(xs, ff["g0"], xn[j * bn:(j + 1) * bn])
             self._ff_tail(xn, ff, x, ws, R)
-        return x
-
-    def _run_blocks_fused(self, P, ws, ctx, nb, b, n, n_live):
-        """bf16 block stack with every LayerNorm fused into the epilogue of the GEMM that produces its input (8 launches per
-        layer): the residual GEMMs write x (fp32) AND LN(x)*gamma (bf16) for the next matrix product; rows of an all-masked
-        CFG branch (>= split) receive the constant cross-attention term to_out(null_v) inside the self-attention output GEMM."""
-        adt, heads = P["adt"], self.transformer_blocks.heads
-        x, xn, q, k, v, ao, stats = ws["x"], ws["xn"], ws["q"], ws["k"], ws["v"], ws["ao"], ws["stats"]
-        bn = b * n
-        R, Rl = nb * bn, n_live * bn
-        layers = P["layers"]
-        ops.layernorm(x, layers[0]["sa"]["g"], xn)                           # the only stand-alone LayerNorm of the forward
-        for li, lay in enumerate(layers):
-            sa, ca, ff = lay["sa"], lay["ca"], lay["ff"]
-            epi = ops.qkv_epilogue(adt, heads, n, q=q, k=k, v=v, q_scale=sa["qs"], k_scale=sa["ks"], key_off=1, null_k=sa["nk"], null_v=sa["nv"])
-            ops.linear(xn, sa["wqkv"], None, epilogue=ops.EPI_QKV, epi=epi)
-            ops.attention(q, k, v, ao, nb * b, heads, n + 1, logit_bound=sa["bound"])
-            # x += attn out; live rows: xn = LN(x)*g_cross; rows >= Rl: x += to_out(null_v), xn = LN(x)*g_ff; FF row statistics reset
-            ops.linear(ao, sa["wo"], x, epilogue=ops.EPI_RESIDUAL, resid=x, ln_out=xn,
-                       ln_gamma=ca["g"] if Rl > 0 else ff["g0"], ln_gamma_b=ff["g0"], ln_add=ca["null_out"], ln_split=Rl)
-            if Rl > 0:
-                kc, vc = ctx["kv"][li]
-                nl = n_live * b
-                epi = ops.qkv_epilogue(adt, heads, n, q=q[:nl * heads], q_scale=ca["qs"])
-                ops.linear(xn[:Rl], ca["wq"], None, epilogue=ops.EPI_QKV, epi=epi)
-                ops.attention(q[:nl * heads], kc[:nl * heads], vc[:nl * heads], ao[:Rl], nl, heads, ctx["m"] + 1, key_mask=ctx["key_mask"][:nl],
-                              logit_bound=ca["bound"])
-                ops.linear(ao[:Rl], ca["wo"], x[:Rl], epilogue=ops.EPI_RESIDUAL, resid=x[:Rl], ln_out=xn[:Rl], ln_gamma=ff["g0"])
-            h = ws["h"][:R, :ff["Fp"]]
-            if ff["Fp"] != ws["h"].shape[1]:
-                h = h.contiguous()
-            stats = ws["stats"][:R, :ff["Fp"] // 32]
-            if stats.shape[1] != ws["stats"].shape[1]:
-                stats = stats.contiguous()
-            ops.linear(xn, ff["w1"], h, epilogue=ops.EPI_GEGLU, row_stats=stats)
-            nxt = layers[li + 1]["sa"]["g"] if li + 1 < len(layers) else None
-            ops.linear(h, ff["w2f"], x, epilogue=ops.EPI_LNFOLD_RESIDUAL, bias=ff["cvec"], resid=x, row_stats=stats, ln_width=ff["F"],
-                       ln_out=xn if nxt is not None else None, ln_gamma=nxt)
         return x
 
     def _ff_tail(self, xn, ff, x, ws, R):
@@ -598,7 +556,7 @@ class MaskGit(nn.Module):
         key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), fmap_size,
                float(temperature), float(topk_filter_thres), int(timesteps), float(cond_scale), int(self.row_offset), tr.precision, self.vae.precision,
                use_critic, float(critic_noise_scale), bool(can_remask_prev_masked), None if aten is None else aten["key"], bool(self.use_native_step),
-               id(self.noise_schedule), os.environ.get("MMG_FUSE_LN", "0"), bool(self.use_fused_tail))
+               id(self.noise_schedule), bool(self.use_fused_tail))
         pack_ids = lambda: (id(tr._pack), id(self.vae._pack), id(self.cond_vae._pack), id(critic_net._pack) if critic_net is not None else 0,
                             id(self.token_critic._head_cache) if isinstance(self.token_critic, SelfCritic) else 0)
         entry = self._graphs.get(key)
@@ -715,7 +673,7 @@ class MaskGit(nn.Module):
         adt = tr._packed()["adt"]
         bufs = dict(e=torch.empty((b * n, tr.dim), device=device, dtype=adt), rows_max=rows_max)
         nbytes = 0
-        if self.use_fused_tail and adt == torch.bfloat16 and k_keep is not None and os.environ.get("MMG_FUSED_TAIL", "1") != "0":
+        if self.use_fused_tail and adt == torch.bfloat16 and k_keep is not None:
             nbytes = ops.logits_fused_workspace_bytes(b * rows_max, V, tr.dim, k_keep)
         if nbytes:
             bufs["fused_ws"] = torch.empty((nbytes,), dtype=torch.uint8, device=device)

@@ -69,8 +69,7 @@ def _split_weight(w, rows, K):
     return s3
 
 
-def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, N=None, epi=None, row_stats=None, ln_width=0,
-           ln_out=None, ln_gamma=None, ln_gamma_b=None, ln_add=None, ln_split=None):
+def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, N=None, epi=None, row_stats=None, ln_width=0):
     """out = a @ w.T (+ epilogue).  a [M, K], w [N, K] same dtype (bf16 -> wgmma, fp32 -> CUDA cores)."""
     _chk(a, "a"); _chk(w, "w")
     assert w.shape[1] == a.shape[1] and a.dtype == w.dtype
@@ -86,10 +85,6 @@ def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, 
         assert out.shape[-1] * 2 >= args.N and out.stride(0) * 2 >= args.N, "GEGLU / GLU write N / 2 columns per row: `out` is too narrow"
     if epi is None:
         epi = _epi(out, out.stride(0), bias, act, resid, resid.stride(0) if resid is not None else 0, row_stats, ln_width)
-        if ln_out is not None:      # fused LayerNorm of the output rows (bf16) for the next matrix product
-            epi.ln_out = ln_out.data_ptr(); epi.ld_ln = ln_out.stride(0); epi.ln_gamma = ln_gamma.data_ptr()
-            epi.ln_gamma_b = L.ptr(ln_gamma_b); epi.ln_add = L.ptr(ln_add)
-            epi.ln_split = args.M if ln_split is None else ln_split
     args.epi = epi
     L.call("mmg_linear", args)
     return out

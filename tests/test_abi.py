@@ -18,7 +18,7 @@ def test_library_exports_header_symbols():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in mmg.h but not exported"
     assert set(_lib.EXPORTS) | set(_lib.PLAIN_EXPORTS) == declared
-    assert _lib.lib().mmg_version() == 100          # also runs the struct-size self check
+    assert _lib.lib().mmg_version() == 101          # also runs the struct-size self check
 
 
 def test_ops_fail_loudly_without_library(monkeypatch, tmp_path):

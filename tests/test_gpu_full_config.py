@@ -246,8 +246,8 @@ def _fp32_reference_math():
 
 @pytest.mark.parametrize("q_only", [False, True], ids=["self_qkv_32768x1536x512", "cross_q_16384x512x512"])
 def test_gemm_generate_shape_qkv(q_only):
-    """The QKV tile epilogue: the self-attention QKV product of a batch-64 CFG step (128 sequences x 256 tokens; tc_gemm_kernel<256, false, 4>)
-    and the cross-attention q product of its 64 conditional sequences (tc_gemm_kernel<128, false, 4>)."""
+    """The QKV tile epilogue: the self-attention QKV product of a batch-64 CFG step (128 sequences x 256 tokens; tc_gemm_kernel<256, 4>)
+    and the cross-attention q product of its 64 conditional sequences (tc_gemm_kernel<128, 4>)."""
     o = ops()
     b, n, heads, dim = (64 if q_only else 128), 256, 8, 512
     inner, nsec = heads * 64, (1 if q_only else 3)
@@ -274,8 +274,8 @@ def test_gemm_generate_shape_qkv(q_only):
 
 
 def test_gemm_generate_shape_ff_geglu_lnfold():
-    """FF1 32768 x 2816 x 512 with the GEGLU tile epilogue + row statistics (tc_gemm_kernel<256, false, 5>) and FF2 32768 x 512 x 1408 with
-    the LayerNorm fold and the in-place TMA reduction (tc_gemm_kernel<256, false, 2>), i.e. x += LN(gate * gelu(a Wx)) W2^T."""
+    """FF1 32768 x 2816 x 512 with the GEGLU tile epilogue + row statistics (tc_gemm_kernel<256, 5>) and FF2 32768 x 512 x 1408 with
+    the LayerNorm fold and the in-place TMA reduction (tc_gemm_kernel<256, 2>), i.e. x += LN(gate * gelu(a Wx)) W2^T."""
     o = ops()
     M_, K, Fu, Fp, dim = 32768, 512, 1365, 1408, 512
     a = grand((M_, K), 11)
@@ -309,7 +309,7 @@ def test_gemm_generate_shape_ff_geglu_lnfold():
 
 @pytest.mark.parametrize("M_", [32768, 16384 + 128 * 3], ids=["32768", "16768"])
 def test_gemm_generate_shape_wo_residual(M_):
-    """attention to_out: x += a Wo^T, 32768 x 512 x 512, in place through the TMA reduction (tc_gemm_kernel<256, false, 2>)."""
+    """attention to_out: x += a Wo^T, 32768 x 512 x 512, in place through the TMA reduction (tc_gemm_kernel<256, 2>)."""
     o = ops()
     a, w = grand((M_, 512), 21), grand((512, 512), 22, 512 ** -0.5)
     x = grand((M_, 512), 23, dtype=torch.float32)
@@ -321,7 +321,7 @@ def test_gemm_generate_shape_wo_residual(M_):
 
 @pytest.mark.parametrize("rows", [64 * 229, 64 * 47 + 5], ids=["14656", "3013_ragged"])
 def test_gemm_generate_shape_logits(rows):
-    """to_logits on the masked rows of a step: rows x 65536 x 512, fp32 out through the TMA-store tiles (tc_gemm_kernel<256, false, 3>)."""
+    """to_logits on the masked rows of a step: rows x 65536 x 512, fp32 out through the TMA-store tiles (tc_gemm_kernel<256, 3>)."""
     o = ops()
     a, w = grand((rows, 512), 31), grand((65536, 512), 32, 512 ** -0.5)
     out = torch.empty((rows + 3, 65536), device="cuda")
@@ -342,7 +342,7 @@ def _nhwc(t):
 
 def test_gemm_generate_shape_conv3x3_glu():
     """VAE decoder GLU res-block conv: 3x3, 2048 -> 4096 on 16 x 16 maps, batch 64, K = 18432: implicit GEMM (4-D tensor-map A operand)
-    with the register epilogue in 128-column tiles, tc_gemm_kernel<128, false, 0>."""
+    with the register epilogue in 128-column tiles, tc_gemm_kernel<128, 0>."""
     o = ops()
     B, H, W, C = 64, 16, 16, 2048
     x = grand((B, C, H, W), 41)
