@@ -70,13 +70,15 @@ enum mmg_epilogue {
                              ids[r] = sum_i ((hi+mid+lo)_i + bias_i > 0) << (bits-1-i), written as int64 to out[r]                */
   MMG_EPI_ARGMIN     = 9, /* nearest codebook row: W = codebook [K, D], bias = ||e_k||^2 [K]; out = uint64 best[M], initialised to
                              all-ones by the caller, updated with atomicMin( orderkey(||e||^2 - 2 x.e) << 32 | k ): lowest k on ties */
+  MMG_EPI_GEGLU_TANH = 10,/* GEGLU interleave (blocks of 32: [x(32) | gate(32)]), no bias, tanh-approximated GELU ("gelu_new" of T5 v1.1,
+                             t5.py): out[r, c/2] = gelu_tanh(x) * gate; mmg_linear only                                        */
 };
 
 typedef struct {
   void*        out;        /* see enum; [M, ldo]                                                                 */
   int64_t      ldo;        /* leading dimension of out (elements)                                                */
   int32_t      out_dtype;  /* MMG_F32 / MMG_BF16                                                                 */
-  int32_t      act;        /* 0 none, 1 leaky_relu(0.1)                                                          */
+  int32_t      act;        /* 0 none, 1 leaky_relu(0.1), 2 relu (STORE of mmg_linear only)                       */
   const float* bias;       /* [N] or NULL (for GEGLU/GLU: interleaved like W rows)                               */
   const void*  resid;      /* RESIDUAL: [M, ldr] of out_dtype                                                    */
   int64_t      ldr;
@@ -364,6 +366,37 @@ typedef struct {
 } mmg_decode_step_args;
 uint64_t mmg_decode_step_workspace_bytes(int32_t b, int32_t branches, int32_t n, int32_t dim, int32_t heads, int32_t Fp, int32_t V, int32_t max_masked);
 int mmg_decode_step(const mmg_decode_step_args* a, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * T5 text encoder (HF T5EncoderModel, eval mode; the text step of MaskGit.generate, t5.py:60-99).
+ * ---------------------------------------------------------------------------------------------- */
+/* T5 self-attention with d_kv = 64:  out[b*T + i, h*64 : h*64+64] = softmax_j( q_i . k_j + rel_bias[rel_bucket[j - i + T - 1], h] + m_j ) v_j
+ * over the T keys of sequence b: no 1/sqrt(d) scaling, m_j = 0 for a live key and -FLT_MAX (finfo(fp32).min) for a masked one, softmax in fp32
+ * (a row with no live key gets uniform weights over the T keys, as in HF).  q, k, v are read straight from the token-major output of one
+ * fused [3*heads*64, d_model] projection: row b*T + t = [q (heads*64) | k (heads*64) | v (heads*64)].
+ * dtype MMG_BF16: wgmma kernel (TMA loads, exact two-pass softmax, bias staged per CTA in shared memory); MMG_F32: CUDA-core fp32 kernel.  */
+typedef struct {
+  const void*    qkv;        /* [B*T, ldqkv] of dtype                                                                   */
+  void*          out;        /* [B*T, ldo] of dtype                                                                     */
+  const uint8_t* key_mask;   /* [B, T] (1 = attend) or NULL                                                             */
+  const int32_t* rel_bucket; /* [2T-1] int32: bucket of the relative position key - query, at index key - query + T - 1 */
+  const float*   rel_bias;   /* [num_buckets, heads] fp32 (relative_attention_bias.weight as stored)                    */
+  int32_t B, T, heads, num_buckets, dtype, _pad;  /* T <= 512                                                           */
+  int64_t ldqkv, ldo;        /* row strides (elements); ldqkv >= 3*heads*64                                             */
+} mmg_t5_attention_args;
+int mmg_t5_attention(const mmg_t5_attention_args* a, void* stream);
+
+/* T5 RMSNorm (T5LayerNorm): y[r, :] = w * (x[r, :] * rsqrt(mean(x[r, :]^2) + eps)), statistics in fp32, no mean, no bias;
+ * rows with row_mask[r] == 0 are written as zeros (the padding zero-fill of t5_encode_text).                          */
+typedef struct {
+  const float*   x;          /* [rows, ldx] fp32                                                                        */
+  void*          y;          /* [rows, ldy] of y_dtype                                                                  */
+  const float*   w;          /* [d]                                                                                     */
+  const uint8_t* row_mask;   /* [rows] or NULL                                                                          */
+  int64_t rows, d, ldx, ldy;
+  float   eps; int32_t y_dtype;
+} mmg_rmsnorm_args;
+int mmg_rmsnorm(const mmg_rmsnorm_args* a, void* stream);
 
 /* dtype conversion / layout helpers used by the host mirror */
 typedef struct { const void* src; void* dst; int64_t n; int32_t src_dtype, dst_dtype; } mmg_cast_args;

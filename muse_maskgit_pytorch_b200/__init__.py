@@ -4,5 +4,6 @@ minus the trainer, which is out of scope."""
 from .vqgan_vae import VQGanVAE
 from .muse_maskgit import Transformer, MaskGit, Muse, MaskGitTransformer, TokenCritic
 from .pack_cache import set_pack_cache
+from .t5 import T5Encoder
 
-__all__ = ["VQGanVAE", "Transformer", "MaskGit", "Muse", "MaskGitTransformer", "TokenCritic", "set_pack_cache"]
+__all__ = ["VQGanVAE", "Transformer", "MaskGit", "Muse", "MaskGitTransformer", "TokenCritic", "set_pack_cache", "T5Encoder"]

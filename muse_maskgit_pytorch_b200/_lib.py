@@ -8,7 +8,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MMG_LIB") or os.path.join(_HERE, "libmmg.so")     # MMG_LIB: an alternative build of the library
 
 F32, BF16 = 0, 1
-EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB, EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN = range(10)
+EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB, EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH = range(11)
 
 vp, i32, i64, f32, u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64
 
@@ -136,6 +136,16 @@ class Split3Args(C.Structure):
     _fields_ = [("src", vp), ("dst", vp), ("rows", i64), ("K", i64), ("lds", i64), ("side", i32), ("_pad", i32)]
 
 
+class T5AttentionArgs(C.Structure):
+    _fields_ = [("qkv", vp), ("out", vp), ("key_mask", vp), ("rel_bucket", vp), ("rel_bias", vp),
+                ("B", i32), ("T", i32), ("heads", i32), ("num_buckets", i32), ("dtype", i32), ("_pad", i32), ("ldqkv", i64), ("ldo", i64)]
+
+
+class RmsNormArgs(C.Structure):
+    _fields_ = [("x", vp), ("y", vp), ("w", vp), ("row_mask", vp), ("rows", i64), ("d", i64), ("ldx", i64), ("ldy", i64),
+                ("eps", f32), ("y_dtype", i32)]
+
+
 EXPORTS = {
     "mmg_linear": LinearArgs, "mmg_conv2d": Conv2dArgs, "mmg_conv_transpose2d": ConvTranspose2dArgs,
     "mmg_conv_in": ConvInArgs, "mmg_groupnorm": GroupNormArgs, "mmg_layernorm": LayerNormArgs, "mmg_embed": EmbedArgs,
@@ -143,6 +153,7 @@ EXPORTS = {
     "mmg_logits_sample": LogitsSampleArgs, "mmg_vq_lfq_encode": LfqEncodeArgs, "mmg_vq_l2_argmin": L2ArgminArgs,
     "mmg_vq_decode_codes": DecodeCodesArgs, "mmg_cast": CastArgs, "mmg_split3": Split3Args, "mmg_critic_score": CriticScoreArgs,
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,
+    "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs,
 }
 PLAIN_EXPORTS = ("mmg_version", "mmg_last_error", "mmg_launch_count", "mmg_sizeof", "mmg_decode_step_workspace_bytes", "mmg_logits_fused_workspace_bytes",
                  "mmg_simt_fallback_count", "mmg_simt_launch_count")

@@ -264,6 +264,53 @@ struct Epilogue {
     }
   }
 
+  // ---- T5 feed-forward epilogues: GEGLU_TANH and STORE with ReLU (act == 2) ----------------------------------------------
+  // Kept out of apply() so that the kernels which never see them compile as before: the tensor-core kernel reaches this through its own
+  // TC_EPI_ACT instantiation, the CUDA-core kernel through a kind test.  gelu_new(x) = 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)));
+  // with a bf16 output the MUFU tanh (relative error ~2^-11) is used, below the bf16 rounding that follows; an fp32 output gets tanhf.
+  static __device__ __forceinline__ float gelu_tanh(float x, bool approx) {
+    const float u = 0.7978845608028654f * fmaf(0.044715f * x, x * x, x);
+    float t;
+    if (approx) asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
+    else t = tanhf(u);
+    return 0.5f * x * (1.0f + t);
+  }
+  __device__ __forceinline__ void apply_act(int64_t row, int col0, float (&v)[64], int nvalid) const {
+    const bool bf = (p.out_dtype == MMG_BF16);
+    if (kind == MMG_EPI_GEGLU_TANH) {
+      float o[32];
+      const int oc = col0 >> 1;
+      if (bf) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] = v[32 + i] * gelu_tanh(v[i], true);
+        bf16* d = reinterpret_cast<bf16*>(p.out) + row * p.ldo + oc;
+        if ((p.ldo & 7) == 0) store32_bf16(d, o);
+        else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) d[i] = from_f<bf16>(o[i]);
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] = v[32 + i] * gelu_tanh(v[i], false);
+        float* d = reinterpret_cast<float*>(p.out) + row * p.ldo + oc;
+        if ((p.ldo & 3) == 0) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) reinterpret_cast<float4*>(d)[i] = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) d[i] = o[i];
+        }
+      }
+      return;
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) v[i] = fmaxf(v[i] + (p.bias && i < nvalid ? __ldg(p.bias + col0 + i) : 0.f), 0.f);
+    const bool vec_ok = (nvalid == 64) && ((p.ldo & 7) == 0);
+    if (bf) store_n(reinterpret_cast<bf16*>(p.out) + row * p.ldo + col0, v, nvalid, vec_ok);
+    else    store_n(reinterpret_cast<float*>(p.out) + row * p.ldo + col0, v, nvalid, vec_ok);
+  }
+  __host__ __device__ __forceinline__ bool is_act() const { return kind == MMG_EPI_GEGLU_TANH || (kind == MMG_EPI_STORE && p.act == 2); }
+
   // ---- residual epilogues with the residual chunk prefetched by the caller (tensor-core kernel) -------------------------
   __device__ __forceinline__ bool can_prefetch_resid() const {
     if (kind == MMG_EPI_LNFOLD_RESIDUAL) return true;
@@ -316,7 +363,8 @@ struct Epilogue {
 // host-side validation shared by the launchers
 inline int validate_epilogue(int kind, const mmg_epilogue_args& e, int64_t N) {
   switch (kind) {
-    case MMG_EPI_STORE: MMG_CHECK_ARG(e.out, "epilogue STORE: out is NULL"); break;
+    case MMG_EPI_STORE: MMG_CHECK_ARG(e.out && e.act >= 0 && e.act <= 2, "epilogue STORE: out is NULL or act not in {0, 1, 2}"); break;
+    case MMG_EPI_GEGLU_TANH: MMG_CHECK_ARG(e.out && (N % 64) == 0 && !e.bias, "epilogue GEGLU_TANH: N %% 64 != 0, out NULL or a bias given"); break;
     case MMG_EPI_RESIDUAL: MMG_CHECK_ARG(e.out && e.resid, "epilogue RESIDUAL: out/resid NULL"); break;
     case MMG_EPI_LFQ_IDS: MMG_CHECK_ARG(e.out && N == 64 && e.ln_width >= 1 && 3 * e.ln_width <= 64, "epilogue LFQ_IDS: N must be 64 and 3*bits <= 64"); break;
     case MMG_EPI_ARGMIN: MMG_CHECK_ARG(e.out && e.bias, "epilogue ARGMIN: out / code norms NULL"); break;

@@ -34,6 +34,13 @@ static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
 
 static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
   const mmg_epilogue_args& e = p.epi.p;
+  if (p.epi.is_act()) {                       // T5 feed-forward epilogues: their own register-epilogue instantiation at BN = 128
+    p.num_n_tiles = (int)((N + 127) / 128);
+    p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
+    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, 128};
+    int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
+    return launch_tc<128, TC_EPI_ACT>(p, st);
+  }
   const bool in_place = (p.epi.kind == MMG_EPI_LNFOLD_RESIDUAL || (p.epi.kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
                         e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && p.mode == 0;
   const bool plain_f32 = p.epi.kind == MMG_EPI_STORE && e.out_dtype == MMG_F32 && p.mode == 0 && !e.bias && e.act == 0 && (e.ldo % 4) == 0 && aligned16(e.out);
@@ -90,7 +97,7 @@ struct ConvGeom {
   int8_t tdy[25], tdx[25];
 };
 
-template <typename T, bool CONV>
+template <typename T, bool CONV, bool ACT>
 __global__ void __launch_bounds__(256)
 simt_gemm_kernel(const T* __restrict__ A, const T* __restrict__ Wt, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldw,
                  ConvGeom g, Epilogue epi) {
@@ -149,9 +156,13 @@ simt_gemm_kernel(const T* __restrict__ A, const T* __restrict__ Wt, int64_t M, i
       for (int i = 0; i < 64; ++i) v[i] = Cs[tid][i];
       int nvalid = (int)(N - n0); if (nvalid > 64) nvalid = 64;
       // CONVT_RGB needs the whole row in one pass and is not offered on this path (validated by the launcher)
-      epi.begin_row(row);
-      epi.template apply<false>(row, n0, v, nvalid);
-      epi.end_row(row);
+      if (ACT) {                                  // the T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU): an instantiation of their own
+        epi.apply_act(row, n0, v, nvalid);
+      } else {
+        epi.begin_row(row);
+        epi.template apply<false>(row, n0, v, nvalid);
+        epi.end_row(row);
+      }
     }
   }
 }
@@ -163,8 +174,11 @@ static int launch_simt(int dtype, const void* a, const void* w, int64_t M, int64
   MMG_CHECK_ARG(M > 0 && N > 0 && K > 0, "empty GEMM");
   dim3 grid((unsigned)((M + 63) / 64), (unsigned)((N + 63) / 64));
   MMG_CHECK_ARG(grid.y < 65536, "N too large for the fp32 path");
-  if (dtype == MMG_F32) simt_gemm_kernel<float, CONV><<<grid, 256, 0, st>>>((const float*)a, (const float*)w, M, N, K, lda, ldw, g, epi);
-  else simt_gemm_kernel<bf16, CONV><<<grid, 256, 0, st>>>((const bf16*)a, (const bf16*)w, M, N, K, lda, ldw, g, epi);
+  if (!CONV && epi.is_act()) {
+    if (dtype == MMG_F32) simt_gemm_kernel<float, false, true><<<grid, 256, 0, st>>>((const float*)a, (const float*)w, M, N, K, lda, ldw, g, epi);
+    else simt_gemm_kernel<bf16, false, true><<<grid, 256, 0, st>>>((const bf16*)a, (const bf16*)w, M, N, K, lda, ldw, g, epi);
+  } else if (dtype == MMG_F32) simt_gemm_kernel<float, CONV, false><<<grid, 256, 0, st>>>((const float*)a, (const float*)w, M, N, K, lda, ldw, g, epi);
+  else simt_gemm_kernel<bf16, CONV, false><<<grid, 256, 0, st>>>((const bf16*)a, (const bf16*)w, M, N, K, lda, ldw, g, epi);
   simt_launch_counter()++;
   MMG_LAUNCHED();
   return MMG_OK;
@@ -233,6 +247,7 @@ extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
   MMG_CHECK_ARG(a->kind != 2 || (a->H % 2 == 0 && a->W % 2 == 0), "mmg_conv2d: stride-2 conv needs even H, W");
   ConvGeom g; conv_geom(a->kind, a->B, a->H, a->W, a->Cin, &g);
   const int64_t M = (int64_t)a->B * g.Ho * g.Wo, N = a->Cout, K = (int64_t)g.ntaps * a->Cin;
+  MMG_CHECK_ARG(a->epilogue != MMG_EPI_GEGLU_TANH && a->epi.act != 2, "mmg_conv2d: GEGLU_TANH / ReLU epilogues are offered by mmg_linear only");
   int rc = validate_epilogue(a->epilogue, a->epi, N); if (rc) return rc;
   Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue; epi.fast = 0; epi.M = M; epi.N = N;
   TcGemmParams p{};

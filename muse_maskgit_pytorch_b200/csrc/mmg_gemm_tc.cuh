@@ -35,6 +35,7 @@ enum TcEpiMode : int {
   TC_EPI_TSTORE = 3,    // plain fp32: per-warp tiles + TMA store
   TC_EPI_QKV = 4,       // QKV heads: per-warp tiles + TMA stores
   TC_EPI_GEGLU = 5,     // GEGLU, BN = 256: per-warp tiles + TMA store
+  TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: from registers, one thread per row
 };
 
 struct alignas(64) TcGemmParams {
@@ -91,7 +92,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   constexpr bool RED = EPI_MODE == TC_EPI_REDUCE || EPI_MODE == TC_EPI_TSTORE, RED_ADD = EPI_MODE == TC_EPI_REDUCE;   // TSTORE: same tiles, plain TMA store
   constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
   constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
-  constexpr bool TILES = EPI_MODE != TC_EPI_REGS;
+  constexpr bool ACTT = EPI_MODE == TC_EPI_ACT;
+  constexpr bool TILES = EPI_MODE != TC_EPI_REGS && !ACTT;
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
   constexpr int STAGES = TILES ? Cfg::STAGES_RED : Cfg::STAGES;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
@@ -273,6 +275,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
               bulk_commit();
             }
           }
+        } else if (ACTT) {
+          if (valid && col0 < p.N) epi.apply_act(row, col0, v, 64);
         } else if (valid && col0 < p.N) {
           if (prefetch_resid) {
             if (!EARLY_RESID) epi.load_resid(row, col0, rbuf);

@@ -6,7 +6,7 @@ import torch
 
 from . import _lib as L
 from ._lib import (F32, BF16, EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB,  # noqa: F401
-                   EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN)
+                   EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH)
 
 
 def _chk(t, name="tensor"):
@@ -81,7 +81,7 @@ def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, 
     args.N = w.shape[0] if N is None else N
     args.K = a.shape[1]; args.lda = a.stride(0); args.ldw = w.stride(0)
     args.dtype = L.dt(a); args.epilogue = epilogue
-    if epilogue in (EPI_GEGLU, EPI_GLU) and out is not None:
+    if epilogue in (EPI_GEGLU, EPI_GLU, EPI_GEGLU_TANH) and out is not None:
         assert out.shape[-1] * 2 >= args.N and out.stride(0) * 2 >= args.N, "GEGLU / GLU write N / 2 columns per row: `out` is too narrow"
     if epi is None:
         epi = _epi(out, out.stride(0), bias, act, resid, resid.stride(0) if resid is not None else 0, row_stats, ln_width)
@@ -194,6 +194,32 @@ def attention(q, k, v, out, B, heads, Tk, key_mask=None, kv_shared=False, scale=
     a.ldo = out.stride(0); a.kv_batch_stride_zero = int(kv_shared); a.scale = scale; a.logit_bound = logit_bound
     L.call("mmg_attention", a)
     return out
+
+
+def t5_attention(qkv, out, B, T, heads, rel_bucket, rel_bias, key_mask=None):
+    """T5 self-attention (d_kv 64, relative-position bias, no scaling).  qkv [B*T, >= 3*heads*64] token-major q | k | v, out [B*T, >= heads*64]
+    of the same dtype (bf16 -> wgmma, fp32 -> CUDA cores); rel_bucket int32 [2T-1]; rel_bias fp32 [num_buckets, heads]; key_mask uint8 [B, T]."""
+    _chk(qkv, "qkv"); _chk(out, "out"); _chk(rel_bucket, "rel_bucket"); _chk(rel_bias, "rel_bias")
+    assert qkv.dtype == out.dtype and rel_bucket.dtype == torch.int32 and rel_bias.dtype == torch.float32 and rel_bucket.numel() == 2 * T - 1
+    assert key_mask is None or (key_mask.dtype == torch.uint8 and key_mask.is_contiguous() and key_mask.numel() == B * T)
+    a = L.T5AttentionArgs()
+    a.qkv = qkv.data_ptr(); a.out = out.data_ptr(); a.key_mask = L.ptr(key_mask); a.rel_bucket = rel_bucket.data_ptr(); a.rel_bias = rel_bias.data_ptr()
+    a.B = B; a.T = T; a.heads = heads; a.num_buckets = rel_bias.shape[0]; a.dtype = L.dt(qkv)
+    a.ldqkv = qkv.stride(0); a.ldo = out.stride(0)
+    L.call("mmg_t5_attention", a)
+    return out
+
+
+def rmsnorm(x, w, y, eps=1e-6, row_mask=None):
+    """T5LayerNorm: y = w * (x * rsqrt(mean(x^2) + eps)); x fp32 [rows, d], y fp32 / bf16; rows with row_mask == 0 (uint8 [rows]) are zeroed."""
+    _chk(x, "x"); _chk(w, "w")
+    assert x.dtype == torch.float32 and w.dtype == torch.float32 and y.stride(1) == 1
+    assert row_mask is None or (row_mask.dtype == torch.uint8 and row_mask.is_contiguous() and row_mask.numel() >= x.shape[0])
+    a = L.RmsNormArgs()
+    a.x = x.data_ptr(); a.y = y.data_ptr(); a.w = w.data_ptr(); a.row_mask = L.ptr(row_mask)
+    a.rows, a.d = x.shape; a.ldx = x.stride(0); a.ldy = y.stride(0); a.eps = eps; a.y_dtype = L.dt(y)
+    L.call("mmg_rmsnorm", a)
+    return y
 
 
 def remask(ids, scores, masked_pos, num_masked, mask_id):
