@@ -34,17 +34,20 @@ struct Epilogue {
     }
   }
 
+  // LNFOLD: (mean, rstd) of a row.  Its (sum, sumsq) = its per-chunk partials added in ascending chunk order: the same bits whichever CTA
+  // wrote which partial when
+  __device__ __forceinline__ void ln_row_stats(int64_t row, float& mean, float& rstd) const {
+    const float2* sp = reinterpret_cast<const float2*>(p.row_stats) + row * (int64_t)p.stats_slots;
+    float sx = 0.f, sq = 0.f;
+    for (int i = 0; i < p.stats_slots; ++i) { const float2 t = __ldg(sp + i); sx += t.x; sq += t.y; }
+    mean = sx / (float)p.ln_width;
+    rstd = rsqrtf(fmaxf(sq / (float)p.ln_width - mean * mean, 0.f) + 1e-5f);
+  }
+
   __device__ __forceinline__ void begin_row(int64_t row) {
     if (kind == MMG_EPI_QKV) { const uint32_t r = (uint32_t)row, d = (uint32_t)p.tokens; r_b = (int)(r / d); r_t = (int)(r - (uint32_t)r_b * d); }
     if (kind == MMG_EPI_CONVT || kind == MMG_EPI_CONVT_RGB) { const uint32_t r = (uint32_t)row, d = (uint32_t)(p.H * p.W); r_b = (int)(r / d); r_t = (int)(r - (uint32_t)r_b * d); }
-    if (kind == MMG_EPI_LNFOLD_RESIDUAL) {
-      // the row's (sum, sumsq) = its per-chunk partials added in ascending chunk order: the same bits whichever CTA wrote which partial when
-      const float2* sp = reinterpret_cast<const float2*>(p.row_stats) + row * (int64_t)p.stats_slots;
-      float sx = 0.f, sq = 0.f;
-      for (int i = 0; i < p.stats_slots; ++i) { const float2 t = __ldg(sp + i); sx += t.x; sq += t.y; }
-      const float mean = sx / (float)p.ln_width;
-      st_a = mean; st_b = rsqrtf(fmaxf(sq / (float)p.ln_width - mean * mean, 0.f) + 1e-5f);
-    }
+    if (kind == MMG_EPI_LNFOLD_RESIDUAL) ln_row_stats(row, st_a, st_b);
     if (kind == MMG_EPI_CONVT_RGB) {
 #pragma unroll
       for (int c = 0; c < 4; ++c) rgb_acc[c] = (c < p.rgb_channels) ? p.rgb_b[c] : 0.f;
@@ -54,11 +57,15 @@ struct Epilogue {
   // row: global output row (< M). col0: first accumulator column of this chunk (multiple of 64). nvalid: columns < N.
   // QKV: which output a 64-column chunk belongs to (0 q, 1 k, 2 v), its head, and the l2-normalisation * scale of q / k in place
   //   F.normalize(dim=-1, eps=1e-12) then * scale   (muse_maskgit_pytorch.py:151-153)
-  template <bool FAST>
-  __device__ __forceinline__ int qkv_chunk(int col0, float (&v)[64], int& h) const {
+  __device__ __forceinline__ int qkv_head(int col0, int& h) const {
     const int hc = col0 >> 6;
     const int which = hc < p.nq_heads ? 0 : (hc < p.nq_heads + p.nk_heads ? 1 : 2);
     h = which == 0 ? hc : (which == 1 ? hc - p.nq_heads : hc - p.nq_heads - p.nk_heads);
+    return which;
+  }
+  template <bool FAST>
+  __device__ __forceinline__ int qkv_chunk(int col0, float (&v)[64], int& h) const {
+    const int which = qkv_head(col0, h);
     const float* sc = which == 0 ? p.q_scale : (which == 1 ? p.k_scale : nullptr);
     if (sc) {
       float s4[4] = {0.f, 0.f, 0.f, 0.f};                    // four partial sums: 16-deep dependency chains instead of 64
@@ -329,20 +336,16 @@ struct Epilogue {
       for (int i = 0; i < 64; ++i) v[i] += r[i] + (p.bias ? __ldg(p.bias + col0 + i) : 0.f);
     }
   }
-  // residual epilogues as an in-place reduction (out == resid): v <- the term added to the row; the caller pushes it with
+  // residual epilogues as an in-place reduction (out == resid): the term added to the row; the caller pushes it with
   // cp.reduce.async.bulk (fp32 add in L2), so the residual row is never read and nothing goes through the L1 wavefront path
   __device__ __forceinline__ bool can_reduce_in_place() const {
     return can_prefetch_resid() && p.out == p.resid && p.ldo == p.ldr && p.out_dtype == MMG_F32 && (p.ldo & 3) == 0 &&
            (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
   }
-  __device__ __forceinline__ void resid_term(int col0, float (&v)[64]) const {
-    if (kind == MMG_EPI_LNFOLD_RESIDUAL) {
-#pragma unroll
-      for (int i = 0; i < 64; ++i) v[i] = st_b * (v[i] - st_a * __ldg(p.bias + col0 + i));
-    } else if (p.bias) {
-#pragma unroll
-      for (int i = 0; i < 64; ++i) v[i] += __ldg(p.bias + col0 + i);
-    }
+  // elementwise: the term for the accumulator v at column col of a row whose LNFOLD (mean, rstd) is (a, b)
+  __device__ __forceinline__ float resid_term(float v, int col, float a, float b) const {
+    if (kind == MMG_EPI_LNFOLD_RESIDUAL) return b * (v - a * __ldg(p.bias + col));
+    return p.bias ? v + __ldg(p.bias + col) : v;
   }
   __device__ __forceinline__ void store_f32(int64_t row, int col0, const float (&v)[64]) const {
     Vec64<float>::store(reinterpret_cast<float*>(p.out) + row * p.ldo + col0, v);

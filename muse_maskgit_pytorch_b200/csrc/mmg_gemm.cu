@@ -9,10 +9,11 @@ int linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* stream)
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// persistent grid of min(tiles, #SM) CTAs; the tile epilogues keep 32 KB of per-warp output tiles next to the operand ring
+// persistent grid of min(tiles, #SM) CTAs; the tile epilogues keep 32 KB of per-warp output tiles next to the operand ring instead of
+// the register epilogues' 66 KB staging buffer
 template <int BN, int EPI_MODE>
 static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
-  constexpr int smem = EPI_MODE == TC_EPI_REGS ? TcCfg<BN>::SMEM_BYTES : TcCfg<BN>::SMEM_BYTES_RED;
+  constexpr int smem = tc_tile_epilogue(EPI_MODE) ? TcCfg<BN>::SMEM_BYTES_RED : TcCfg<BN>::SMEM_BYTES;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, EPI_MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
@@ -52,13 +53,15 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
   // the register epilogue keeps 128 accumulator registers per thread at BN = 256 next to its 64-column chunk and spills; the
   // tile epilogues at BN = 256 and every epilogue at BN = 128 fit the consumer warpgroups' registers
   if (epi_mode == TC_EPI_REGS && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
+  // the tile epilogues write whole 32- / 64-column boxes: pick_bn's widths divide N (N % 64 == 0 on this path)
+  MMG_CHECK_ARG(epi_mode == TC_EPI_REGS || N % bn == 0, "tile epilogue: tile width %d does not divide N = %lld", bn, (long long)N);
   p.num_n_tiles = (int)((N + bn - 1) / bn);
   p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
   uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
   int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
   if (epi_mode == TC_EPI_QKV) {
     const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads;
-    uint64_t str[1] = {128}; uint32_t box[2] = {64, 32};
+    uint64_t str[1] = {128}; uint32_t box[2] = {64, 16};
     if (e.nq_heads) { uint64_t d[2] = {64, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
     if (e.nk_heads) {
       uint64_t d[2] = {64, seqs * (uint64_t)e.kv_rows};
@@ -68,12 +71,12 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
     return bn == 256 ? launch_tc<256, TC_EPI_QKV>(p, st) : launch_tc<128, TC_EPI_QKV>(p, st);
   }
   if (epi_mode == TC_EPI_GEGLU) {
-    uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 32};
+    uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 16};
     rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
     return launch_tc<256, TC_EPI_GEGLU>(p, st);
   }
   if (epi_mode != TC_EPI_REGS) {
-    uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 32};
+    uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 16};
     rc = make_tmap_f32(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
   }
   if (epi_mode == TC_EPI_TSTORE) return bn == 256 ? launch_tc<256, TC_EPI_TSTORE>(p, st) : launch_tc<128, TC_EPI_TSTORE>(p, st);   // 128: the sample GEMM of the fused tail at small batch

@@ -2,10 +2,10 @@
 //
 //   warp 0      : TMA producer  (one elected lane) — A tile 128x64 and W tile BNx64 per k-block, SWIZZLE_128B, STAGES-deep ring
 //   warps 4..11 : two consumer warpgroups.  Warpgroup g multiplies rows [64 g, 64 g + 64) of the tile (wgmma m64nBNk16, 4 per k-block,
-//                 accumulators in registers), then runs the fused Epilogue on those rows: the accumulators go through a shared-memory
-//                 staging buffer (128 columns at a time) so that one thread owns one output row, 64 columns per chunk; two warps share a
-//                 32-row quarter and take alternate 64-column chunks.  Results leave directly, or through a per-warp shared-memory tile and
-//                 a TMA store / TMA reduction (EPI_MODE below).  setmaxnreg moves registers from warpgroup 0 (40/thread) to the consumers
+//                 accumulators in registers), then runs the fused Epilogue on those rows (EPI_MODE below): either from the accumulator
+//                 registers into per-warp shared-memory boxes and a TMA store / TMA reduction, or through a shared-memory staging buffer
+//                 (128 columns at a time) so that one thread owns one output row, 64 columns per chunk; two warps then share a 32-row
+//                 quarter and take alternate 64-column chunks.  setmaxnreg moves registers from warpgroup 0 (40/thread) to the consumers
 //                 (232/thread).
 //   persistent grid (<= #SM CTAs), static tile schedule (M- or N-fastest); the producer runs ahead into the next tile while the consumers
 //   finish the epilogue of the current one.
@@ -37,12 +37,14 @@ enum TcEpiMode : int {
   TC_EPI_GEGLU = 5,     // GEGLU, BN = 256: per-warp tiles + TMA store
   TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: from registers, one thread per row
 };
+// the modes whose epilogue runs from the accumulator fragments through per-warp output boxes (no staging buffer)
+constexpr bool tc_tile_epilogue(int mode) { return mode != TC_EPI_REGS && mode != TC_EPI_ACT; }
 
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
   CUtensorMap tma_b;
-  CUtensorMap tma_out;      // REDUCE / TSTORE: the fp32 output [M, N] in boxes of 32 rows x 32 columns (128 B), SWIZZLE_128B; GEGLU: bf16 [M, N/2], 32 x 64
-  CUtensorMap tma_qkv[3];   // QKV: q / k / v as [rows, 64] bf16 matrices in boxes of 32 rows x 64 columns (128 B)
+  CUtensorMap tma_out;      // REDUCE / TSTORE: the fp32 output [M, N] in boxes of 16 rows x 32 columns (128 B), SWIZZLE_128B; GEGLU: bf16 [M, N/2], 16 x 64
+  CUtensorMap tma_qkv[3];   // QKV: q / k / v as [rows, 64] bf16 matrices in boxes of 16 rows x 64 columns (128 B)
   int64_t M, N;
   int num_kb, num_m_tiles, num_n_tiles;
   int mode;                 // 0 dense, 1 conv (4-D A maps)
@@ -57,7 +59,9 @@ struct alignas(64) TcGemmParams {
   Epilogue epi;
 };
 
-// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][per-warp output tiles, 32 KB (tile epilogues only)][staging, 2 x 64 x 132 fp32]
+// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][register epilogues: staging, 2 x 64 x 132 fp32 | tile epilogues: per-warp
+// output tiles, 32 KB].  Without the staging buffer the tile epilogues get 4 operand stages at BN = 256 and 6 at BN <= 128 (register
+// epilogues: 3, 4 and 6 at BN = 256, 128, 64); the 512 B static s_scale fits in what the 227 KB limit leaves over.
 template <int BN> struct TcCfg {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;
   static constexpr int B_BYTES = BN * TC_BK * 2;
@@ -65,25 +69,28 @@ template <int BN> struct TcCfg {
   static constexpr int STG_BYTES = 2 * 64 * TC_STG_LD * 4;
   static constexpr int TILE_BYTES = TC_EPI_WARPS * 4096;
   static constexpr int stages(int extra) {
-    return (TC_SMEM_LIMIT - 1024 - 1024 - STG_BYTES - extra) / STAGE_BYTES < 6 ? (TC_SMEM_LIMIT - 1024 - 1024 - STG_BYTES - extra) / STAGE_BYTES : 6;
+    return (TC_SMEM_LIMIT - 1024 - 1024 - extra) / STAGE_BYTES < 6 ? (TC_SMEM_LIMIT - 1024 - 1024 - extra) / STAGE_BYTES : 6;
   }
-  static constexpr int STAGES = stages(0);
+  static constexpr int STAGES = stages(STG_BYTES);
   static constexpr int STAGES_RED = stages(TILE_BYTES);
   static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 1024 + STG_BYTES;
-  static constexpr int SMEM_BYTES_RED = 1024 + STAGES_RED * STAGE_BYTES + 1024 + TILE_BYTES + STG_BYTES;
+  static constexpr int SMEM_BYTES_RED = 1024 + STAGES_RED * STAGE_BYTES + 1024 + TILE_BYTES;
   static_assert(STAGES >= 2 && STAGES_RED >= 2, "operand ring too shallow");
+  static_assert(SMEM_BYTES + 512 <= TC_SMEM_LIMIT && SMEM_BYTES_RED + 512 <= TC_SMEM_LIMIT, "dynamic + static shared memory over the opt-in limit");
 };
 
-// One thread owns one output ROW, so a direct 32-byte store / load touches 32 different 128-byte lines per instruction, and the L1
-// retires such row-strided accesses slowly.  The fp32 epilogues therefore leave through shared memory and the TMA engine instead:
-// TC_EPI_REDUCE: in-place residual epilogues (out == resid, fp32) write the term they add into a per-warp
-// 32 x 32 tile and push it with ONE TMA reduction (cp.reduce.async.bulk.tensor .add): the residual is never read, the adds happen
-// in L2, and the L1 sees 8 conflict-free shared-memory stores per thread instead of 16 row-strided global accesses.
-// TC_EPI_TSTORE: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same tiles with a TMA store.
-// TC_EPI_QKV: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 32 rows are 32 consecutive tokens of one
-// sequence and land on 32 consecutive rows of one head of q / k / v): head chunk -> tile -> one TMA store per warp and chunk.
-// TC_EPI_GEGLU: the GEGLU epilogue (bf16 out, BN == 256): the two warps of a lane quarter take ADJACENT chunk pairs (0,1 | 2,3), so a
-// warp's 2 x 32 outputs per row are 128 contiguous bytes -> one 32-row x 128-byte tile -> one TMA store per warp and tile.
+// Register epilogues (TC_EPI_REGS, TC_EPI_ACT) need one thread to own a whole output row, so the accumulators go through the staging
+// buffer.  The tile epilogues need no such thing: each of their terms is elementwise, or (GEGLU) pairs column i with column 32 + i, which
+// the wgmma fragment keeps in the same thread.  They go from the accumulator registers straight into the warp's output boxes, and the
+// TMA engine writes the boxes out.  Thread t of a warpgroup (warp w, lane l) holds rows 16 w + l / 4 and + 8 at columns 8 j + 2 (l % 4)
+// and + 1, so a warp owns 16 whole rows; a box is 16 rows x 128 bytes (TMA 128-byte swizzle), and the warp's 4 KB tile double-buffers two.
+// The launcher takes a tile epilogue only at a tile width BN that divides N, so every box lies inside the N columns.
+// TC_EPI_REDUCE: in-place residual epilogues (out == resid, fp32) push the term they add with a TMA reduction
+// (cp.reduce.async.bulk.tensor .add), 32 columns per box: the residual is never read and the adds happen in L2.
+// TC_EPI_TSTORE: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same boxes with a TMA store.
+// TC_EPI_QKV: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 16 rows are 16 consecutive tokens of one
+// sequence and land on 16 consecutive rows of one head of q / k / v): one box and one TMA store per warp and head chunk.
+// TC_EPI_GEGLU: the GEGLU epilogue (bf16 out, BN == 256): two 64-column chunks make 64 outputs = one box per warp.
 template <int BN, int EPI_MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
@@ -93,7 +100,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
   constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
   constexpr bool ACTT = EPI_MODE == TC_EPI_ACT;
-  constexpr bool TILES = EPI_MODE != TC_EPI_REGS && !ACTT;
+  constexpr bool TILES = tc_tile_epilogue(EPI_MODE);
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
   constexpr int STAGES = TILES ? Cfg::STAGES_RED : Cfg::STAGES;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
@@ -108,8 +115,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint8_t* tiles = smem + STAGES * STAGE_BYTES + 1024;
-  float* staging = reinterpret_cast<float*>(tiles + (TILES ? Cfg::TILE_BYTES : 0));
+  uint8_t* tiles = smem + STAGES * STAGE_BYTES + 1024;      // tile epilogues: per-warp output tiles
+  float* staging = reinterpret_cast<float*>(tiles);         // register epilogues: staging buffer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
@@ -171,6 +178,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
     if (epi.kind == MMG_EPI_QKV) { epi.p.q_scale = s_scale; epi.p.k_scale = s_scale + 64; }
     const bool whole_row = (epi.kind == MMG_EPI_CONVT_RGB);      // needs every chunk of a row in one thread
     const bool prefetch_resid = epi.can_prefetch_resid();
+    const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;   // tile epilogues: this warp's two 2 KB output boxes
+    uint32_t nbox = 0;                                                         // boxes this warp has filled so far
     int stage = 0; uint32_t phase = 0;
     float acc[BN / 2];
 #pragma unroll
@@ -188,12 +197,16 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         row = ((int64_t)b * p.Ho + (yt * p.TH + ty)) * p.Wo + xt * p.TW + tx;
       }
       const bool mine = !whole_row || half == 0;
-      const int c_first = GEGLUT ? 2 * half : whole_row ? 0 : half, c_step = (GEGLUT || whole_row) ? 1 : 2;
-      const int c_end = GEGLUT ? c_first + 2 : BN / 64;
-      const bool pre = EARLY_RESID && !RED && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
+      const int c_first = whole_row ? 0 : half, c_step = whole_row ? 1 : 2, c_end = BN / 64;
+      const bool pre = EARLY_RESID && !TILES && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
       float rbuf[64];
       if (pre) epi.load_resid(row, n_blk * BN + c_first * 64, rbuf);      // in flight during the main loop
-      if (valid && mine) epi.begin_row(row);                               // row geometry / folded-LayerNorm statistics: independent of the accumulator
+      if (!TILES && valid && mine) epi.begin_row(row);                     // row geometry / folded-LayerNorm statistics: independent of the accumulator
+      // tile epilogues: the warp's 16 fragment rows start at brow; LNFOLD statistics of row brow + l / 4 + 8 (l % 4) in lanes l % 4 < 2
+      const int64_t brow = (int64_t)m_blk * TC_BM + wg * 64 + 16 * wq;
+      float ln_a = 0.f, ln_b = 0.f;
+      if (RED_ADD && epi.kind == MMG_EPI_LNFOLD_RESIDUAL && (lane & 3) < 2 && brow + (lane >> 2) + 8 * (lane & 3) < p.M)
+        epi.ln_row_stats(brow + (lane >> 2) + 8 * (lane & 3), ln_a, ln_b);
 
       // ---- main loop: 4 wgmma (K = 16) per k-block; a ring slot goes back to the producer once the wgmma group after it was issued ----
       int prev_stage = -1;
@@ -216,96 +229,189 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
       reg_fence(acc);
       if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
 
-      // the epilogue of one 64-column accumulator chunk held in v
-      auto chunk = [&](const int c, float (&v)[64]) {
-        const int col0 = n_blk * BN + c * 64;
-        if (GEGLUT) {
-          // columns past N are zero accumulators (TMA zero-fills the missing W rows) and are clipped by the tensor map, rows past M too
-          float o[32];
-          epi.template geglu_chunk<true>(v, o, row, col0, valid && col0 < p.N);
-          const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
-          const int cc = c - c_first;                       // 0 / 1: left / right 64 bytes of the warp's 128-byte rows
-          if (cc == 0) { if (lane == 0) bulk_wait_read0(); __syncwarp(); }     // this warp's previous store has left the tile
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" :: "r"(wtile + (uint32_t)lane * 128u + (uint32_t)(((cc * 4 + j) ^ (lane & 7)) * 16)),
-                         "r"(pack_bf16(o[8 * j], o[8 * j + 1])), "r"(pack_bf16(o[8 * j + 2], o[8 * j + 3])),
-                         "r"(pack_bf16(o[8 * j + 4], o[8 * j + 5])), "r"(pack_bf16(o[8 * j + 6], o[8 * j + 7])) : "memory");
-          if (cc == 1) {
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) { tma_store_2d(&p.tma_out, wtile, (n_blk * BN + c_first * 64) >> 1, m_blk * TC_BM + quarter * 32); bulk_commit(); }
+      if constexpr (TILES) {
+        // ---- tile epilogues, from the accumulator fragments (layout above the kernel) ----
+        // acc[4 j + e] / acc[4 j + 2 + e] = rows fr / fr + 8 of the warp's 16 at column 8 j + 2 q + e of the tile; the boxes' rows are
+        // 128 bytes whose 16-byte chunk k sits at k ^ (row & 7), and (fr + 8) & 7 == fr
+        const int q = lane & 3, fr = lane >> 2;
+        const uint32_t rowa = (uint32_t)fr * 128u, rowb = rowa + 1024u;
+        // the next free 2 KB box of the warp's tile: the store two boxes back has read it
+        auto box_begin = [&]() {
+          if (lane == 0) bulk_wait_read1();
+          __syncwarp();
+          const uint32_t b = wtile + (nbox & 1u) * 2048u;
+          ++nbox;
+          return b;
+        };
+        // generic-proxy writes -> visible to the TMA (async-proxy) read
+        auto box_ready = [&]() { fence_proxy_async(); __syncwarp(); };
+        if constexpr (RED) {
+          // rows past M are zero accumulators and are clipped by the tensor map
+          float a0 = 0.f, b0 = 0.f, a1 = 0.f, b1 = 0.f;
+          if (RED_ADD && epi.kind == MMG_EPI_LNFOLD_RESIDUAL) {
+            a0 = __shfl_sync(0xffffffffu, ln_a, lane & ~3); b0 = __shfl_sync(0xffffffffu, ln_b, lane & ~3);
+            a1 = __shfl_sync(0xffffffffu, ln_a, (lane & ~3) | 1); b1 = __shfl_sync(0xffffffffu, ln_b, (lane & ~3) | 1);
           }
-        } else if (QKVT && col0 < p.N) {
-          int h;
-          const int which = epi.template qkv_chunk<true>(col0, v, h);
-          const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
-          const uint32_t rw = (uint32_t)(m_blk * TC_BM + quarter * 32), tok = (uint32_t)epi.p.tokens;
-          const uint32_t bq = rw / tok, t0 = rw - bq * tok;                       // warp-uniform: the 32 rows are tokens t0 .. t0+31 of sequence bq
-          const int64_t drow = which == 0 ? ((int64_t)bq * epi.p.heads + h) * epi.p.q_rows + t0
-                                          : ((int64_t)bq * epi.p.heads + h) * epi.p.kv_rows + epi.p.key_off + t0;
-          if (lane == 0) bulk_wait_read0();          // the store that last used this tile has read it
-          __syncwarp();
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" :: "r"(wtile + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) * 16)),
-                         "r"(pack_bf16(v[8 * j], v[8 * j + 1])), "r"(pack_bf16(v[8 * j + 2], v[8 * j + 3])),
-                         "r"(pack_bf16(v[8 * j + 4], v[8 * j + 5])), "r"(pack_bf16(v[8 * j + 6], v[8 * j + 7])) : "memory");
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) { tma_store_2d(&p.tma_qkv[which], wtile, 0, (int)drow); bulk_commit(); }
-          if (which != 0 && t0 == 0 && lane == 0) epi.qkv_null_row(which, bq, h);
-        } else if (RED && col0 < p.N) {
-          // rows past M hold garbage here and are clipped by the tensor map; the tile layout is the TMA 128-byte swizzle
-          if (RED_ADD) epi.resid_term(col0, v);
-          const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
+          for (int g = 0; g < BN / 32; ++g) {                 // one box = 32 fp32 columns
+            const int col = n_blk * BN + 32 * g;
+            const uint32_t box = box_begin();
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (lane == 0) bulk_wait_read0();             // this warp's previous push has left the tile
-            __syncwarp();
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" :: "r"(wtile + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) * 16)),
-                           "f"(v[32 * h + 4 * j]), "f"(v[32 * h + 4 * j + 1]), "f"(v[32 * h + 4 * j + 2]), "f"(v[32 * h + 4 * j + 3]) : "memory");
-            fence_proxy_async();                          // generic-proxy writes -> visible to the TMA (async-proxy) read
-            __syncwarp();
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * g + jj, c = col + 8 * jj + 2 * q;
+              float x0 = acc[4 * j], x1 = acc[4 * j + 1], y0 = acc[4 * j + 2], y1 = acc[4 * j + 3];
+              if (RED_ADD) {
+                x0 = epi.resid_term(x0, c, a0, b0); x1 = epi.resid_term(x1, c + 1, a0, b0);
+                y0 = epi.resid_term(y0, c, a1, b1); y1 = epi.resid_term(y1, c + 1, a1, b1);
+              }
+              const uint32_t off = (uint32_t)(((2 * jj + (q >> 1)) ^ fr) * 16 + 8 * (q & 1));
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" :: "r"(box + rowa + off), "f"(x0), "f"(x1) : "memory");
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" :: "r"(box + rowb + off), "f"(y0), "f"(y1) : "memory");
+            }
+            box_ready();
             if (lane == 0) {
-              if (RED_ADD) tma_reduce_add_2d(&p.tma_out, wtile, col0 + 32 * h, m_blk * TC_BM + quarter * 32);
-              else tma_store_2d(&p.tma_out, wtile, col0 + 32 * h, m_blk * TC_BM + quarter * 32);
+              if (RED_ADD) tma_reduce_add_2d(&p.tma_out, box, col, (int)brow);
+              else tma_store_2d(&p.tma_out, box, col, (int)brow);
               bulk_commit();
             }
           }
-        } else if (ACTT) {
-          if (valid && col0 < p.N) epi.apply_act(row, col0, v, 64);
-        } else if (valid && col0 < p.N) {
-          if (prefetch_resid) {
-            if (!EARLY_RESID) epi.load_resid(row, col0, rbuf);
-            epi.fuse_resid(col0, v, rbuf);
-            const int cn = col0 + c_step * 64;
-            if (EARLY_RESID && c + c_step < BN / 64 && cn < p.N) epi.load_resid(row, cn, rbuf);   // next chunk's residual overlaps the stores
-            epi.store_f32(row, col0, v);
-          } else {
-            epi.template apply<true>(row, col0, v, 64);
+        } else if constexpr (GEGLUT) {
+          // rows past M are zero accumulators and are clipped by the tensor map
+#pragma unroll
+          for (int bx = 0; bx < 2; ++bx) {                    // one box = chunks 2 bx, 2 bx + 1 = 64 bf16 outputs
+            const int col0 = n_blk * BN + 128 * bx;
+            const uint32_t box = box_begin();
+#pragma unroll
+            for (int cc = 0; cc < 2; ++cc) {
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {                // output columns 32 cc + 8 jj + 2 q + e = x column 8 jx + ..., gate column 8 jg + ...
+                const int jx = 8 * (2 * bx + cc) + jj, jg = jx + 4;
+                const uint32_t off = (uint32_t)(((4 * cc + jj) ^ fr) * 16 + 4 * q);
+                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowa + off),
+                             "r"(pack_bf16(acc[4 * jg] * gelu_fast(acc[4 * jx]), acc[4 * jg + 1] * gelu_fast(acc[4 * jx + 1]))) : "memory");
+                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowb + off),
+                             "r"(pack_bf16(acc[4 * jg + 2] * gelu_fast(acc[4 * jx + 2]), acc[4 * jg + 3] * gelu_fast(acc[4 * jx + 3]))) : "memory");
+              }
+            }
+            box_ready();
+            if (lane == 0) { tma_store_2d(&p.tma_out, box, col0 >> 1, (int)brow); bulk_commit(); }
+            if (epi.p.row_stats) {
+              // each chunk's (sum, sumsq) of its bf16 outputs in ascending column order (geglu_chunk's), read back from the box:
+              // lane l sums row l % 16 of chunk 2 bx + l / 16
+              const int rr = lane & 15, cc = lane >> 4, cs = col0 + 64 * cc;
+              if (brow + rr < p.M) {
+                float sx = 0.f, sq = 0.f;
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                  uint32_t w[4];
+                  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3])
+                               : "r"(box + (uint32_t)rr * 128u + (uint32_t)(((4 * cc + jj) ^ (rr & 7)) * 16)) : "memory");
+#pragma unroll
+                  for (int k = 0; k < 8; ++k) {
+                    const float t = __uint_as_float((k & 1) ? (w[k >> 1] & 0xffff0000u) : (w[k >> 1] << 16));
+                    sx += t; sq = fmaf(t, t, sq);
+                  }
+                }
+                reinterpret_cast<float2*>(epi.p.row_stats)[(brow + rr) * (int64_t)epi.p.stats_slots + (cs >> 6)] = make_float2(sx, sq);
+              }
+            }
+          }
+        } else if constexpr (QKVT) {
+          const uint32_t rw = (uint32_t)brow, tok = (uint32_t)epi.p.tokens;
+          const uint32_t bq = rw / tok, t0 = rw - bq * tok;   // warp-uniform: the 16 rows are tokens t0 .. t0+15 of sequence bq
+#pragma unroll
+          for (int c = 0; c < BN / 64; ++c) {                 // one box = one head chunk
+            const int col0 = n_blk * BN + 64 * c;
+            int h;
+            const int which = epi.qkv_head(col0, h);
+            const float* sc = which == 0 ? epi.p.q_scale : (which == 1 ? epi.p.k_scale : nullptr);
+            float t[32];                                      // t[2 jj + e]: row fr, t[16 + 2 jj + e]: row fr + 8, at head column 8 jj + 2 q + e
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) { t[2 * jj + e] = acc[4 * (8 * c + jj) + e]; t[16 + 2 * jj + e] = acc[4 * (8 * c + jj) + 2 + e]; }
+            if (sc) {
+              // qkv_chunk's sum of squares, bit for bit: chain k = i & 3 over ascending columns i, then (s0 + s1) + (s2 + s3).  Chain
+              // 2 (q & 1) + e of a row is columns 8 jj + 2 (q & 1) + e (lane q & 1) and + 4 (lane q | 2), jj ascending: lanes q < 2 run
+              // it for row fr, lanes q >= 2 for row fr + 8, each after fetching the other half from lane q ^ 2
+              const bool up = (q & 2) != 0;
+              float s[2] = {0.f, 0.f};
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float mine = up ? t[16 + 2 * jj + e] : t[2 * jj + e], give = up ? t[2 * jj + e] : t[16 + 2 * jj + e];
+                  const float got = __shfl_xor_sync(0xffffffffu, give, 2);
+                  const float lo = up ? got : mine, hi = up ? mine : got;
+                  s[e] = fmaf(lo, lo, s[e]);
+                  s[e] = fmaf(hi, hi, s[e]);
+                }
+              const float pair = s[0] + s[1];
+              const float ss = pair + __shfl_xor_sync(0xffffffffu, pair, 1);
+              const float inv = rsqrtf(fmaxf(ss, 1e-24f)), inv_x = __shfl_xor_sync(0xffffffffu, inv, 2);
+              const float i0 = up ? inv_x : inv, i1 = up ? inv : inv_x;
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float sv = sc[8 * jj + 2 * q + e];
+                  t[2 * jj + e] = t[2 * jj + e] * i0 * sv;
+                  t[16 + 2 * jj + e] = t[16 + 2 * jj + e] * i1 * sv;
+                }
+            }
+            const uint32_t box = box_begin();
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const uint32_t off = (uint32_t)((jj ^ fr) * 16 + 4 * q);
+              asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowa + off), "r"(pack_bf16(t[2 * jj], t[2 * jj + 1])) : "memory");
+              asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowb + off), "r"(pack_bf16(t[16 + 2 * jj], t[16 + 2 * jj + 1])) : "memory");
+            }
+            box_ready();
+            if (lane == 0) {
+              const int64_t drow = which == 0 ? ((int64_t)bq * epi.p.heads + h) * epi.p.q_rows + t0
+                                              : ((int64_t)bq * epi.p.heads + h) * epi.p.kv_rows + epi.p.key_off + t0;
+              tma_store_2d(&p.tma_qkv[which], box, 0, (int)drow);
+              bulk_commit();
+              if (which != 0 && t0 == 0) epi.qkv_null_row(which, bq, h);
+            }
           }
         }
-      };
+      } else {
+        // ---- register epilogues: columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread ----
+        // the epilogue of one 64-column accumulator chunk held in v
+        auto chunk = [&](const int c, float (&v)[64]) {
+          const int col0 = n_blk * BN + c * 64;
+          if (ACTT) {
+            if (valid && col0 < p.N) epi.apply_act(row, col0, v, 64);
+          } else if (valid && col0 < p.N) {
+            if (prefetch_resid) {
+              if (!EARLY_RESID) epi.load_resid(row, col0, rbuf);
+              epi.fuse_resid(col0, v, rbuf);
+              const int cn = col0 + c_step * 64;
+              if (EARLY_RESID && c + c_step < BN / 64 && cn < p.N) epi.load_resid(row, cn, rbuf);   // next chunk's residual overlaps the stores
+              epi.store_f32(row, col0, v);
+            } else {
+              epi.template apply<true>(row, col0, v, 64);
+            }
+          }
+        };
 #pragma unroll
-      for (int rd = 0; rd < ROUNDS; ++rd) {
-        // columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread
-        named_sync(1 + wg, 128);                   // the previous round's (tile's) readers are done with the staging buffer
-        stage_acc<BN / 2, TC_STG_LD>(acc, stg, 128 * rd, BN - 128 * rd < 128 ? BN - 128 * rd : 128);
-        named_sync(1 + wg, 128);
+        for (int rd = 0; rd < ROUNDS; ++rd) {
+          named_sync(1 + wg, 128);                   // the previous round's (tile's) readers are done with the staging buffer
+          stage_acc<BN / 2, TC_STG_LD>(acc, stg, 128 * rd, BN - 128 * rd < 128 ? BN - 128 * rd : 128);
+          named_sync(1 + wg, 128);
 #pragma unroll 1
-        for (int c = c_first; c < c_end; c += c_step) {
-          if (!mine) break;
-          if ((c >> 1) != rd) continue;
-          float v[64];
-          stage_ld32(my_row + (c & 1) * 64, v);
-          stage_ld32(my_row + (c & 1) * 64 + 32, v + 32);
-          chunk(c, v);
+          for (int c = c_first; c < c_end; c += c_step) {
+            if (!mine) break;
+            if ((c >> 1) != rd) continue;
+            float v[64];
+            stage_ld32(my_row + (c & 1) * 64, v);
+            stage_ld32(my_row + (c & 1) * 64 + 32, v + 32);
+            chunk(c, v);
+          }
         }
+        if (valid && mine) epi.end_row(row);
       }
-      if (valid && mine) epi.end_row(row);
     }
   }
 

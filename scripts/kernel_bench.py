@@ -1,9 +1,10 @@
 """Per-kernel microbenchmarks at the C3 (B=64) shapes: CUDA-event timing with an L2 flush between iterations, achieved
-TFLOP/s or GB/s against MEASURED_PEAKS.json.  Also the command ncu wraps (`--only <name>` runs one kernel a few times).
+TFLOP/s or GB/s against the H100 data sheet (or MEASURED_PEAKS.json).  Also the command ncu wraps (`--only <name>` runs one kernel a few times).
 usage: python scripts/kernel_bench.py [--only gemm|ln|sample|attn|conv|vq] [--iters 5]"""
 import argparse
 import json
 import os
+import subprocess
 import sys
 import torch
 
@@ -16,7 +17,9 @@ ap.add_argument("--only", default="")
 ap.add_argument("--iters", type=int, default=5)
 args = ap.parse_args()
 pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-PK_T, PK_B = pk.get("bf16_tflops", 1590.0), pk.get("hbm_gbs", 6650.0)
+# bench.py's figures: the H100 SXM data sheet (dense bf16, HBM3) unless MEASURED_PEAKS.json is present
+PK_T, PK_B = pk.get("bf16_tflops_sustained", pk.get("bf16_tflops", 989.0)), pk.get("hbm_gbs", 3350.0)
+PK_SRC = "measured" if pk else "H100 SXM data sheet"
 flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
 bf = torch.bfloat16
 
@@ -38,10 +41,10 @@ def report(name, ms, flops=None, bytes_=None):
     s = f"{name:58s} best {ms[0] * 1e3:9.1f} us  avg {ms[1] * 1e3:9.1f} us"
     if flops:
         t = flops / (ms[0] * 1e-3) / 1e12
-        s += f"  {t:8.1f} TFLOP/s ({t / PK_T:5.1%} of measured {PK_T:.0f})"
+        s += f"  {t:8.1f} TFLOP/s ({t / PK_T:5.1%} of {PK_T:.0f})"
     if bytes_:
         g = bytes_ / (ms[0] * 1e-3) / 1e9
-        s += f"  {g:8.1f} GB/s ({g / PK_B:5.1%} of measured {PK_B:.0f})"
+        s += f"  {g:8.1f} GB/s ({g / PK_B:5.1%} of {PK_B:.0f})"
     print(s, flush=True)
 
 
@@ -49,28 +52,92 @@ def want(k):
     return not args.only or k in args.only.split(",")
 
 
+def smi(q):
+    try:
+        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-i", str(torch.cuda.current_device())],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        return ""
+
+
+print(f"# {torch.cuda.get_device_name()}  nvidia-smi name, power.limit [W], clocks.max.sm [MHz]: {smi('name,power.limit,clocks.max.sm') or 'unavailable'}"
+      f"  peaks: {PK_T:.0f} TFLOP/s, {PK_B:.0f} GB/s ({PK_SRC})", flush=True)
+
 R = 2 * 64 * 256            # rows of a CFG decode step at B=64
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def tc_tile_n(M, N):
+    """The wgmma kernel's tile width for a tile epilogue (mmg_gemm.cu pick_bn)."""
+    mt = (M + 127) // 128
+    if N % 256 == 0 and mt * (N // 256) >= 2 * SMS:
+        return 256
+    if N % 128 == 0 and (mt * (N // 128) >= SMS or N >= 1024):
+        return 128
+    return 64 if (N % 64 == 0 and N % 128 != 0) else (128 if mt * ((N + 127) // 128) >= 96 else 64)
+
+
+def gemm_case(kind, M, N, K):
+    """Operands and the launch that generate() makes for one product (muse_maskgit.py _run_blocks / _ff_tail, the fused tail)."""
+    heads, n = 8, 256
+    a = torch.randn((M, K), device="cuda").to(bf); w = (torch.randn((N, K), device="cuda") * K ** -0.5).to(bf)
+    if kind == "qkv":           # self-attention: q, k, v heads, l2-normalised q / k, null k / v in key row 0
+        bh, tk = M // n * heads, (n + 1 + 7) // 8 * 8
+        q = torch.empty((bh, n, 64), device="cuda", dtype=bf); k = torch.zeros((bh, tk, 64), device="cuda", dtype=bf); v = torch.zeros_like(k)
+        qs, ks = torch.rand(64, device="cuda") + 0.5, torch.rand(64, device="cuda") + 0.5
+        nk, nv = torch.randn((heads, 64), device="cuda").to(bf), torch.randn((heads, 64), device="cuda").to(bf)
+        e = ops.qkv_epilogue(bf, heads, n, q=q, k=k, v=v, q_scale=qs, k_scale=ks, key_off=1, null_k=nk, null_v=nv)
+        # the epilogue block holds raw pointers: the closure keeps the tensors behind them alive
+        return lambda keep=(q, k, v, qs, ks, nk, nv): ops.linear(a, w, None, epilogue=ops.EPI_QKV, epi=e)
+    if kind == "q":             # cross-attention queries
+        q = torch.empty((M // n * heads, n, 64), device="cuda", dtype=bf); qs = torch.rand(64, device="cuda") + 0.5
+        e = ops.qkv_epilogue(bf, heads, n, q=q, q_scale=qs)
+        return lambda keep=(q, qs): ops.linear(a, w, None, epilogue=ops.EPI_QKV, epi=e)
+    if kind == "resid":         # to_out: x += ao @ W^T in place
+        x = torch.zeros((M, N), device="cuda")
+        return lambda: ops.linear(a, w, x, epilogue=ops.EPI_RESIDUAL, resid=x)
+    if kind == "geglu":         # FF1: GEGLU + per-chunk row statistics
+        h = torch.empty((M, N // 2), device="cuda", dtype=bf); st = torch.zeros((M, N // 64, 2), device="cuda")
+        return lambda: ops.linear(a, w, h, epilogue=ops.EPI_GEGLU, row_stats=st)
+    if kind == "lnfold":        # FF2: folded LayerNorm of h (statistics of FF1's 44 chunks) + residual, in place
+        x = torch.zeros((M, N), device="cuda"); st = torch.ones((M, 44, 2), device="cuda") * 31; cv = torch.randn(N, device="cuda")
+        return lambda: ops.linear(a, w, x, epilogue=ops.EPI_LNFOLD_RESIDUAL, bias=cv, resid=x, row_stats=st, ln_width=1365)
+    out = torch.empty((M, N), device="cuda")   # "tstore": the fused tail's sample GEMM, fp32 [rows, 4096] (contiguous W here)
+    return lambda: ops.linear(a, w, out)
+
+
 if want("gemm"):
-    for name, M, N, K, epi in [("qkv  M=32768 N=1536 K=512", R, 1536, 512, "store_bf16"), ("wo   M=32768 N=512 K=512 +resid", R, 512, 512, "resid"),
-                               ("ff1  M=32768 N=2816 K=512 geglu", R, 2816, 512, "geglu"), ("ff1  M=32768 N=2816 K=512 geglu+rowstats", R, 2816, 512, "geglu_stats"),
-                               ("ff2  M=32768 N=512 K=1408 +resid", R, 512, 1408, "resid"), ("ff2  M=32768 N=512 K=1408 lnfold+resid", R, 512, 1408, "lnfold"),
-                               ("logits M=10240 N=65536 K=512 fp32 out", 10240, 65536, 512, "store_f32"), ("logits M=16384 N=65536 K=512 fp32 out", 16384, 65536, 512, "store_f32"),
-                               ("logits M=64 N=65536 K=512 fp32 out", 64, 65536, 512, "store_f32"), ("square 8192^3 bf16 out", 8192, 8192, 8192, "store_bf16")]:
+    # the products generate() launches at C3, per layer, and a K sweep of each: time per call = tiles per CTA x (per-tile fixed cost +
+    # K / 64 x per-k-block cost).  The intercept is the epilogue + pipeline refill, the slope is set against the k-block at the
+    # data-sheet tensor rate (128 x BN x 64 x 2 FLOP at 4096 FLOP / cycle / SM).
+    for name, kind, M, N, K in [("qkv      (self)   ", "qkv", R, 1536, 512), ("to_out   (self)  +x", "resid", R, 512, 512),
+                                ("q        (cross)  ", "q", R // 2, 512, 512), ("to_out   (cross) +x", "resid", R // 2, 512, 512),
+                                ("ff1 geglu+stats   ", "geglu", R, 2816, 512), ("ff2 lnfold      +x", "lnfold", R, 512, 1408),
+                                ("tail sample f32   ", "tstore", 16384, 4096, 512)]:
+        bn = tc_tile_n(M, N)
+        tiles = (M + 127) // 128 * ((N + bn - 1) // bn)
+        per_cta = -(-tiles // min(tiles, SMS))
+        pts = []
+        for f in (1, 2, 4):
+            fn = gemm_case(kind, M, N, K * f)
+            ms = timeit(fn)
+            mhz = smi("clocks.sm")
+            report(f"gemm {name} M={M} N={N} K={K * f} BN={bn}", ms, flops=2.0 * M * N * K * f)
+            pts.append((K * f / 64, ms[0] * 1e3 / per_cta, float(mhz) if mhz.replace(".", "").isdigit() else float("nan")))
+            del fn
+            torch.cuda.empty_cache()
+        xs, ys = [p[0] for p in pts], [p[1] for p in pts]
+        xm, ym = sum(xs) / 3, sum(ys) / 3
+        slope = sum((x - xm) * (y - ym) for x, y in zip(xs, ys)) / sum((x - xm) ** 2 for x in xs)
+        icpt = ym - slope * xm
+        clk = min(p[2] for p in pts)
+        print(f"    K sweep: {per_cta} tiles/CTA  intercept {icpt:.2f} us/tile  slope {slope * 1e3:.1f} ns/k-block = {slope * clk:.0f} cycles at "
+              f"{clk:.0f} MHz (peak rate {128 * bn * 64 * 2 // 4096})", flush=True)
+    for name, M, N, K, odt in [("logits M=16384 N=65536 K=512 fp32 out", 16384, 65536, 512, torch.float32),
+                               ("logits M=64 N=65536 K=512 fp32 out", 64, 65536, 512, torch.float32), ("square 8192^3 bf16 out", 8192, 8192, 8192, bf)]:
         a = torch.randn((M, K), device="cuda").to(bf); w = (torch.randn((N, K), device="cuda") * K ** -0.5).to(bf)
-        if epi == "store_bf16":
-            out = torch.empty((M, N), device="cuda", dtype=bf); fn = lambda: ops.linear(a, w, out)
-        elif epi == "store_f32":
-            out = torch.empty((M, N), device="cuda"); fn = lambda: ops.linear(a, w, out)
-        elif epi == "resid":
-            out = torch.zeros((M, N), device="cuda"); fn = lambda: ops.linear(a, w, out, epilogue=ops.EPI_RESIDUAL, resid=out)
-        elif epi == "geglu_stats":
-            out = torch.empty((M, N // 2), device="cuda", dtype=bf); st = torch.zeros((M, N // 64, 2), device="cuda"); fn = lambda: ops.linear(a, w, out, epilogue=ops.EPI_GEGLU, row_stats=st)
-        elif epi == "lnfold":
-            out = torch.zeros((M, N), device="cuda"); st = torch.ones((M, K // 32, 2), device="cuda") * 31; cv = torch.zeros(N, device="cuda")
-            fn = lambda: ops.linear(a, w, out, epilogue=ops.EPI_LNFOLD_RESIDUAL, bias=cv, resid=out, row_stats=st, ln_width=1365)
-        else:
-            out = torch.empty((M, N // 2), device="cuda", dtype=bf); e = ops._epi(out, N // 2); fn = lambda: ops.linear(a, w, None, epilogue=ops.EPI_GEGLU, epi=e)
-        report("gemm " + name, timeit(fn), flops=2.0 * M * N * K)
+        out = torch.empty((M, N), device="cuda", dtype=odt)
+        report("gemm " + name, timeit(lambda: ops.linear(a, w, out)), flops=2.0 * M * N * K)
         del a, w, out
 
 if want("ln"):
