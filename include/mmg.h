@@ -210,6 +210,21 @@ typedef struct {
 } mmg_remask_args;
 int mmg_remask(const mmg_remask_args* a, void* stream);
 
+/* re-mask with frozen positions and a count per batch row (MaskGit.inpaint).  Row b ranks the scores of its non-frozen
+ * positions only (ties: lowest position first) and selects c_b = min(num_masked[b], rows) of them: mask_id is written
+ * there, every score of the row is set to -1e5, masked_pos[b, 0 .. c_b) gets the ascending selected positions and
+ * masked_pos[b, c_b .. rows) the row's first frozen position (pad rows).  rows is the step's largest count over the batch;
+ * a row with a smaller count must have a frozen position, so that with `only_masked` the sampler computes its pad rows but
+ * writes no id for them, and their scores land on a position the next re-mask ignores.  num_masked is read on the device
+ * (one launch per step, no host synchronisation).                                                                      */
+typedef struct {
+  int64_t* ids; float* scores; int32_t* masked_pos;   /* [B, n], [B, n], [B, rows]                                 */
+  const uint8_t* frozen;                              /* [B, n], 1 = keep                                          */
+  const int32_t* num_masked;                          /* [B] device counts for this step, each <= rows             */
+  int32_t B, n, rows; int64_t mask_id;
+} mmg_remask_frozen_args;
+int mmg_remask_frozen(const mmg_remask_frozen_args* a, void* stream);
+
 /* Final LayerNorm + classifier-free-guidance combine on the masked rows only, in embedding space:
  *   e[j] = LN(x_null[r]) + (LN(x_cond[r]) - LN(x_null[r])) * cond_scale,  r = b*n + masked_pos[b, j]
  * (to_logits is linear and bias-free, so W e == null + (cond - null) * scale of muse_maskgit_pytorch.py:254).    */

@@ -69,6 +69,11 @@ class RemaskArgs(C.Structure):
                 ("mask_id", i64)]
 
 
+class RemaskFrozenArgs(C.Structure):
+    _fields_ = [("ids", vp), ("scores", vp), ("masked_pos", vp), ("frozen", vp), ("num_masked", vp), ("B", i32), ("n", i32), ("rows", i32),
+                ("mask_id", i64)]
+
+
 class FinalEmbedArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("masked_pos", vp), ("e", vp), ("e_dtype", i32),
                 ("B", i32), ("n", i32), ("num_masked", i32), ("dim", i32), ("cond_scale", f32)]
@@ -153,7 +158,7 @@ EXPORTS = {
     "mmg_logits_sample": LogitsSampleArgs, "mmg_vq_lfq_encode": LfqEncodeArgs, "mmg_vq_l2_argmin": L2ArgminArgs,
     "mmg_vq_decode_codes": DecodeCodesArgs, "mmg_cast": CastArgs, "mmg_split3": Split3Args, "mmg_critic_score": CriticScoreArgs,
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,
-    "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs,
+    "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs,
 }
 PLAIN_EXPORTS = ("mmg_version", "mmg_last_error", "mmg_launch_count", "mmg_sizeof", "mmg_decode_step_workspace_bytes", "mmg_logits_fused_workspace_bytes",
                  "mmg_simt_fallback_count", "mmg_simt_launch_count")

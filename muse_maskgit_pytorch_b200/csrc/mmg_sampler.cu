@@ -369,20 +369,26 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // re-mask: per batch row pick the num_masked largest scores (ties: lowest position), scatter mask_id, reset scores.
+// FROZEN (inpainting): positions with frozen[b, i] != 0 are neither ranked nor selected; row b selects
+// min(num_masked_dev[b], rows) positions and pads masked_pos[b, c_b .. rows) with its first frozen position.
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-remask_kernel(int64_t* __restrict__ ids, float* __restrict__ scores, int32_t* __restrict__ masked_pos, int n, int num_masked, int64_t mask_id) {
-  extern __shared__ float sc[];                       // [n] scores, then [n] flags (as int)
-  int* flag = reinterpret_cast<int*>(sc + n);
-  __shared__ int woff[9];
-  pdl_wait(); pdl_trigger();
+template <bool FROZEN>
+__device__ __forceinline__ void remask_row(int64_t* __restrict__ ids, float* __restrict__ scores, int32_t* __restrict__ masked_pos,
+                                           const uint8_t* __restrict__ frozen, int n, int num_masked, int rows, int64_t mask_id,
+                                           float* sc, int* flag, uint8_t* fz, int* woff) {
   const int b = blockIdx.x, tid = threadIdx.x;
   for (int i = tid; i < n; i += 256) sc[i] = scores[(int64_t)b * n + i];
+  if (FROZEN) for (int i = tid; i < n; i += 256) fz[i] = frozen[(int64_t)b * n + i] != 0;
   __syncthreads();
   for (int i = tid; i < n; i += 256) {
     const float s = sc[i]; int rank = 0;
-    for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += (t > s) || (t == s && j < i); }
-    flag[i] = rank < num_masked;
+    if (FROZEN) {
+      for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += !fz[j] && ((t > s) || (t == s && j < i)); }
+      flag[i] = !fz[i] && rank < num_masked;
+    } else {
+      for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += (t > s) || (t == s && j < i); }
+      flag[i] = rank < num_masked;
+    }
   }
   __syncthreads();
   // ordered compaction: each thread owns a contiguous chunk
@@ -400,9 +406,38 @@ remask_kernel(int64_t* __restrict__ ids, float* __restrict__ scores, int32_t* __
   __syncthreads();
   int o = woff[warp] + incl - c;
   for (int i = lo; i < hi; ++i) {
-    if (flag[i]) { masked_pos[(int64_t)b * num_masked + o++] = i; ids[(int64_t)b * n + i] = mask_id; }
+    if (flag[i]) { masked_pos[(int64_t)b * rows + o++] = i; ids[(int64_t)b * n + i] = mask_id; }
     scores[(int64_t)b * n + i] = -1e5f;
   }
+  if (FROZEN) {
+    // pad rows: the sampler computes them but (only_masked) writes no id at a frozen position, and every pad row of this image computes
+    // the same value, so the repeated score writes are deterministic.  An image without frozen positions has count == rows (mmg.h).
+    const int selected = woff[8];
+    if (selected < rows) {
+      int first = n;
+      for (int i = 0; i < n; ++i) if (fz[i]) { first = i; break; }
+      for (int r = selected + tid; r < rows; r += 256) masked_pos[(int64_t)b * rows + r] = first < n ? first : 0;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256)
+remask_kernel(int64_t* __restrict__ ids, float* __restrict__ scores, int32_t* __restrict__ masked_pos, int n, int num_masked, int64_t mask_id) {
+  extern __shared__ float sc[];                       // [n] scores, then [n] flags (as int)
+  __shared__ int woff[9];
+  pdl_wait(); pdl_trigger();
+  remask_row<false>(ids, scores, masked_pos, nullptr, n, num_masked, num_masked, mask_id, sc, reinterpret_cast<int*>(sc + n), nullptr, woff);
+}
+
+__global__ void __launch_bounds__(256)
+remask_frozen_kernel(const mmg_remask_frozen_args a) {
+  extern __shared__ float sc[];                       // [n] scores, [n] flags (as int), [n] frozen bytes
+  __shared__ int woff[9];
+  pdl_wait(); pdl_trigger();
+  const int count = a.num_masked[blockIdx.x];
+  const int limit = count < a.rows ? (count > 0 ? count : 0) : a.rows;
+  remask_row<true>(a.ids, a.scores, a.masked_pos, a.frozen, a.n, limit, a.rows, a.mask_id, sc, reinterpret_cast<int*>(sc + a.n),
+                   reinterpret_cast<uint8_t*>(sc + 2 * a.n), woff);
 }
 
 
@@ -489,6 +524,19 @@ extern "C" int mmg_remask(const mmg_remask_args* a, void* stream) {
   MMG_CHECK_ARG(a->n > 0 && a->num_masked >= 1 && a->num_masked <= a->n && a->n <= 16384, "mmg_remask: n=%d num_masked=%d", a->n, a->num_masked);
   if (a->B == 0) return MMG_OK;
   MMG_CUDA(launch_pdl(remask_kernel, dim3(a->B), dim3(256), (size_t)a->n * 8, st, a->ids, a->scores, a->masked_pos, a->n, a->num_masked, a->mask_id));
+  MMG_LAUNCHED();
+  return MMG_OK;
+}
+
+extern "C" int mmg_remask_frozen(const mmg_remask_frozen_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->ids && a->scores && a->masked_pos && a->frozen && a->num_masked, "mmg_remask_frozen: NULL pointer");
+  MMG_CHECK_ARG(a->B >= 0 && a->n > 0 && a->rows >= 1 && a->rows <= a->n && a->n <= 16384, "mmg_remask_frozen: B=%d n=%d rows=%d", a->B, a->n, a->rows);
+  if (a->B == 0) return MMG_OK;
+  const size_t smem = (size_t)a->n * 9;                 // scores, flags, frozen bytes
+  static const cudaError_t attr = cudaFuncSetAttribute(remask_frozen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 9);
+  if (attr != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(remask_frozen): %s", cudaGetErrorString(attr));
+  MMG_CUDA(launch_pdl(remask_frozen_kernel, dim3(a->B), dim3(256), smem, st, *a));
   MMG_LAUNCHED();
   return MMG_OK;
 }

@@ -431,6 +431,32 @@ def cosine_schedule(t):
     return torch.cos(t * math.pi * 0.5)
 
 
+def regen_tokens(mask, b, image_size, fmap_size):
+    """Inpainting mask -> (b, fmap_size, fmap_size) bool, True = regenerate the token.  `mask` is bool or {0, 1}, True = regenerate, at pixel
+    resolution ((b, H, W) or (b, 1, H, W), H = W = image_size) or at token resolution ((b, fmap_size, fmap_size)).  A token is regenerated when
+    any pixel of its patch is masked."""
+    if not isinstance(mask, torch.Tensor):
+        raise TypeError(f"mask must be a torch.Tensor, got {type(mask).__name__}")
+    if mask.dtype != torch.bool:
+        if mask.is_complex() or not ((mask == 0) | (mask == 1)).all():
+            raise ValueError("mask must be bool or hold only the values 0 and 1")
+        mask = mask != 0
+    if mask.dim() == 4:
+        if mask.shape[1] != 1:
+            raise ValueError(f"a 4-d mask must be (b, 1, H, W), got {tuple(mask.shape)}")
+        mask = mask[:, 0]
+    f = fmap_size
+    if mask.dim() != 3 or mask.shape[0] != b or mask.shape[1:] not in ((image_size, image_size), (f, f)):
+        raise ValueError(f"mask must be (b, H, W), (b, 1, H, W) with H = W = image_size = {image_size}, or (b, f, f) with f = fmap_size = {f}, "
+                         f"for b = {b}; got {tuple(mask.shape)}")
+    if mask.shape[1] == f:
+        return mask
+    p = image_size // f
+    if p * f != image_size:
+        raise ValueError(f"image_size {image_size} is not a multiple of fmap_size {f}: pass the mask at token resolution")
+    return mask.reshape(b, f, p, f, p).any(dim=4).any(dim=2)
+
+
 # ------------------------------------------------------------------------------------------------ MaskGit
 class MaskGit(nn.Module):
     def __init__(self, image_size, transformer: MaskGitTransformer, noise_schedule: Callable = cosine_schedule,
@@ -507,8 +533,46 @@ class MaskGit(nn.Module):
         finally:
             self.train(was_training)
 
+    @torch.no_grad()
+    def inpaint(self, texts: List[str], images: torch.Tensor, mask: torch.Tensor, cond_images: Optional[torch.Tensor] = None, temperature=1.,
+                topk_filter_thres=0.9, can_remask_prev_masked=False, force_not_use_token_critic=False, timesteps=18, cond_scale=3,
+                critic_noise_scale=1, return_ids=False):
+        """Regenerates the masked region of `images` and keeps the rest (an extension: the reference has no inpainting).
+
+        images: fp32 NCHW (b, C, image_size, image_size), as `vae.encode` takes them.  mask: bool or {0, 1}, True = regenerate, either
+        (b, H, W) / (b, 1, H, W) at pixel resolution or (b, f, f) at token resolution (f = fmap_size); a token is regenerated when any pixel
+        of its patch is masked.  Outpainting is the same call on a canvas whose border is masked.
+
+        The tokens start as vae.encode_ids(images) with mask_id at the regenerated positions, which decode as in generate() except that
+        each image re-masks only among its own regenerated tokens, on its own schedule max(int(noise_schedule(t) * N_b), 1) (N_b = its
+        number of regenerated tokens, 0 when it has none).  Every other token id equals the encoded one bit for bit.  The pixels are
+        vae.decode_from_ids(ids): the unmasked region is the VAE reconstruction, not the input pixels; pasting the input back is the
+        caller's job.  With every token masked the result equals generate() under the same seed or injected noise.
+        Returns what generate() returns.  `use_native_step` does not apply here (mmg_decode_step has no frozen positions)."""
+        b = len(texts)
+        device = next(self.parameters()).device
+        fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
+        if not isinstance(images, torch.Tensor) or tuple(images.shape) != (b, self.vae.channels, self.image_size, self.image_size):
+            raise ValueError(f"images must be a (b, {self.vae.channels}, {self.image_size}, {self.image_size}) tensor for b = {b} texts, got "
+                             f"{tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__}")
+        regen = regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1)
+        counts = [int(c) for c in regen.sum(dim=1).tolist()]                      # N_b: the call's one device-to-host read for a GPU mask
+        n_max = max(counts, default=0)
+        table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in counts]
+        inp = dict(n_max=n_max,
+                   dev=dict(images=images.to(device, torch.float32).contiguous(),
+                            frozen=(~regen).to(device=device, dtype=torch.uint8).contiguous(),
+                            counts=torch.tensor(table, dtype=torch.int32).t().contiguous().to(device)))       # [timesteps, b]
+        was_training = self.training
+        self.eval()
+        try:
+            return self._generate(texts, None, cond_images, None, temperature, topk_filter_thres, can_remask_prev_masked,
+                                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, inpaint=inp)
+        finally:
+            self.train(was_training)
+
     def _generate(self, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
-                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, seed=None):
+                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, seed=None, inpaint=None):
         tr = self.transformer
         if negative_texts is not None:
             raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
@@ -545,18 +609,26 @@ class MaskGit(nn.Module):
         body = partial(self._generate_body, fmap_size=fmap_size, temperature=temperature, topk_filter_thres=topk_filter_thres,
                        timesteps=timesteps, cond_scale=cond_scale, b=b, use_critic=use_critic, critic_noise_scale=critic_noise_scale,
                        score_all=bool(can_remask_prev_masked) and not use_critic, aten=aten)
+        if inpaint is not None:
+            body = partial(body, inpaint_rows=inpaint["n_max"])
+        inp_dev = None if inpaint is None else inpaint["dev"]
+        inp_kw = lambda d: {} if inpaint is None else dict(inpaint=d)
+        rerun = lambda: self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres,
+                                               can_remask_prev_masked, force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale,
+                                               return_ids, **inp_kw(inpaint))
         critic_net = self.token_critic if isinstance(self.token_critic, Transformer) and use_critic else None
         if not self.use_cuda_graph or self.sampler_noise_fn is not None:
-            images, ids, status = body(text_embeds, cond_images)
+            images, ids, status = body(text_embeds, cond_images, **inp_kw(inp_dev))
             if self._fused_tail_overflowed(status):
-                return self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
-                                              force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids)
+                return rerun()
             return (images, ids) if return_ids else images
         # ---- whole-call CUDA graph: 18 decode steps + VAE decode replayed as one launch (no per-kernel host work) ----
         key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), fmap_size,
                float(temperature), float(topk_filter_thres), int(timesteps), float(cond_scale), int(self.row_offset), tr.precision, self.vae.precision,
                use_critic, float(critic_noise_scale), bool(can_remask_prev_masked), None if aten is None else aten["key"], bool(self.use_native_step),
                id(self.noise_schedule), bool(self.use_fused_tail))
+        if inpaint is not None:
+            key += (("inpaint", inpaint["n_max"]),)
         pack_ids = lambda: (id(tr._pack), id(self.vae._pack), id(self.cond_vae._pack), id(critic_net._pack) if critic_net is not None else 0,
                             id(self.token_critic._head_cache) if isinstance(self.token_critic, SelfCritic) else 0)
         entry = self._graphs.get(key)
@@ -565,16 +637,17 @@ class MaskGit(nn.Module):
         if entry is None:
             te_s = text_embeds.clone()
             ci_s = None if cond_images is None else cond_images.clone()
-            body(te_s, ci_s)                                   # eager warm-up: lazy packing, workspaces, function attributes
+            inp_s = None if inp_dev is None else {k: v.clone() for k, v in inp_dev.items()}     # images, frozen, count table
+            body(te_s, ci_s, **inp_kw(inp_s))                  # eager warm-up: lazy packing, workspaces, function attributes
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                out_images, out_ids, out_status = body(te_s, ci_s)
+                out_images, out_ids, out_status = body(te_s, ci_s, **inp_kw(inp_s))
             # the entry keeps alive everything the captured kernels point at (packed weights, workspaces)
             entry = (graph, te_s, ci_s, out_images, (out_ids, out_status), pack_ids(),
                      (tr._pack, self.vae._pack, self.cond_vae._pack, dict(getattr(tr, "_ws", {})),
                       None if critic_net is None else (critic_net._pack, dict(getattr(critic_net, "_ws", {}))),
-                      self.token_critic._head_cache if isinstance(self.token_critic, SelfCritic) else None))
+                      self.token_critic._head_cache if isinstance(self.token_critic, SelfCritic) else None), inp_s)
             if len(self._graphs) >= 4:
                 self._graphs.pop(next(iter(self._graphs)))       # least recently used (hits are moved to the end below)
         self._graphs.pop(key, None)
@@ -583,11 +656,13 @@ class MaskGit(nn.Module):
         te_s.copy_(text_embeds, non_blocking=True)
         if ci_s is not None:
             ci_s.copy_(cond_images, non_blocking=True)
+        if inp_dev is not None:
+            for k, v in entry[7].items():
+                v.copy_(inp_dev[k], non_blocking=True)
         graph.replay()
         images, ids = out_images.clone(), out_ids.clone()
         if self._fused_tail_overflowed(out_status):
-            return self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
-                                          force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids)
+            return rerun()
         return (images, ids) if return_ids else images
 
     def _fused_tail_overflowed(self, status):
@@ -598,16 +673,16 @@ class MaskGit(nn.Module):
         self.last_fused_fallback_rows, overflow = (int(v) for v in status.tolist())
         return overflow != 0
 
-    def _generate_unfused(self, seed, *args):
-        """Repeats a generate() call whose fused tail overflowed on the materialised path, with the same noise: the same libmmg seed, or the
-        ATen generator position the failed attempt started from."""
+    def _generate_unfused(self, seed, *args, **kw):
+        """Repeats a generate() / inpaint() call whose fused tail overflowed on the materialised path, with the same noise: the same libmmg
+        seed, or the ATen generator position the failed attempt started from."""
         saved = self.use_fused_tail
         self.use_fused_tail = False
         try:
             if self.sampler_rng == "aten" and self.sampler_noise_fn is None:       # re-read the generator position the failed attempt consumed
                 gen = torch.cuda.default_generators[next(self.parameters()).device.index or 0]
                 gen.set_offset(self._aten_start_offset)
-            return self._generate(*args, seed=seed)
+            return self._generate(*args, seed=seed, **kw)
         finally:
             self.use_fused_tail = saved
 
@@ -703,8 +778,10 @@ class MaskGit(nn.Module):
         ops.logits_sample(lg, pos, ids, scores, rows_b, k_keep, temp, **kw)
 
     def _generate_body(self, text_embeds, cond_images, *, fmap_size, temperature, topk_filter_thres, timesteps, cond_scale, b,
-                       use_critic=False, critic_noise_scale=1., score_all=False, aten=None):
-        """The device-side work of generate(): no host synchronisation, no data-dependent host control flow."""
+                       use_critic=False, critic_noise_scale=1., score_all=False, aten=None, inpaint=None, inpaint_rows=None):
+        """The device-side work of generate(): no host synchronisation, no data-dependent host control flow.
+        inpaint (inpaint()): dict(images, frozen uint8 [b, n], counts int32 [timesteps, b]) device tensors; inpaint_rows = the largest
+        number of regenerated tokens of an image, whose schedule gives the rows sampled per step (pad rows fill the smaller counts)."""
         tr = self.transformer
         device = text_embeds.device
         n = fmap_size ** 2
@@ -714,15 +791,18 @@ class MaskGit(nn.Module):
         ctx = tr._prepare_context(text_embeds, cond_ids, [False, True][:nb])
         P = tr._packed()
         adt = P["adt"]
-        ids = torch.full((b, n), self.mask_id, dtype=torch.long, device=device)
+        if inpaint is None:
+            ids = torch.full((b, n), self.mask_id, dtype=torch.long, device=device)
+        else:
+            ids = self.vae.encode_ids(inpaint["images"]).reshape(b, n).masked_fill(inpaint["frozen"] == 0, self.mask_id)
         scores = torch.zeros((b, n), dtype=torch.float32, device=device)
         masked_pos = torch.empty((b, n), dtype=torch.int32, device=device)
         k_keep = math.ceil((1 - topk_filter_thres) * V)                        # muse_maskgit_pytorch.py:414
-        sched = self.mask_schedule(n, timesteps)
+        sched = self.mask_schedule(n if inpaint is None else inpaint_rows, timesteps)
         bn = b * n
         native = None
         if (self.use_native_step and adt == torch.bfloat16 and not self.self_cond and not use_critic and not score_all and aten is None
-                and all("w2f" in l["ff"] for l in P["layers"])):
+                and inpaint is None and all("w2f" in l["ff"] for l in P["layers"])):
             native = self._native_step_setup(ctx, P, b, n, nb, max(sched), V, device)
         rows_max = n if score_all else max(sched)
         tail = self._tail_buffers(b, n, rows_max, V, device, k_keep) if native is None else None
@@ -757,7 +837,10 @@ class MaskGit(nn.Module):
                 a.u = None if u is None else u.data_ptr(); a.seed = 0; a.seed_dev = self._seed_dev.data_ptr(); a.row_offset = self.row_offset * n
                 _lib.call("mmg_decode_step", a)
                 continue
-            ops.remask(ids, scores, masked_pos, num_masked, self.mask_id)
+            if inpaint is None:
+                ops.remask(ids, scores, masked_pos, num_masked, self.mask_id)
+            else:      # each image re-masks among its own regenerated tokens; num_masked rows per image, the surplus padded
+                ops.remask_frozen(ids, scores, masked_pos, inpaint["frozen"], inpaint["counts"][step], num_masked, self.mask_id)
             x = tr._run_blocks(ids, ctx, nb, sc_embed if (self.self_cond and step > 0) else None)
             if self.self_cond:                                                 # embed of the conditional forward, fed back next step (:574)
                 ops.layernorm(x[:bn], P["gf"], sc_embed)
@@ -769,7 +852,7 @@ class MaskGit(nn.Module):
                 u = self.sampler_noise_fn(step, (b, n, V)).to(device=device, dtype=torch.float32).contiguous()
             seed_dev = self._seed_dev if aten is None else self._aten_dev[0:1]
             self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(cond_scale), k_keep, tail, seed_dev=seed_dev,
-                              only_masked_id=self.mask_id if score_all else None,
+                              only_masked_id=self.mask_id if score_all or inpaint is not None else None,
                               aten=None if aten is None else (step * aten["per_step"], self._aten_dev[1:2], aten["stride_g"]))
             if use_critic:
                 xc = cnet._run_blocks(ids, cctx, cnb)

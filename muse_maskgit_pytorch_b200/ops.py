@@ -229,6 +229,19 @@ def remask(ids, scores, masked_pos, num_masked, mask_id):
     L.call("mmg_remask", a)
 
 
+def remask_frozen(ids, scores, masked_pos, frozen, num_masked, rows, mask_id):
+    """remask over the non-frozen positions with a device count per sequence: frozen uint8 [B, n] (1 = keep), num_masked int32 [B];
+    masked_pos [B, rows] gets each sequence's selected positions, padded with its first frozen position."""
+    _chk(ids, "ids"); _chk(scores, "scores"); _chk(masked_pos, "masked_pos"); _chk(frozen, "frozen"); _chk(num_masked, "num_masked")
+    assert frozen.dtype == torch.uint8 and frozen.shape == ids.shape and num_masked.dtype == torch.int32 and num_masked.numel() == ids.shape[0]
+    assert masked_pos.dtype == torch.int32 and masked_pos.numel() >= ids.shape[0] * rows
+    a = L.RemaskFrozenArgs()
+    a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.masked_pos = masked_pos.data_ptr()
+    a.frozen = frozen.data_ptr(); a.num_masked = num_masked.data_ptr()
+    a.B, a.n = ids.shape; a.rows = rows; a.mask_id = mask_id
+    L.call("mmg_remask_frozen", a)
+
+
 def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_scale):
     a = L.FinalEmbedArgs()
     a.x_cond = x_cond.data_ptr(); a.x_null = L.ptr(x_null); a.gamma = gamma.data_ptr(); a.masked_pos = masked_pos.data_ptr()

@@ -24,4 +24,5 @@ runall aten_rng 600 tests/test_gpu_aten_rng.py
 runall full_config 900 tests/test_gpu_full_config.py
 runall fused_tail 600 tests/test_gpu_fused_tail.py
 runall t5 900 tests/test_gpu_t5.py
+runall inpaint 900 tests/test_gpu_inpaint.py
 cat $OUT/summary.txt
