@@ -19,6 +19,7 @@
 #include "mmg_tmap.cuh"
 #include "mmg_sampler.cuh"
 #include <mutex>
+#include <type_traits>
 
 namespace mmg {
 
@@ -31,19 +32,58 @@ constexpr int LF_FIFO = 32;                 // candidate entries of the per-thre
 constexpr int LF_FB_CAP = 128;              // rows per step that may take the materialised fallback
 constexpr int LF_MAX_SPLITS = 64;
 constexpr int LF_A_BYTES = LF_BM * LF_BK * 2, LF_B_BYTES = LF_BN * LF_BK * 2;
-constexpr int LF_STG_LD = LF_BN + 4;        // accumulator staging row stride (floats)
+constexpr int LF_SLICES = 5;                // epilogue slices of a tile run between the next tile's k-blocks (4 x 16 columns, then the drains)
 
-// Shared memory: the candidate FIFOs (64 KB) and the accumulator staging (2 x 64 x 132 fp32) leave room for two 32 KB operand stages
-// within the 227 KB of a block: the tile is 128 x 128.
+// Shared memory: the epilogue runs from the accumulator registers, so next to the candidate FIFOs (64 KB) there is room for four 32 KB
+// operand stages within the 227 KB of a block: 1 KB alignment + 128 KB ring + 8 KB barriers / padding + 64 KB FIFOs = 201 KB.
 struct LfCfg {
   static constexpr int STAGE_BYTES = LF_A_BYTES + LF_B_BYTES;
   static constexpr int FIFO_BYTES = LF_EPI_WARPS * LF_FIFO * 32 * 8;
-  static constexpr int STG_BYTES = 2 * 64 * LF_STG_LD * 4;
-  static constexpr int STAGES = 2;
-  // [<= 1 KB to align][operand ring][barriers + padding up to the next 8 KB boundary][FIFO region, 8 KB aligned like its per-warp stride][staging]
-  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 8192 + FIFO_BYTES + STG_BYTES;
+  static constexpr int STAGES = 4;
+  // [<= 1 KB to align][operand ring][barriers + padding up to the next 8 KB boundary][FIFO region, 8 KB aligned like its per-warp stride]
+  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 8192 + FIFO_BYTES;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
+
+// Fragment -> chunk hand-over.  In the m64n128k16 accumulator fragment the lane quad q = lane % 4 of a row group holds rows r0 and r0 + 8
+// (r0 = 16 warp + lane / 4) x both 64-column halves, 16 values of each (row, half) chunk per lane: columns 8 j + 2 q + e (j < 8, e < 2) of
+// the half.  Chunk c = 2 half + (row == r0 + 8) belongs to lane c of the quad.  Block (s, kk) below is the 16 values kk = 2 j + e of chunk
+// (or, after the exchange, source lane) s: fragment register lf_frag(s, kk).
+__host__ __device__ constexpr int lf_frag(int s, int kk) { return 32 * (s >> 1) + 4 * (kk >> 1) + 2 * (s & 1) + (kk & 1); }
+
+// blocks s <-> s ^ x for every s (a lane-dependent permutation: two selects per pair of registers)
+__device__ __forceinline__ void lf_xor_blocks(float (&d)[64], int x) {
+#pragma unroll
+  for (int bit = 1; bit <= 2; bit <<= 1) {
+    const bool sw = (x & bit) != 0;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      if (s & bit) continue;
+#pragma unroll
+      for (int kk = 0; kk < 16; ++kk) {
+        const float a = d[lf_frag(s, kk)], b = d[lf_frag(s | bit, kk)];
+        d[lf_frag(s, kk)] = sw ? b : a; d[lf_frag(s | bit, kk)] = sw ? a : b;
+      }
+    }
+  }
+}
+
+// 4 x 4 block transpose inside the quad, from the accumulators acc (left as they are: the next tile's wgmma owns them) into v: afterwards
+// block s of v holds chunk q's 16 values from source lane s, so that the chunk's column i = 8 j + 2 s + e is v[lf_frag(s, 2 j + e)]
+// (lf_col below).  Block m first holds the lane's share of chunk q ^ m (sent to lane q ^ m by the xor-m shuffle, which brings back lane
+// q ^ m's share of chunk q), then block s takes the share of lane s.
+__device__ __forceinline__ void lf_quad_transpose(const float (&acc)[64], float (&v)[64], int q) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) v[i] = acc[i];
+  lf_xor_blocks(v, q);
+#pragma unroll
+  for (int m = 1; m < 4; ++m)
+#pragma unroll
+    for (int kk = 0; kk < 16; ++kk) v[lf_frag(m, kk)] = __shfl_xor_sync(0xffffffffu, v[lf_frag(m, kk)], m);
+  lf_xor_blocks(v, q);
+}
+// register of column i (0..63) of the lane's chunk after lf_quad_transpose
+__host__ __device__ constexpr int lf_col(int i) { return lf_frag((i >> 1) & 3, 2 * (i >> 3) + (i & 1)); }
 
 struct alignas(64) LfParams {
   CUtensorMap tma_a, tma_b;
@@ -66,7 +106,6 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
   // FIFO region: aligned (in the shared-memory window) to its 8 KB per-warp stride, so that a thread's slot address is base | slot << 8
   uint8_t* fifo_all = smem + STAGES * STAGE_BYTES + 256;
   fifo_all += (8192u - (smem_u32(fifo_all) & 8191u)) & 8191u;
-  float* staging = reinterpret_cast<float*>(fifo_all + Cfg::FIFO_BYTES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_items = p.num_pm * p.S;
@@ -107,11 +146,9 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
     // ===================== consumer warpgroups: wgmma on 64 rows each, then one thread = one row x one 64-column chunk per tile =====================
     constexpr float LOG2E = 1.4426950408889634f;
     const int wg = (warp - 4) >> 2, wq = warp & 3;
-    const int quarter = 2 * wg + (wq & 1);        // this warp's 32 rows of the tile, inside its warpgroup's 64
-    const int half = wq >> 1;                     // the 64-column chunk of every tile this warp takes
-    const int r_in_tile = quarter * 32 + lane;
-    float* stg = staging + wg * 64 * LF_STG_LD;
-    const float* my_row = stg + ((wq & 1) * 32 + lane) * LF_STG_LD + half * 64;
+    const int q = lane & 3;                       // the lane's chunk of its quad's rows (lf_quad_transpose)
+    const int half = q >> 1;                      // the 64-column chunk of every tile this thread takes
+    const int r_in_tile = wg * 64 + wq * 16 + (lane >> 2) + 8 * (q & 1);
     // FIFO slot s of this thread lives at fifo | s << 8 (the warp's 8 KB region is 8 KB aligned, a slot row is 32 lanes x 8 bytes)
     const uint32_t fifo = smem_u32(fifo_all) + (uint32_t)(warp - 4) * (LF_FIFO * 256) + (uint32_t)lane * 8u;
     int stage = 0; uint32_t phase = 0;
@@ -127,8 +164,9 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
       float m_run = -1e30f, s_run = 0.f;
       uint32_t pos8 = 0;                          // appended entries << 8 (slot byte offset before wrapping)
       int flushed = 0, ovf = 0;
-      for (int j = 0; j < p.npt; ++j) {
-        const int n_blk = sp * p.npt + j;
+      // the wgmma main loop of tile n_blk into acc; between(kb) runs after k-block kb's group is issued and the previous stage released,
+      // while the tensor pipe works on it
+      auto mainloop = [&](int n_blk, auto&& between) {
         int prev_stage = -1;
         for (int kb = 0; kb < p.num_kb; ++kb) {
           mbar_wait(full_bar + stage, phase);
@@ -144,55 +182,81 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
           if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
           prev_stage = stage;
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          between(kb);
         }
         wgmma_wait<0>();
         reg_fence(acc);
         if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
-        named_sync(1 + wg, 128);                   // the previous tile's readers are done with the staging buffer
-        stage_acc<LF_BN / 2, LF_STG_LD>(acc, stg, 0, LF_BN);
-        named_sync(1 + wg, 128);
-        {
-          const int c = half;
-          float v[64];
-          stage_ld32(my_row, v);
-          stage_ld32(my_row + 32, v + 32);
-          // ---- online softmax statistics of the row ----
-          float lm = fmaxf(v[0], v[1]);
+      };
+      mainloop(sp * p.npt, [](int) {});
+      for (int j = 0; j < p.npt; ++j) {
+        const int n_blk = sp * p.npt + j;
+        const int c = half;
+        // the tile's chunk leaves the accumulators (which the next tile's wgmma then owns): column i in v[lf_col(i)]
+        float v[64];
+        lf_quad_transpose(acc, v, q);
+        // ---- online softmax statistics of the row ----
+        float lm = fmaxf(v[lf_col(0)], v[lf_col(1)]);
 #pragma unroll
-          for (int i = 2; i < 64; i += 2) lm = fmaxf(lm, fmaxf(v[i], v[i + 1]));
-          if (lm > m_run) { s_run *= ex2_approx((m_run - lm) * LOG2E); m_run = lm; }
-          const float mb = m_run * LOG2E;
-          float s0 = 0.f, s1 = 0.f;
+        for (int i = 2; i < 64; i += 2) lm = fmaxf(lm, fmaxf(v[lf_col(i)], v[lf_col(i + 1)]));
+        if (lm > m_run) { s_run *= ex2_approx((m_run - lm) * LOG2E); m_run = lm; }
+        const float mb = m_run * LOG2E;
+        float s0 = 0.f, s1 = 0.f;
+        const uint32_t col0 = (uint32_t)(n_blk * LF_BN + c * 64);
+        const uint32_t pos8_before = pos8;
+        // slices 0..3: the exp sums (even / odd column chains, in column order) and the candidate appends of 16 columns each;
+        // slice 4: overflow check and the sector drains, after all 64 appends as before
+        auto slice = [&](auto sc) {
+          constexpr int SL = decltype(sc)::value;
+          if constexpr (SL < 4) {
 #pragma unroll
-          for (int i = 0; i < 64; i += 2) { s0 += ex2_approx(fmaf(v[i], LOG2E, -mb)); s1 += ex2_approx(fmaf(v[i + 1], LOG2E, -mb)); }
-          s_run += s0 + s1;
-          // ---- candidates >= t_lo -> private FIFO (predicated, no branch) ----
-          const uint32_t col0 = (uint32_t)(n_blk * LF_BN + c * 64);
-          const uint32_t pos8_before = pos8;
+            for (int i = 16 * SL; i < 16 * SL + 16; i += 2) { s0 += ex2_approx(fmaf(v[lf_col(i)], LOG2E, -mb)); s1 += ex2_approx(fmaf(v[lf_col(i + 1)], LOG2E, -mb)); }
+            // ---- candidates >= t_lo -> private FIFO (predicated, no branch) ----
 #pragma unroll
-          for (int i = 0; i < 64; ++i) {
-            if (v[i] >= tlo) {
-              const uint32_t a = fifo | (pos8 & ((LF_FIFO - 1) << 8));
-              asm volatile("st.shared.b32 [%0], %1;\n\tst.shared.b32 [%0+4], %2;" :: "r"(a), "r"(__float_as_uint(v[i])), "r"(col0 + (uint32_t)i) : "memory");
-              pos8 += 256u;
+            for (int i = 16 * SL; i < 16 * SL + 16; ++i) {
+              if (v[lf_col(i)] >= tlo) {
+                const uint32_t a = fifo | (pos8 & ((LF_FIFO - 1) << 8));
+                asm volatile("st.shared.b32 [%0], %1;\n\tst.shared.b32 [%0+4], %2;" :: "r"(a), "r"(__float_as_uint(v[lf_col(i)])), "r"(col0 + (uint32_t)i) : "memory");
+                pos8 += 256u;
+              }
+            }
+          } else {
+            s_run += s0 + s1;
+            // more than LF_FIFO - 3 candidates in 64 columns wrapped over unflushed entries (12 % are expected: never on real rows) -> fallback row
+            if (pos8 - pos8_before > (uint32_t)((LF_FIFO - 3) << 8)) ovf = 1;
+            // ---- drain whole 32-byte sectors: most lanes have one or two to write, all at the same point ----
+            while ((int)(pos8 >> 8) - flushed >= 4) {
+              if (flushed + 4 <= p.cap) {
+                const uint32_t b0 = fifo | (((uint32_t)flushed << 8) & ((LF_FIFO - 1) << 8));      // flushed % 4 == 0: the four slots do not wrap
+                uint32_t w[8];
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(w[2 * i]), "=r"(w[2 * i + 1]) : "r"(b0 + (uint32_t)(i * 256)));
+                st256(seg + flushed, w[0], w[1], w[2], w[3], w[4], w[5], w[6], w[7]);
+              } else {
+                ovf = 1;
+              }
+              flushed += 4;
             }
           }
-          // more than LF_FIFO - 3 candidates in 64 columns wrapped over unflushed entries (12 % are expected: never on real rows) -> fallback row
-          if (pos8 - pos8_before > (uint32_t)((LF_FIFO - 3) << 8)) ovf = 1;
-          // ---- drain whole 32-byte sectors: most lanes have one or two to write, all at the same point ----
-          while ((int)(pos8 >> 8) - flushed >= 4) {
-            if (flushed + 4 <= p.cap) {
-              const uint32_t b0 = fifo | (((uint32_t)flushed << 8) & ((LF_FIFO - 1) << 8));      // flushed % 4 == 0: the four slots do not wrap
-              uint32_t w[8];
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(w[2 * i]), "=r"(w[2 * i + 1]) : "r"(b0 + (uint32_t)(i * 256)));
-              st256(seg + flushed, w[0], w[1], w[2], w[3], w[4], w[5], w[6], w[7]);
-            } else {
-              ovf = 1;
-            }
-            flushed += 4;
+        };
+        auto slice_at = [&](int s) {
+          switch (s) {
+            case 0: slice(std::integral_constant<int, 0>{}); break;
+            case 1: slice(std::integral_constant<int, 1>{}); break;
+            case 2: slice(std::integral_constant<int, 2>{}); break;
+            case 3: slice(std::integral_constant<int, 3>{}); break;
+            case 4: slice(std::integral_constant<int, 4>{}); break;
           }
+        };
+        if (j + 1 < p.npt) {
+          // the next tile of the item runs on the tensor pipe while this one's epilogue is sliced in between its k-blocks
+          mainloop(n_blk + 1, [&](int kb) { if (kb < LF_SLICES) slice_at(kb); });
+          for (int s = p.num_kb; s < LF_SLICES; ++s) slice_at(s);
+        } else {
+          // the item's last tile: finish its epilogue before the next item switches rows
+          slice(std::integral_constant<int, 0>{}); slice(std::integral_constant<int, 1>{}); slice(std::integral_constant<int, 2>{});
+          slice(std::integral_constant<int, 3>{}); slice(std::integral_constant<int, 4>{});
         }
       }
       // ---- end of the work item: the last (< 4) entries as one padded sector, then the partial record ----
