@@ -287,6 +287,35 @@ typedef struct {
 uint64_t mmg_logits_fused_workspace_bytes(int64_t rows_capacity, int32_t V, int32_t K, int32_t k);
 int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream);
 
+/* Cross-entropy of the labelled rows of MaskGit.forward (muse_maskgit_pytorch.py:335, 717-726) without a [rows, V] logits buffer:
+ *   nll[r] = logsumexp_v(e_r . W_v) - e_r . W_labels[r]   (fp32; bf16 operands, wgmma)
+ * The logits GEMM of mmg_logits_fused runs with an epilogue that keeps, per (row, split of the vocabulary, 64-column half), the
+ * online-softmax partials (max, sum of exp) and the logit at the label column; a second kernel merges a row's records in split order,
+ * so the result is bitwise the same on every run.  Labels must lie in [0, V) (a row whose label lies outside gets NaN).             */
+typedef struct {
+  const void* e;           /* [rows, K] bf16: final-LayerNormed embeddings of the labelled rows                                 */
+  const void* w;           /* [V, K] bf16 to_logits weight                                                                        */
+  const int32_t* labels;   /* [rows]                                                                                              */
+  float* nll;              /* [rows] out                                                                                          */
+  int64_t rows, rows_capacity;   /* rows_capacity: the row count the workspace was sized for (0: rows)                            */
+  int32_t V, K;
+  void* workspace; uint64_t workspace_bytes;   /* >= mmg_logits_xent_workspace_bytes(rows_capacity, V, K), 256-byte aligned        */
+} mmg_logits_xent_args;
+/* 0 when the shape is not supported by the fused path (V % 128, K % 64, K < 64): mmg_logits_xent then returns MMG_EINVAL */
+uint64_t mmg_logits_xent_workspace_bytes(int64_t rows_capacity, int32_t V, int32_t K);
+int mmg_logits_xent(const mmg_logits_xent_args* a, void* stream);
+
+/* The same nll from materialised fp32 logits rows (precision="fp32", shapes mmg_logits_xent does not take, the token-critic branch of
+ * MaskGit.forward): one CTA per row, a fixed reduction order.  A label outside [0, V) gives NaN.                                    */
+typedef struct {
+  const float* logits;     /* [rows, ld] fp32                                                                                     */
+  int64_t ld;
+  const int32_t* labels;   /* [rows]                                                                                              */
+  float* nll;              /* [rows] out                                                                                          */
+  int64_t rows; int32_t V, _pad;
+} mmg_logits_xent_rows_args;
+int mmg_logits_xent_rows(const mmg_logits_xent_rows_args* a, void* stream);
+
 /* token-critic scoring branch of MaskGit.generate (muse_maskgit_pytorch.py:590-600; TokenCritic :383-386, SelfCritic :352-361):
  *   s[r] = dot(LayerNorm(x_cond[r]) * gamma, w) + bias;   x_null != NULL: s = s_null + (s - s_null) * cond_scale  (CFG, :257)
  *   scores[r] = s + (u[r] - 0.5) * noise_mul       noise_mul = critic_noise_scale * steps_until_x0 / timesteps

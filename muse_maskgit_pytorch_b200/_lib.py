@@ -92,6 +92,15 @@ class LogitsFusedArgs(C.Structure):
                 ("workspace", vp), ("workspace_bytes", u64), ("status", vp)]
 
 
+class LogitsXentArgs(C.Structure):
+    _fields_ = [("e", vp), ("w", vp), ("labels", vp), ("nll", vp), ("rows", i64), ("rows_capacity", i64), ("V", i32), ("K", i32),
+                ("workspace", vp), ("workspace_bytes", u64)]
+
+
+class LogitsXentRowsArgs(C.Structure):
+    _fields_ = [("logits", vp), ("ld", i64), ("labels", vp), ("nll", vp), ("rows", i64), ("V", i32), ("_pad", i32)]
+
+
 class CriticScoreArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("w", vp), ("bias", f32), ("cond_scale", f32), ("noise_mul", f32),
                 ("dim", i32), ("u", vp), ("scores", vp), ("rows", i64), ("row_offset", i64), ("seed", u64), ("seed_dev", vp),
@@ -159,9 +168,10 @@ EXPORTS = {
     "mmg_vq_decode_codes": DecodeCodesArgs, "mmg_cast": CastArgs, "mmg_split3": Split3Args, "mmg_critic_score": CriticScoreArgs,
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,
     "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs,
+    "mmg_logits_xent": LogitsXentArgs, "mmg_logits_xent_rows": LogitsXentRowsArgs,
 }
 PLAIN_EXPORTS = ("mmg_version", "mmg_last_error", "mmg_launch_count", "mmg_sizeof", "mmg_decode_step_workspace_bytes", "mmg_logits_fused_workspace_bytes",
-                 "mmg_simt_fallback_count", "mmg_simt_launch_count")
+                 "mmg_logits_xent_workspace_bytes", "mmg_simt_fallback_count", "mmg_simt_launch_count")
 
 _lib = None
 
@@ -193,6 +203,8 @@ def lib():
         l.mmg_decode_step_workspace_bytes.restype = u64
         l.mmg_logits_fused_workspace_bytes.argtypes = [i64, i32, i32, i32]
         l.mmg_logits_fused_workspace_bytes.restype = u64
+        l.mmg_logits_xent_workspace_bytes.argtypes = [i64, i32, i32]
+        l.mmg_logits_xent_workspace_bytes.restype = u64
         for name, st in list(EXPORTS.items()) + [("mmg_epilogue", EpilogueArgs), ("mmg_attn_weights", AttnWeights), ("mmg_layer_weights", LayerWeights)]:
             if l.mmg_sizeof(name.encode()) != C.sizeof(st):
                 raise MMGError(f"ABI mismatch for {name}: C {l.mmg_sizeof(name.encode())} vs ctypes {C.sizeof(st)}")

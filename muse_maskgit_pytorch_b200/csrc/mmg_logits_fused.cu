@@ -36,10 +36,12 @@ constexpr int LF_SLICES = 5;                // epilogue slices of a tile run bet
 
 // Shared memory: the epilogue runs from the accumulator registers, so next to the candidate FIFOs (64 KB) there is room for four 32 KB
 // operand stages within the 227 KB of a block: 1 KB alignment + 128 KB ring + 8 KB barriers / padding + 64 KB FIFOs = 201 KB.
+// The cross-entropy epilogue (XENT, mmg_logits_xent) keeps no candidates: its 64 KB go to two more stages, 1 + 192 + 8 = 201 KB.
+template <bool XENT>
 struct LfCfg {
   static constexpr int STAGE_BYTES = LF_A_BYTES + LF_B_BYTES;
-  static constexpr int FIFO_BYTES = LF_EPI_WARPS * LF_FIFO * 32 * 8;
-  static constexpr int STAGES = 4;
+  static constexpr int FIFO_BYTES = XENT ? 0 : LF_EPI_WARPS * LF_FIFO * 32 * 8;
+  static constexpr int STAGES = XENT ? 6 : 4;
   // [<= 1 KB to align][operand ring][barriers + padding up to the next 8 KB boundary][FIFO region, 8 KB aligned like its per-warp stride]
   static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 8192 + FIFO_BYTES;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
@@ -91,13 +93,18 @@ struct alignas(64) LfParams {
   int num_kb, num_m_tiles, num_pm, S, npt, cap;
   const float* thr;               // [R] candidate threshold per row
   float4* parts;                  // [R][S][2]: (running max, sum of exp(x - max), candidate count as int bits, overflow flag as int bits)
+                                  // XENT: (running max, sum of exp(x - max), logit at the label column, 1 as int bits if the segment saw the label)
   uint2* lists;                   // [R][S][2][cap]: (logit bits, vocabulary index)
+  const int32_t* labels;          // XENT: [R] label column per row
 };
 
+// XENT = false: the candidate / softmax epilogue of the fused sampling tail.  XENT = true: the cross-entropy epilogue of mmg_logits_xent,
+// which keeps the softmax partials only and takes the label's logit from the one 64-column chunk that holds it.
+template <bool XENT>
 __global__ void __launch_bounds__(LF_THREADS, 1)
 tc_logits_kernel(const __grid_constant__ LfParams p) {
   using namespace sm90;
-  using Cfg = LfCfg;
+  using Cfg = LfCfg<XENT>;
   constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -159,7 +166,9 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
       const int m_blk = item % p.num_pm, sp = item / p.num_pm;
       const int64_t row = (int64_t)m_blk * LF_BM + r_in_tile;
       const bool valid = row < p.R;
-      const float tlo = valid ? __ldg(p.thr + row) : FLT_MAX;            // rows past R never produce a candidate
+      const float tlo = (!XENT && valid) ? __ldg(p.thr + row) : FLT_MAX;            // rows past R never produce a candidate
+      const int lab = (XENT && valid) ? __ldg(p.labels + row) : -1;
+      float xl = 0.f; int has_label = 0;
       uint2* seg = p.lists + ((row * p.S + sp) * LF_SEGS + half) * (int64_t)p.cap;
       float m_run = -1e30f, s_run = 0.f;
       uint32_t pos8 = 0;                          // appended entries << 8 (slot byte offset before wrapping)
@@ -195,6 +204,14 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
         // the tile's chunk leaves the accumulators (which the next tile's wgmma then owns): column i in v[lf_col(i)]
         float v[64];
         lf_quad_transpose(acc, v, q);
+        if constexpr (XENT) {
+          const uint32_t off = (uint32_t)lab - (uint32_t)(n_blk * LF_BN + c * 64);      // one chunk of the row holds the label column
+          if (off < 64u) {
+#pragma unroll
+            for (int i = 0; i < 64; ++i) if ((uint32_t)i == off) xl = v[lf_col(i)];
+            has_label = 1;
+          }
+        }
         // ---- online softmax statistics of the row ----
         float lm = fmaxf(v[lf_col(0)], v[lf_col(1)]);
 #pragma unroll
@@ -211,15 +228,19 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
           if constexpr (SL < 4) {
 #pragma unroll
             for (int i = 16 * SL; i < 16 * SL + 16; i += 2) { s0 += ex2_approx(fmaf(v[lf_col(i)], LOG2E, -mb)); s1 += ex2_approx(fmaf(v[lf_col(i + 1)], LOG2E, -mb)); }
-            // ---- candidates >= t_lo -> private FIFO (predicated, no branch) ----
+            if constexpr (!XENT) {
+              // ---- candidates >= t_lo -> private FIFO (predicated, no branch) ----
 #pragma unroll
-            for (int i = 16 * SL; i < 16 * SL + 16; ++i) {
-              if (v[lf_col(i)] >= tlo) {
-                const uint32_t a = fifo | (pos8 & ((LF_FIFO - 1) << 8));
-                asm volatile("st.shared.b32 [%0], %1;\n\tst.shared.b32 [%0+4], %2;" :: "r"(a), "r"(__float_as_uint(v[lf_col(i)])), "r"(col0 + (uint32_t)i) : "memory");
-                pos8 += 256u;
+              for (int i = 16 * SL; i < 16 * SL + 16; ++i) {
+                if (v[lf_col(i)] >= tlo) {
+                  const uint32_t a = fifo | (pos8 & ((LF_FIFO - 1) << 8));
+                  asm volatile("st.shared.b32 [%0], %1;\n\tst.shared.b32 [%0+4], %2;" :: "r"(a), "r"(__float_as_uint(v[lf_col(i)])), "r"(col0 + (uint32_t)i) : "memory");
+                  pos8 += 256u;
+                }
               }
             }
+          } else if constexpr (XENT) {
+            s_run += s0 + s1;
           } else {
             s_run += s0 + s1;
             // more than LF_FIFO - 3 candidates in 64 columns wrapped over unflushed entries (12 % are expected: never on real rows) -> fallback row
@@ -258,6 +279,10 @@ tc_logits_kernel(const __grid_constant__ LfParams p) {
           slice(std::integral_constant<int, 0>{}); slice(std::integral_constant<int, 1>{}); slice(std::integral_constant<int, 2>{});
           slice(std::integral_constant<int, 3>{}); slice(std::integral_constant<int, 4>{});
         }
+      }
+      if constexpr (XENT) {
+        if (valid) p.parts[(row * p.S + sp) * LF_SEGS + half] = make_float4(m_run, s_run, xl, __int_as_float(has_label));
+        continue;
       }
       // ---- end of the work item: the last (< 4) entries as one padded sector, then the partial record ----
       const int pos = (int)(pos8 >> 8);
@@ -611,17 +636,90 @@ static bool lf_supported(int V, int K, int k) {
   return n_exp + 4.0 * sd <= SMP_CAP;
 }
 
+template <bool XENT>
 static int launch_lf(const LfParams& p, cudaStream_t st) {
-  constexpr int SMEM = LfCfg::SMEM_BYTES;
+  constexpr int SMEM = LfCfg<XENT>::SMEM_BYTES;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_logits_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); });
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_logits_kernel<XENT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); });
   if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "tc_logits setup: %s", cudaGetErrorString(attr_err));
   const int items = p.num_pm * p.S;
   const int units = items < num_sms() ? items : num_sms();
-  MMG_CUDA(launch_pdl(tc_logits_kernel, dim3(units), dim3(LF_THREADS), SMEM, st, p));
+  MMG_CUDA(launch_pdl(tc_logits_kernel<XENT>, dim3(units), dim3(LF_THREADS), SMEM, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// cross-entropy (MaskGit.forward, muse_maskgit_pytorch.py:335, 717-726): nll[r] = logsumexp_v(e_r . W_v) - e_r . W_label[r]
+// ---------------------------------------------------------------------------------------------------------------------------
+static bool lx_supported(int V, int K) { return V >= LF_BN && V % LF_BN == 0 && K >= 64 && K % 64 == 0; }
+
+// the largest record array over every row count up to R_max (S shrinks as R grows)
+static uint64_t lx_parts_bytes(int64_t R_max, int V) {
+  uint64_t parts = 0;
+  for (int64_t R = LF_BM; ; R += LF_BM) {
+    const int64_t Rc = R < R_max ? R : R_max;
+    const uint64_t pb = (uint64_t)Rc * lf_plan(Rc, V, 1).S * LF_SEGS * 16;
+    if (pb > parts) parts = pb;
+    if (R >= R_max) break;
+  }
+  return parts;
+}
+
+// one thread per row: the row's S x 2 segment records merged in split order (the same sums in the same order on every run)
+__global__ void __launch_bounds__(256)
+logits_xent_merge_kernel(const float4* __restrict__ parts, int nseg, int64_t R, float* __restrict__ nll) {
+  pdl_wait(); pdl_trigger();
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const float4* rec = parts + r * nseg;
+  float M = -FLT_MAX;
+  for (int i = 0; i < nseg; ++i) M = fmaxf(M, rec[i].x);
+  float sum = 0.f, xl = __int_as_float(0x7fc00000);              // NaN unless a segment saw the label column
+  for (int i = 0; i < nseg; ++i) {
+    const float4 t = rec[i];
+    sum += t.y * expf(t.x - M);
+    if (__float_as_int(t.w)) xl = t.z;
+  }
+  nll[r] = M + logf(sum) - xl;
+}
+
+// materialised logits: one CTA per row, one pass of per-thread online (max, sum exp) pairs combined in a fixed tree order
+constexpr int LXR_THREADS = 256;
+__device__ __forceinline__ void lse_push(float& m, float& s, float x) {
+  if (x > m) { s = s * expf(m - x) + 1.f; m = x; } else s += expf(x - m);
+}
+__device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os) {
+  const float M = fmaxf(m, om);
+  s = s * expf(m - M) + os * expf(om - M); m = M;
+}
+__global__ void __launch_bounds__(LXR_THREADS)
+logits_xent_rows_kernel(const float* __restrict__ logits, int64_t ld, int V, const int32_t* __restrict__ labels, float* __restrict__ nll) {
+  __shared__ float s_m[LXR_THREADS / 32], s_s[LXR_THREADS / 32];
+  pdl_wait(); pdl_trigger();
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t r = blockIdx.x;
+  const float* row = logits + r * ld;
+  float m = -FLT_MAX, s = 0.f;
+  if ((reinterpret_cast<uintptr_t>(row) & 15) == 0 && V % 4 == 0) {
+    for (int i = tid; i < V / 4; i += LXR_THREADS) {
+      const float4 x = __ldcs(reinterpret_cast<const float4*>(row) + i);
+      lse_push(m, s, x.x); lse_push(m, s, x.y); lse_push(m, s, x.z); lse_push(m, s, x.w);
+    }
+  } else {
+    for (int i = tid; i < V; i += LXR_THREADS) lse_push(m, s, __ldcs(row + i));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { const float om = __shfl_xor_sync(0xffffffffu, m, o), os = __shfl_xor_sync(0xffffffffu, s, o); lse_merge(m, s, om, os); }
+  if (lane == 0) { s_m[warp] = m; s_s[warp] = s; }
+  __syncthreads();
+  if (tid == 0) {
+    m = s_m[0]; s = s_s[0];
+    for (int w = 1; w < LXR_THREADS / 32; ++w) lse_merge(m, s, s_m[w], s_s[w]);
+    const int lab = labels[r];
+    nll[r] = (lab >= 0 && lab < V) ? m + logf(s) - row[lab] : __int_as_float(0x7fc00000);
+  }
 }
 
 }  // namespace mmg
@@ -678,7 +776,7 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
     if ((rc = make_tmap_bf16(&p.tma_a, a->e, 2, da, sa, ba))) return rc;
     uint64_t db[2] = {(uint64_t)a->K, (uint64_t)s.V}; uint64_t sb[1] = {(uint64_t)a->K * 2}; uint32_t bb[2] = {LF_BK, (uint32_t)LF_BN};
     if ((rc = make_tmap_bf16(&p.tma_b, a->w, 2, db, sb, bb))) return rc;
-    if ((rc = launch_lf(p, st))) return rc;
+    if ((rc = launch_lf<false>(p, st))) return rc;
   }
   float t = s.temperature; if (t < 1e-10f) t = 1e-10f;      // max(temperature, 1e-10): muse_maskgit_pytorch.py:411
   {   // 4. finish
@@ -703,5 +801,51 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
     fs.logits = logits_fb; fs.row_index = fb_rows; fs.row_count_dev = fb_count; fs.row_index_cap = LF_FB_CAP;
     if ((rc = mmg_logits_sample(&fs, stream))) return rc;
   }
+  return MMG_OK;
+}
+
+extern "C" uint64_t mmg_logits_xent_workspace_bytes(int64_t rows_capacity, int32_t V, int32_t K) {
+  if (rows_capacity <= 0 || !lx_supported(V, K)) return 0;
+  return up256(lx_parts_bytes(rows_capacity, V));
+}
+
+extern "C" int mmg_logits_xent(const mmg_logits_xent_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->e && a->w && a->labels && a->nll && a->workspace, "mmg_logits_xent: NULL pointer");
+  MMG_CHECK_ARG(lx_supported(a->V, a->K), "mmg_logits_xent: unsupported V=%d K=%d (use mmg_linear + mmg_logits_xent_rows)", a->V, a->K);
+  MMG_CHECK_ARG(a->rows >= 0, "mmg_logits_xent: rows=%lld", (long long)a->rows);
+  const int64_t R = a->rows;
+  if (R == 0) return MMG_OK;
+  const int64_t R_cap = a->rows_capacity > 0 ? a->rows_capacity : R;
+  MMG_CHECK_ARG(R <= R_cap, "mmg_logits_xent: %lld rows > rows_capacity %lld", (long long)R, (long long)R_cap);
+  const uint64_t need = up256(lx_parts_bytes(R_cap, a->V));
+  MMG_CHECK_ARG(a->workspace_bytes >= need, "mmg_logits_xent: workspace %llu < %llu bytes", (unsigned long long)a->workspace_bytes, (unsigned long long)need);
+  MMG_CHECK_ARG((reinterpret_cast<uintptr_t>(a->workspace) & 255) == 0 && (reinterpret_cast<uintptr_t>(a->e) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15) == 0,
+                "mmg_logits_xent: workspace must be 256-byte aligned, e / w 16-byte aligned");
+  float4* parts = static_cast<float4*>(a->workspace);
+  const LfPlan pl = lf_plan(R, a->V, 1);
+  int rc;
+  {   // the logits GEMM with the cross-entropy epilogue: per (row, split, 64-column half) softmax partials and the label's logit
+    LfParams p{};
+    p.R = R; p.num_kb = a->K / LF_BK; p.num_m_tiles = pl.num_m_tiles; p.num_pm = pl.num_pm; p.S = pl.S; p.npt = pl.npt;
+    p.parts = parts; p.labels = a->labels;
+    uint64_t da[2] = {(uint64_t)a->K, (uint64_t)R}; uint64_t sa[1] = {(uint64_t)a->K * 2}; uint32_t ba[2] = {LF_BK, LF_BM};
+    if ((rc = make_tmap_bf16(&p.tma_a, a->e, 2, da, sa, ba))) return rc;
+    uint64_t db[2] = {(uint64_t)a->K, (uint64_t)a->V}; uint64_t sb[1] = {(uint64_t)a->K * 2}; uint32_t bb[2] = {LF_BK, (uint32_t)LF_BN};
+    if ((rc = make_tmap_bf16(&p.tma_b, a->w, 2, db, sb, bb))) return rc;
+    if ((rc = launch_lf<true>(p, st))) return rc;
+  }
+  MMG_CUDA(launch_pdl(logits_xent_merge_kernel, dim3((unsigned)((R + 255) / 256)), dim3(256), 0, st, (const float4*)parts, LF_SEGS * pl.S, R, a->nll));
+  MMG_LAUNCHED();
+  return MMG_OK;
+}
+
+extern "C" int mmg_logits_xent_rows(const mmg_logits_xent_rows_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->logits && a->labels && a->nll, "mmg_logits_xent_rows: NULL pointer");
+  MMG_CHECK_ARG(a->V >= 1 && a->rows >= 0 && a->ld >= a->V, "mmg_logits_xent_rows: rows=%lld V=%d ld=%lld", (long long)a->rows, a->V, (long long)a->ld);
+  if (a->rows == 0) return MMG_OK;
+  MMG_CUDA(launch_pdl(logits_xent_rows_kernel, dim3((unsigned)a->rows), dim3(LXR_THREADS), 0, st, a->logits, a->ld, a->V, a->labels, a->nll));
+  MMG_LAUNCHED();
   return MMG_OK;
 }

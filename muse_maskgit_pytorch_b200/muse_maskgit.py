@@ -11,6 +11,7 @@ constant to_out(null_v) (every text key masked -> softmax puts weight exactly 1 
 import ctypes
 import math
 import os
+import random
 from functools import partial
 from pathlib import Path
 from typing import Callable, List, Optional
@@ -431,6 +432,24 @@ def cosine_schedule(t):
     return torch.cos(t * math.pi * 0.5)
 
 
+def _aten_uniform_geometry(device, numel):
+    """(stride, Philox offset increment) of one ATen CUDA `uniform_` call over `numel` values.  Launch geometry as ATen's
+    calc_execution_policy: block 256, grid = min(SMs * maxThreadsPerSM / 256, ceil(numel / 256)), 4 values per thread and round."""
+    props = torch.cuda.get_device_properties(device)
+    cap = props.multi_processor_count * (props.max_threads_per_multi_processor // 256)
+    stride = 256 * min(cap, (numel + 255) // 256)
+    return stride, ((numel - 1) // (stride * 4) + 1) * 4
+
+
+def _mask_subset_prob(mask, prob, draw, min_mask=0):
+    """ref: muse_maskgit_pytorch.py:46-60 (get_mask_subset_prob) with its torch.rand drawn through `draw`."""
+    num_to_mask = (mask.sum(dim=-1, keepdim=True) * prob).clamp(min=min_mask)
+    logits = draw(mask.shape).masked_fill(~mask, -1)
+    randperm = logits.argsort(dim=-1).argsort(dim=-1).float()
+    randperm -= (~mask).sum(dim=-1, keepdim=True)
+    return (randperm < num_to_mask).masked_fill_(~mask, False)
+
+
 def regen_tokens(mask, b, image_size, fmap_size):
     """Inpainting mask -> (b, fmap_size, fmap_size) bool, True = regenerate the token.  `mask` is bool or {0, 1}, True = regenerate, at pixel
     resolution ((b, H, W) or (b, 1, H, W), H = W = image_size) or at token resolution ((b, fmap_size, fmap_size)).  A token is regenerated when
@@ -725,12 +744,10 @@ class MaskGit(nn.Module):
         grid = min(SMs * maxThreadsPerSM / 256, ceil(numel / 256)), 4 values per thread and round.  The generator is read here and
         advanced by what the reference would have consumed; seed / offset reach the kernels through device words (graph replay)."""
         gen = torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
-        props = torch.cuda.get_device_properties(device)
-        cap = props.multi_processor_count * (props.max_threads_per_multi_processor // 256)
         B = self.global_batch if self.global_batch is not None else b
-        stride = lambda numel: 256 * min(cap, (numel + 255) // 256)
-        inc = lambda numel: ((numel - 1) // (stride(numel) * 4) + 1) * 4
         ng, nc = B * n * V, B * n
+        stride = lambda numel: _aten_uniform_geometry(device, numel)[0]
+        inc = lambda numel: _aten_uniform_geometry(device, numel)[1]
         per_step = inc(ng) + (inc(nc) if use_critic else 0)
         seed, off = gen.initial_seed(), gen.get_offset()
         self._aten_start_offset = off
@@ -872,8 +889,145 @@ class MaskGit(nn.Module):
             torch.cuda.nvtx.range_pop()
         return images, ids, (tail.get("status") if tail is not None else None)
 
-    def forward(self, *args, **kwargs):
-        raise NotImplementedError("MaskGit.forward is the training loss (muse_maskgit_pytorch.py:623-741); training is out of scope")
+    def forward(self, images_or_ids, ignore_index=-1, cond_images: Optional[torch.Tensor] = None, cond_token_ids: Optional[torch.Tensor] = None,
+                texts: Optional[List[str]] = None, text_embeds: Optional[torch.Tensor] = None, cond_drop_prob=None, train_only_generator=False,
+                sample_temperature=None):
+        """The training objective of the reference (muse_maskgit_pytorch.py:623-741), evaluated without gradients: the mean cross-entropy of
+        the masked tokens, plus critic_loss_weight * the token critic's BCE when a critic is present and train_only_generator is False.
+        Returns a 0-d fp32 tensor on the model's device (NaN when no position is labelled, as F.cross_entropy).
+
+        The random draws are the reference's, in its order, from torch on the model's device (python's `random` for the self-conditioning
+        and sampling-temperature draws): with `sampler_noise_fn` set, every torch uniform draw is noise_fn(0, shape) instead.  The gumbel
+        noise of the critic branch follows `sampler_rng` as in generate().  Must run under torch.no_grad() / torch.inference_mode()."""
+        if torch.is_grad_enabled():
+            raise RuntimeError("MaskGit.forward evaluates the loss without gradients (there are no backward kernels): call it under "
+                               "torch.no_grad() or torch.inference_mode()")
+        tr = self.transformer
+        V, mask_id = tr.num_tokens, self.mask_id
+        device = next(self.parameters()).device
+        if images_or_ids.dtype == torch.float:
+            assert all(s == self.image_size for s in images_or_ids.shape[-2:]), "the image you passed in is not of the correct dimensions"
+        else:
+            assert not self.resize_image_for_cond_image, ("you cannot pass in raw image token ids if you want the framework to autoresize image "
+                                                          "for conditioning super res transformer")
+            self._check_ids(images_or_ids, "images_or_ids")
+        assert not (cond_images is not None and cond_token_ids is not None), \
+            "if conditioning on low resolution, cannot pass in both images and token ids"
+        if cond_token_ids is not None:
+            self._check_ids(cond_token_ids, "cond_token_ids")
+        assert (texts is None) != (text_embeds is None), "pass exactly one of texts / text_embeds"
+        for net in (tr, self.vae, self.cond_vae, self.token_critic if isinstance(self.token_critic, Transformer) else None):
+            if net is not None:
+                net._check_weights()
+        if images_or_ids.dtype == torch.float:
+            ids = self.vae.encode_ids(images_or_ids.to(device, torch.float32).contiguous())
+        else:
+            ids = images_or_ids.to(device, torch.long)
+        ids = ids.reshape(ids.shape[0], -1)
+        b, n = ids.shape
+        cond_drop_prob = self.cond_drop_prob if cond_drop_prob is None else cond_drop_prob
+        if cond_images is not None:
+            assert all(s == self.cond_image_size for s in cond_images.shape[-2:])
+            cond_token_ids = self.cond_vae.encode_ids(cond_images.to(device, torch.float32).contiguous())
+        cond_ids = None if cond_token_ids is None else cond_token_ids.to(device, torch.long).reshape(b, -1).contiguous()
+        if self.sampler_noise_fn is not None:
+            draw = lambda shape: self.sampler_noise_fn(0, shape).to(device=device, dtype=torch.float32)
+        else:
+            draw = lambda shape: torch.zeros(shape, device=device).uniform_(0, 1)
+        # ---- masks and labels (:670-686): labels use the mask before the no-mask subset is removed, the input x the mask after it
+        num_token_masked = (n * self.noise_schedule(draw((b,)))).round().clamp(min=1)
+        mask = draw((b, n)).argsort(dim=-1) < num_token_masked[:, None]
+        labels = torch.where(mask, ids, ignore_index)
+        if self.no_mask_token_prob > 0.:
+            mask &= ~_mask_subset_prob(mask, self.no_mask_token_prob, draw)
+        x = torch.where(mask, mask_id, ids).contiguous()
+        flat = (labels != ignore_index).reshape(-1)
+        R = int(flat.sum().item())
+        if R == 0:
+            return torch.full((), float("nan"), device=device)
+        pos = flat.nonzero()[:, 0].to(torch.int32).contiguous()                   # labelled flat positions, ascending
+        lab = labels.reshape(-1)[pos.long()].to(torch.int32).contiguous()
+        if texts is not None:
+            text_embeds = tr.encode_text(texts)
+        text_embeds = text_embeds.to(device, torch.float32)
+        P = tr._packed()
+        # ---- self-conditioning (:696-708): one stack without drop, its final-LayerNorm embed fed to the loss pass
+        sc_embed = None
+        if tr.self_cond and random.random() < self.self_cond_prob:
+            xs = tr._run_blocks(x, tr._prepare_context(text_embeds, cond_ids, [False]), 1)
+            sc_embed = torch.empty((b * n, tr.dim), device=device, dtype=torch.float32)
+            ops.layernorm(xs, P["gf"], sc_embed)
+        # ---- the loss pass (:712-720): final LayerNorm of the labelled rows only, then to_logits + cross-entropy
+        te = self._drop_text(text_embeds, cond_drop_prob, draw)
+        xres = tr._run_blocks(x, tr._prepare_context(te, cond_ids, [cond_drop_prob == 1]), 1, sc_embed)
+        e = torch.empty((R, tr.dim), device=device, dtype=P["adt"])
+        ops.final_embed(xres, None, P["gf"], pos, e, 1, b * n, R, 1.)
+        nll = torch.empty((R,), device=device, dtype=torch.float32)
+        use_critic = self.token_critic is not None and not train_only_generator
+        nbytes = 0
+        if self.use_fused_tail and P["adt"] == torch.bfloat16 and not use_critic:
+            nbytes = ops.logits_xent_workspace_bytes(R, V, tr.dim)
+        if nbytes:
+            ops.logits_xent(e, P["wlog"], lab, nll, torch.empty((nbytes,), dtype=torch.uint8, device=device))
+        else:
+            logits = torch.empty((R, V), device=device, dtype=torch.float32)
+            ops.linear(e, P["wlog"], logits)
+            ops.logits_xent_rows(logits, lab, nll)
+        ce_loss = nll.mean()
+        if not use_critic:
+            return ce_loss
+        # ---- token critic (:728-741): gumbel sample over the full vocabulary at the masked rows, then the critic's BCE over all b * n
+        temperature = random.random()                                          # drawn even when given: default(...) evaluates it
+        if sample_temperature is not None:
+            temperature = sample_temperature
+        critic_input = x.clone()
+        kw = dict(seed=0, step=0, row_offset=0, only_masked_id=mask_id)
+        if self.sampler_noise_fn is not None:
+            kw["u"] = draw((b, n, V)).contiguous()
+        elif self.sampler_rng == "aten":
+            gen = torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
+            stride, inc = _aten_uniform_geometry(device, b * n * V)
+            seed, off = gen.initial_seed(), gen.get_offset()
+            gen.set_offset(off + inc)
+            kw.update(seed=seed, aten=(off, None, stride))
+        else:
+            assert self.sampler_rng == "mmg", self.sampler_rng
+            kw["seed"] = self.sampler_seed if self.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+        # one sequence of b * n positions: the noise of flat position p is that of (p // n, p % n) in the (b, n, V) draw
+        ops.logits_sample(logits, pos.view(1, R), critic_input.view(1, b * n), torch.empty((1, b * n), device=device), R, V,
+                          float(temperature), **kw)
+        critic_labels = (ids != critic_input).float()
+        te_c = self._drop_text(text_embeds, cond_drop_prob, draw)
+        if isinstance(self.token_critic, SelfCritic):
+            cnet = tr
+            whead, bhead = self.token_critic._head()
+            whead = whead.to(device)
+        else:
+            cnet = self.token_critic
+            whead, bhead = cnet._packed()["whead"], 0.
+            assert whead is not None, "token_critic must have dim_out == 1"
+        xc = cnet._run_blocks(critic_input, cnet._prepare_context(te_c, cond_ids, [cond_drop_prob == 1]), 1)
+        critic_logits = torch.empty((b * n,), device=device, dtype=torch.float32)
+        ops.critic_score(xc, None, cnet._packed()["gf"], whead, float(bhead), 1., 0., critic_logits)
+        bce_loss = torch.nn.functional.binary_cross_entropy_with_logits(critic_logits.view(b, n), critic_labels)
+        return ce_loss + self.critic_loss_weight * bce_loss
+
+    def _check_ids(self, t, name):
+        """Token ids must lie in [0, num_tokens): checked on the host side before any kernel reads them (the reference would hit a
+        device-side assert in the embedding)."""
+        V = self.transformer.num_tokens
+        if t.numel() and (int(t.min()) < 0 or int(t.max()) >= V):
+            raise ValueError(f"{name} must lie in [0, num_tokens = {V}); got values in [{int(t.min())}, {int(t.max())}]")
+
+    @staticmethod
+    def _drop_text(text_embeds, cond_drop_prob, draw):
+        """The conditioning drop of Transformer.forward (muse_maskgit_pytorch.py:306-310, prob_mask_like :393-399): a dropped sequence's text
+        embeddings are zeroed, which masks its text keys.  Draws only when 0 < cond_drop_prob < 1; 1 drops every text key through the
+        branch flag of _prepare_context."""
+        if not 0. < cond_drop_prob < 1.:
+            return text_embeds
+        keep = draw((text_embeds.shape[0], 1)) < (1. - cond_drop_prob)
+        return text_embeds * keep[:, :, None]
 
 
 # ------------------------------------------------------------------------------------------------ Muse

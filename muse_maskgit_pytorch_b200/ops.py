@@ -289,6 +289,37 @@ def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, work
     L.call("mmg_logits_fused", a)
 
 
+def logits_xent_workspace_bytes(rows_capacity, V, K):
+    """Bytes of workspace mmg_logits_xent needs for up to `rows_capacity` rows; 0 = shape not supported by the fused path."""
+    return int(L.lib().mmg_logits_xent_workspace_bytes(int(rows_capacity), int(V), int(K)))
+
+
+def logits_xent(e, w, labels, nll, workspace, rows_capacity=0):
+    """nll[r] = logsumexp(e[r] @ w.T) - (e[r] @ w.T)[labels[r]] without a [rows, V] logits buffer.  e [R, K], w [V, K] bf16; labels int32 [R]
+    in [0, V); nll fp32 [R]."""
+    _chk(e, "e"); _chk(w, "w"); _chk(labels, "labels"); _chk(nll, "nll"); _chk(workspace, "workspace")
+    assert e.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and w.shape[1] == e.shape[1]
+    assert labels.dtype == torch.int32 and nll.dtype == torch.float32 and labels.numel() >= e.shape[0] and nll.numel() >= e.shape[0]
+    a = L.LogitsXentArgs()
+    a.e = e.data_ptr(); a.w = w.data_ptr(); a.labels = labels.data_ptr(); a.nll = nll.data_ptr()
+    a.rows = e.shape[0]; a.rows_capacity = rows_capacity; a.V, a.K = w.shape
+    a.workspace = workspace.data_ptr(); a.workspace_bytes = workspace.numel() * workspace.element_size()
+    L.call("mmg_logits_xent", a)
+    return nll
+
+
+def logits_xent_rows(logits, labels, nll):
+    """nll[r] = logsumexp(logits[r]) - logits[r, labels[r]] from fp32 logits rows [R, V] (row stride allowed)."""
+    assert logits.is_cuda and logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
+    _chk(labels, "labels"); _chk(nll, "nll")
+    assert labels.dtype == torch.int32 and nll.dtype == torch.float32 and labels.numel() >= logits.shape[0] and nll.numel() >= logits.shape[0]
+    a = L.LogitsXentRowsArgs()
+    a.logits = logits.data_ptr(); a.ld = logits.stride(0) if logits.shape[0] > 1 else logits.shape[1]
+    a.labels = labels.data_ptr(); a.nll = nll.data_ptr(); a.rows, a.V = logits.shape
+    L.call("mmg_logits_xent_rows", a)
+    return nll
+
+
 def critic_score(x_cond, x_null, gamma, w, bias, cond_scale, noise_mul, scores, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
                  aten=None):
     """scores[r] = CFG(dot(LN(x[r]) * gamma, w) + bias) + (u[r] - 0.5) * noise_mul   (ref: muse_maskgit_pytorch.py:590-600)"""
