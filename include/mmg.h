@@ -34,6 +34,7 @@ extern "C" {
 /* operand dtypes */
 #define MMG_F32  0
 #define MMG_BF16 1
+#define MMG_E4M3 2   /* fp8 e4m3 (OCP E4M3FN: largest finite 448, no infinities): mmg_linear_fp8 operands, mmg_layernorm_fp8 output */
 
 int         mmg_version(void);
 const char* mmg_last_error(void);
@@ -111,6 +112,24 @@ typedef struct {
 } mmg_linear_args;
 int mmg_linear(const mmg_linear_args* a, void* stream);
 
+/* The same product with e4m3 operands and one fp32 scale per row of A and per row of W (precision="fp8"):
+ *   acc[r, c] = sum_k qa[r, k] qw[c, k]  (fp32 accumulation on the fp8 tensor cores),  C[r, c] = acc[r, c] * a_scale[r] * w_scale[c]
+ * then the epilogue exactly as mmg_linear's tile epilogue: MMG_EPI_QKV (bf16 q / k / v, tokens % 32 == 0, M % 128 == 0, N % 128 == 0,
+ * nk_heads == nv_heads) or MMG_EPI_GEGLU (bf16 out, N % 256 == 0, ldo % 8 == 0, optional row_stats partials of the dequantised outputs).
+ * K % 128 == 0, lda / ldw % 16 == 0, 16-byte aligned operands, w_scale 8-byte aligned.  Any other shape or epilogue returns MMG_EINVAL;
+ * there is no fallback kernel.                                                                                        */
+typedef struct {
+  const void*  a;          /* [M, lda] e4m3                                                                      */
+  const void*  w;          /* [N, ldw] e4m3 (nn.Linear weight layout, K contiguous)                              */
+  const float* a_scale;    /* [M] (mmg_layernorm_fp8 row_scale)                                                  */
+  const float* w_scale;    /* [N]                                                                                */
+  int64_t M, N, K, lda, ldw;
+  int32_t dtype;           /* MMG_E4M3                                                                           */
+  int32_t epilogue;        /* MMG_EPI_QKV or MMG_EPI_GEGLU                                                       */
+  mmg_epilogue_args epi;
+} mmg_linear_fp8_args;
+int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream);
+
 /* Convolutions as implicit GEMM over NHWC activations; weights pre-packed [Cout, taps*Cin] (tap-major, Cin
  * contiguous).  kind: 0 = 1x1; 1 = 3x3 stride 1 pad 1; 2 = 4x4 stride 2 pad 1; 3 = 5x5 stride 1 pad 2.
  * replaces: nn.Conv2d at vqgan_vae.py:224,231,232,255,258,261,271,274,277.                                        */
@@ -171,6 +190,23 @@ typedef struct {
   int64_t rows, width, ldx, ldy;
 } mmg_layernorm_args;
 int mmg_layernorm(const mmg_layernorm_args* a, void* stream);
+
+/* Quantising LayerNorm: the fp32 x -> fp32 y of mmg_layernorm (same arithmetic, same add / x_out / add_from handling), then per row
+ *   amax = max_c |y[r, c]|;  inv = amax == 0 ? 0 : 448 / amax (IEEE division);  q[r, c] = cvt.rn.satfinite.e4m3(y[r, c] * inv);
+ *   row_scale[r] = amax / 448
+ * so that q * row_scale ~= y; columns [width, ldy) are written as 0.  x fp32, width % 4 == 0, width <= 2048, ldx % 4 == 0, ldy % 16 == 0,
+ * x, y, add 16-byte aligned.                                                                                          */
+typedef struct {
+  const float* x;          /* [rows, ldx] fp32                                                                   */
+  void*        y;          /* [rows, ldy] e4m3                                                                   */
+  float*       row_scale;  /* [rows]                                                                             */
+  const float* gamma;      /* [width]                                                                            */
+  const float* add;        /* [width] or NULL                                                                    */
+  float*       x_out;      /* fp32 [rows, ldx] or NULL                                                           */
+  int64_t      add_from;   /* `add` / `x_out` apply to rows >= add_from only                                     */
+  int64_t rows, width, ldx, ldy;
+} mmg_layernorm_fp8_args;
+int mmg_layernorm_fp8(const mmg_layernorm_fp8_args* a, void* stream);
 
 /* x[r, :] = token_emb[ids[r]] + pos_emb[r % n]  (fp32): muse_maskgit_pytorch.py:322-323; `copies` replicas of the
  * whole [rows, dim] block are written back to back (cond / null CFG branches share the embedding).               */

@@ -7,7 +7,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MMG_LIB") or os.path.join(_HERE, "libmmg.so")     # MMG_LIB: an alternative build of the library
 
-F32, BF16 = 0, 1
+F32, BF16, E4M3 = 0, 1, 2
 EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB, EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH = range(11)
 
 vp, i32, i64, f32, u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64
@@ -25,6 +25,11 @@ class EpilogueArgs(C.Structure):
 
 class LinearArgs(C.Structure):
     _fields_ = [("a", vp), ("w", vp), ("M", i64), ("N", i64), ("K", i64), ("lda", i64), ("ldw", i64),
+                ("dtype", i32), ("epilogue", i32), ("epi", EpilogueArgs)]
+
+
+class LinearFp8Args(C.Structure):
+    _fields_ = [("a", vp), ("w", vp), ("a_scale", vp), ("w_scale", vp), ("M", i64), ("N", i64), ("K", i64), ("lda", i64), ("ldw", i64),
                 ("dtype", i32), ("epilogue", i32), ("epi", EpilogueArgs)]
 
 
@@ -50,6 +55,11 @@ class GroupNormArgs(C.Structure):
 
 class LayerNormArgs(C.Structure):
     _fields_ = [("x", vp), ("x_dtype", i32), ("y_dtype", i32), ("y", vp), ("gamma", vp), ("add", vp), ("x_out", vp), ("zero_stats", vp), ("add_from", i64),
+                ("rows", i64), ("width", i64), ("ldx", i64), ("ldy", i64)]
+
+
+class LayerNormFp8Args(C.Structure):
+    _fields_ = [("x", vp), ("y", vp), ("row_scale", vp), ("gamma", vp), ("add", vp), ("x_out", vp), ("add_from", i64),
                 ("rows", i64), ("width", i64), ("ldx", i64), ("ldy", i64)]
 
 
@@ -169,6 +179,7 @@ EXPORTS = {
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,
     "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs,
     "mmg_logits_xent": LogitsXentArgs, "mmg_logits_xent_rows": LogitsXentRowsArgs,
+    "mmg_linear_fp8": LinearFp8Args, "mmg_layernorm_fp8": LayerNormFp8Args,
 }
 PLAIN_EXPORTS = ("mmg_version", "mmg_last_error", "mmg_launch_count", "mmg_sizeof", "mmg_decode_step_workspace_bytes", "mmg_logits_fused_workspace_bytes",
                  "mmg_logits_xent_workspace_bytes", "mmg_simt_fallback_count", "mmg_simt_launch_count")

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
@@ -13,6 +14,7 @@
 namespace mmg {
 
 typedef __nv_bfloat16 bf16;
+typedef __nv_fp8_e4m3 fp8e4;
 
 // ---- thread-local error string -------------------------------------------------------------------
 inline char* err_buf() { static thread_local char buf[512] = {0}; return buf; }

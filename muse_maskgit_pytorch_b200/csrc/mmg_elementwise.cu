@@ -218,6 +218,74 @@ layernorm_rows2_kernel(const float* __restrict__ x, bf16* __restrict__ y, const 
   }
 }
 
+// Quantising LayerNorm (precision="fp8"): the row is normalised with exactly the statements of layernorm_vec_kernel<float, float, CH>
+// (so y is bitwise that kernel's fp32 output), then scaled by 448 / max|y| and rounded to e4m3 (round to nearest even, saturating);
+// row_scale = max|y| / 448 dequantises it.  One warp per row, 4 columns per lane and chunk.
+template <int CH>
+__global__ void __launch_bounds__(256)
+layernorm_fp8_kernel(const float* __restrict__ x, uint8_t* __restrict__ y, float* __restrict__ row_scale, const float* __restrict__ gamma,
+                     const float* __restrict__ add, float* __restrict__ x_out, int64_t add_from, int64_t rows, int width, int64_t ldx, int64_t ldy) {
+  constexpr int VN = 4;
+  pdl_wait(); pdl_trigger();
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  if (row < add_from) { add = nullptr; x_out = nullptr; }
+  const float* xr = x + row * ldx;
+  float v[CH][VN];
+  float sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    const int c = (i * 32 + lane) * VN;
+    if (c < width) {
+      VecIO<float>::ld(xr + c, v[i]);
+      if (add) { const float4 a = *reinterpret_cast<const float4*>(add + c); v[i][0] += a.x; v[i][1] += a.y; v[i][2] += a.z; v[i][3] += a.w; }
+      if (x_out) *reinterpret_cast<float4*>(x_out + row * ldx + c) = make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);   // width % 4 == 0
+#pragma unroll
+      for (int j = 0; j < VN; ++j) { if (c + j >= width) v[i][j] = 0.f; sum += v[i][j]; }
+    } else {
+#pragma unroll
+      for (int j = 0; j < VN; ++j) v[i][j] = 0.f;
+    }
+  }
+  const float mean = warp_sum(sum) / (float)width;
+  float sq = 0.f;
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    const int c = (i * 32 + lane) * VN;
+#pragma unroll
+    for (int j = 0; j < VN; ++j) if (c + j < width) { const float d = v[i][j] - mean; sq += d * d; }
+  }
+  const float rstd = rsqrtf(warp_sum(sq) / (float)width + 1e-5f);
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    const int c = (i * 32 + lane) * VN;
+#pragma unroll
+    for (int j = 0; j < VN; ++j) {
+      v[i][j] = (c + j < width) ? (v[i][j] - mean) * rstd * __ldg(gamma + c + j) : 0.f;
+      amax = fmaxf(amax, fabsf(v[i][j]));
+    }
+  }
+  amax = warp_max(amax);
+  const float inv = amax == 0.f ? 0.f : 448.f / amax;
+  if (lane == 0) row_scale[row] = amax / 448.f;
+  uint8_t* yr = y + row * ldy;
+#pragma unroll
+  for (int i = 0; i < CH; ++i) {
+    const int c = (i * 32 + lane) * VN;
+    if (c < ldy) {
+      uint32_t w = 0;
+      if (c < width) {
+        const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(v[i][0] * inv, v[i][1] * inv), __NV_SATFINITE, __NV_E4M3);
+        const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(v[i][2] * inv, v[i][3] * inv), __NV_SATFINITE, __NV_E4M3);
+        w = (uint32_t)lo | ((uint32_t)hi << 16);
+      }
+      *reinterpret_cast<uint32_t*>(yr + c) = w;
+    }
+  }
+}
+
 // x[copy][r, :] = token_emb[ids[r]] + pos_emb[r % n]        ref: muse_maskgit_pytorch.py:322-323 (and 316 with use_pos = 0)
 __global__ void embed_kernel(const int64_t* __restrict__ ids, const float* __restrict__ tok, const float* __restrict__ pos,
                              float* __restrict__ x, int64_t rows, int64_t n, int64_t dim, int copies, int use_pos) {
@@ -459,6 +527,26 @@ extern "C" int mmg_layernorm(const mmg_layernorm_args* a, void* stream) {
 #undef LNV
 #undef LNV_DISPATCH
 #undef LN_LAUNCH
+  MMG_LAUNCHED();
+  return MMG_OK;
+}
+
+extern "C" int mmg_layernorm_fp8(const mmg_layernorm_fp8_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  MMG_CHECK_ARG(a && a->x && a->y && a->row_scale && a->gamma, "mmg_layernorm_fp8: NULL pointer");
+  MMG_CHECK_ARG(a->width > 0 && a->width <= LN_MAXV * 128 && a->width % 4 == 0, "mmg_layernorm_fp8: width %lld not a multiple of 4 in (0, %d]",
+                (long long)a->width, LN_MAXV * 128);
+  MMG_CHECK_ARG(a->ldx >= a->width && a->ldy >= a->width && a->ldx % 4 == 0 && a->ldy % 16 == 0 && a->ldy <= LN_MAXV * 128,
+                "mmg_layernorm_fp8: leading dims ldx %lld (%% 4), ldy %lld (%% 16, <= %d)", (long long)a->ldx, (long long)a->ldy, LN_MAXV * 128);
+  MMG_CHECK_ARG(al16(a->x) && al16(a->y) && (!a->add || al16(a->add)) && (!a->x_out || al16(a->x_out)), "mmg_layernorm_fp8: 16-byte alignment");
+  if (a->rows == 0) return MMG_OK;
+  const unsigned grid = (unsigned)((a->rows + 7) / 8);
+  const int w = (int)a->width, ch = (int)((a->ldy + 127) / 128);
+#define LNF(CH) launch_pdl(layernorm_fp8_kernel<CH>, dim3(grid), dim3(256), 0, st, a->x, (uint8_t*)a->y, a->row_scale, a->gamma, a->add, a->x_out, \
+                           a->add_from, a->rows, w, a->ldx, a->ldy)
+  if (ch <= 4) MMG_CUDA(LNF(4)); else if (ch <= 8) MMG_CUDA(LNF(8)); else MMG_CUDA(LNF(16));
+#undef LNF
   MMG_LAUNCHED();
   return MMG_OK;
 }

@@ -11,16 +11,16 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 // persistent grid of min(tiles, #SM) CTAs; the tile epilogues keep 32 KB of per-warp output tiles next to the operand ring instead of
 // the register epilogues' 66 KB staging buffer
-template <int BN, int EPI_MODE>
+template <int BN, int EPI_MODE, typename TA = bf16>
 static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
   constexpr int smem = tc_tile_epilogue(EPI_MODE) ? TcCfg<BN>::SMEM_BYTES_RED : TcCfg<BN>::SMEM_BYTES;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, EPI_MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, EPI_MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
   if (attr_err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(tc_gemm<%d, %d>): %s", BN, EPI_MODE, cudaGetErrorString(attr_err));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, EPI_MODE>, dim3(grid), dim3(TC_THREADS), smem, st, p));
+  MMG_CUDA(launch_pdl(tc_gemm_kernel<BN, EPI_MODE, TA>, dim3(grid), dim3(TC_THREADS), smem, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }
@@ -31,6 +31,26 @@ static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
   if (N % 128 == 0 && M_tiles * (N / 128) >= num_sms()) return 128;
   if (N % 128 == 0 && N >= 1024) return 128;
   return (N % 64 == 0 && N % 128 != 0) ? 64 : ((M_tiles * ((N + 127) / 128) >= 96) ? 128 : 64);
+}
+
+// the output tensor maps of the QKV (q / k / v heads) and GEGLU (bf16 [M, N / 2]) tile epilogues
+static int bf16_out_maps(TcGemmParams& p, int epi_mode) {
+  const mmg_epilogue_args& e = p.epi.p;
+  int rc = MMG_OK;
+  if (epi_mode == TC_EPI_QKV) {
+    const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads;
+    uint64_t str[1] = {128}; uint32_t box[2] = {64, 16};
+    if (e.nq_heads) { uint64_t d[2] = {64, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
+    if (e.nk_heads) {
+      uint64_t d[2] = {64, seqs * (uint64_t)e.kv_rows};
+      rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
+      rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
+    }
+  } else if (epi_mode == TC_EPI_GEGLU) {
+    uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 16};
+    rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob);
+  }
+  return rc;
 }
 
 static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
@@ -60,19 +80,11 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
   uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
   int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
   if (epi_mode == TC_EPI_QKV) {
-    const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads;
-    uint64_t str[1] = {128}; uint32_t box[2] = {64, 16};
-    if (e.nq_heads) { uint64_t d[2] = {64, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
-    if (e.nk_heads) {
-      uint64_t d[2] = {64, seqs * (uint64_t)e.kv_rows};
-      rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
-      rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
-    }
+    rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
     return bn == 256 ? launch_tc<256, TC_EPI_QKV>(p, st) : launch_tc<128, TC_EPI_QKV>(p, st);
   }
   if (epi_mode == TC_EPI_GEGLU) {
-    uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 16};
-    rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
+    rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
     return launch_tc<256, TC_EPI_GEGLU>(p, st);
   }
   if (epi_mode != TC_EPI_REGS) {
@@ -241,6 +253,47 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   const int bn = pick_bn(p.num_m_tiles, a->N, a->epilogue);
   MMG_CHECK_ARG(bn == 64 || bn == 128 || bn == 256, "mmg_linear: unsupported N=%lld for this epilogue", (long long)a->N);
   return dispatch_tc(p, bn, a->w, a->N, a->K, a->ldw, st);
+}
+
+// e4m3 operands: the QKV and GEGLU tile epilogues only, at the tile widths and tile order the bf16 product of the same shape takes
+extern "C" int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->a && a->w && a->a_scale && a->w_scale, "mmg_linear_fp8: NULL operand or scale");
+  MMG_CHECK_ARG(a->dtype == MMG_E4M3, "mmg_linear_fp8: dtype %d is not MMG_E4M3", a->dtype);
+  MMG_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0 && a->K % 128 == 0, "mmg_linear_fp8: bad shape M=%lld N=%lld K=%lld (K %% 128 == 0)",
+                (long long)a->M, (long long)a->N, (long long)a->K);
+  MMG_CHECK_ARG(a->lda >= a->K && a->ldw >= a->K && a->lda % 16 == 0 && a->ldw % 16 == 0 && aligned16(a->a) && aligned16(a->w) &&
+                (reinterpret_cast<uintptr_t>(a->w_scale) & 7) == 0, "mmg_linear_fp8: operands need 16-byte rows, w_scale 8-byte alignment");
+  MMG_CHECK_ARG(a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_GEGLU, "mmg_linear_fp8: epilogue %d (QKV or GEGLU only)", a->epilogue);
+  int rc = validate_epilogue(a->epilogue, a->epi, a->N); if (rc) return rc;
+  const mmg_epilogue_args& e = a->epi;
+  const int64_t m_tiles = (a->M + TC_BM - 1) / TC_BM;
+  int bn = 256, epi_mode = TC_EPI_GEGLU;
+  if (a->epilogue == MMG_EPI_QKV) {
+    MMG_CHECK_ARG(e.out_dtype == MMG_BF16 && e.tokens > 0 && e.tokens % 32 == 0 && a->M % 128 == 0 && a->N % 128 == 0 && e.nk_heads == e.nv_heads &&
+                  (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out))),
+                  "mmg_linear_fp8: QKV needs bf16 outputs, tokens %% 32 == 0, M %% 128 == 0, N %% 128 == 0 (M=%lld N=%lld tokens=%d)",
+                  (long long)a->M, (long long)a->N, e.tokens);
+    bn = pick_bn(m_tiles, a->N, a->epilogue) == 256 ? 256 : 128;
+    epi_mode = TC_EPI_QKV;
+  } else {
+    MMG_CHECK_ARG(e.out_dtype == MMG_BF16 && a->N % 256 == 0 && e.ldo % 8 == 0 && aligned16(e.out),
+                  "mmg_linear_fp8: GEGLU needs bf16 out, N %% 256 == 0, ldo %% 8 == 0 (N=%lld)", (long long)a->N);
+  }
+  TcGemmParams p{};
+  p.M = a->M; p.N = a->N; p.num_kb = (int)(a->K / 128); p.mode = 0;
+  p.num_m_tiles = (int)m_tiles;
+  p.num_n_tiles = (int)(a->N / bn);
+  p.n_fast = ((int64_t)a->N * a->K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;   // the bf16 product's tile order
+  p.epi.p = a->epi; p.epi.kind = a->epilogue; p.epi.fast = 1; p.epi.M = a->M; p.epi.N = a->N;
+  p.a_scale = a->a_scale; p.w_scale = a->w_scale;
+  { uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda}; uint32_t box[2] = {128, TC_BM};
+    rc = make_tmap_u8(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc; }
+  { uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->N}; uint64_t str[1] = {(uint64_t)a->ldw}; uint32_t box[2] = {128, (uint32_t)bn};
+    rc = make_tmap_u8(&p.tma_b, a->w, 2, dims, str, box); if (rc) return rc; }
+  rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
+  if (epi_mode == TC_EPI_GEGLU) return launch_tc<256, TC_EPI_GEGLU, fp8e4>(p, st);
+  return bn == 256 ? launch_tc<256, TC_EPI_QKV, fp8e4>(p, st) : launch_tc<128, TC_EPI_QKV, fp8e4>(p, st);
 }
 
 extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {

@@ -1,6 +1,7 @@
-// wgmma / TMA GEMM for sm_90a:  C[M,N] = A[M,K] * W[N,K]^T, bf16 operands, fp32 accumulation in registers.
+// wgmma / TMA GEMM for sm_90a:  C[M,N] = A[M,K] * W[N,K]^T, bf16 (or e4m3) operands, fp32 accumulation in registers.
 //
 //   warp 0      : TMA producer  (one elected lane) — A tile 128x64 and W tile BNx64 per k-block, SWIZZLE_128B, STAGES-deep ring
+//                 (e4m3 operands: 128 x 128 and BN x 128 — the same 128-byte rows, so the ring, boxes and descriptors are unchanged)
 //   warps 4..11 : two consumer warpgroups.  Warpgroup g multiplies rows [64 g, 64 g + 64) of the tile (wgmma m64nBNk16, 4 per k-block,
 //                 accumulators in registers), then runs the fused Epilogue on those rows (EPI_MODE below): either from the accumulator
 //                 registers into per-warp shared-memory boxes and a TMA store / TMA reduction, or through a shared-memory staging buffer
@@ -57,6 +58,8 @@ struct alignas(64) TcGemmParams {
   int Ho, Wo, B;
   const int* skip_if_zero;  // optional device word written by an earlier kernel of the stream: 0 -> every CTA returns at once
   Epilogue epi;
+  const float* a_scale;     // e4m3 operands: the product of row r, column c is acc * a_scale[r] * w_scale[c] ([M], [N])
+  const float* w_scale;
 };
 
 // Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][register epilogues: staging, 2 x 64 x 132 fp32 | tile epilogues: per-warp
@@ -91,11 +94,30 @@ template <int BN> struct TcCfg {
 // TC_EPI_QKV: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 16 rows are 16 consecutive tokens of one
 // sequence and land on 16 consecutive rows of one head of q / k / v): one box and one TMA store per warp and head chunk.
 // TC_EPI_GEGLU: the GEGLU epilogue (bf16 out, BN == 256): two 64-column chunks make 64 outputs = one box per warp.
-template <int BN, int EPI_MODE>
+// e4m3 operands (TA = __nv_fp8_e4m3; QKV and GEGLU tile epilogues only): a k-block is 128 elements, four m64nBNk32 wgmma, and the tile
+// epilogue starts by dequantising the fragment with dequant_acc; everything after it is the bf16 code.
+template <int BN>
+__device__ __forceinline__ void dequant_acc(float (&acc)[BN / 2], const float* __restrict__ a_scale, const float* __restrict__ w_scale,
+                                            int64_t brow, int64_t M, int col0, int lane) {
+  const int q = lane & 3, fr = lane >> 2;
+  const float sa0 = brow + fr < M ? __ldg(a_scale + brow + fr) : 0.f;         // rows past M hold zero accumulators
+  const float sa1 = brow + fr + 8 < M ? __ldg(a_scale + brow + fr + 8) : 0.f;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const float2 ws = __ldg(reinterpret_cast<const float2*>(w_scale + col0 + 8 * j + 2 * q));
+    acc[4 * j] *= sa0 * ws.x; acc[4 * j + 1] *= sa0 * ws.y;
+    acc[4 * j + 2] *= sa1 * ws.x; acc[4 * j + 3] *= sa1 * ws.y;
+  }
+}
+
+template <int BN, int EPI_MODE, typename TA = bf16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   using namespace sm90;
   using Cfg = TcCfg<BN>;
+  constexpr bool FP8 = sizeof(TA) == 1;
+  constexpr int BK = 128 / (int)sizeof(TA);           // elements per k-block: one 128-byte row
+  static_assert(!FP8 || EPI_MODE == TC_EPI_QKV || EPI_MODE == TC_EPI_GEGLU, "e4m3 operands are dequantised by the QKV / GEGLU tile epilogues only");
   constexpr bool RED = EPI_MODE == TC_EPI_REDUCE || EPI_MODE == TC_EPI_TSTORE, RED_ADD = EPI_MODE == TC_EPI_REDUCE;   // TSTORE: same tiles, plain TMA store
   constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
   constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
@@ -155,12 +177,12 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
           uint8_t* sb = sa + Cfg::A_BYTES;
           mbar_expect_tx(full_bar + stage, STAGE_BYTES);
           if (p.mode == 0) {
-            tma_load_2d(sa, &p.tma_a[0], full_bar + stage, kb * TC_BK, m_blk * TC_BM);
+            tma_load_2d(sa, &p.tma_a[0], full_bar + stage, kb * BK, m_blk * TC_BM);
           } else {
             const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
             tma_load_4d(sa, &p.tma_a[p.tap_map[tap]], full_bar + stage, cc * TC_BK, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], b0);
           }
-          tma_load_2d(sb, &p.tma_b, full_bar + stage, kb * TC_BK, n_blk * BN);
+          tma_load_2d(sb, &p.tma_b, full_bar + stage, kb * BK, n_blk * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -208,7 +230,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
       if (RED_ADD && epi.kind == MMG_EPI_LNFOLD_RESIDUAL && (lane & 3) < 2 && brow + (lane >> 2) + 8 * (lane & 3) < p.M)
         epi.ln_row_stats(brow + (lane >> 2) + 8 * (lane & 3), ln_a, ln_b);
 
-      // ---- main loop: 4 wgmma (K = 16) per k-block; a ring slot goes back to the producer once the wgmma group after it was issued ----
+      // ---- main loop: 4 wgmma (K = 16, e4m3: 32) per k-block; a ring slot goes back to the producer once the wgmma group after it was issued ----
       int prev_stage = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(full_bar + stage, phase);
@@ -217,8 +239,10 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         const uint64_t bdesc = smem_desc_kmajor_sw128(sa + Cfg::A_BYTES);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)
-          Wgmma<BN>::template mma<0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+        for (int k = 0; k < 4; ++k) {
+          if constexpr (FP8) WgmmaE4m3<BN>::mma(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+          else Wgmma<BN>::template mma<0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+        }
         wgmma_commit();
         wgmma_wait<1>();
         if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
@@ -233,6 +257,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         // ---- tile epilogues, from the accumulator fragments (layout above the kernel) ----
         // acc[4 j + e] / acc[4 j + 2 + e] = rows fr / fr + 8 of the warp's 16 at column 8 j + 2 q + e of the tile; the boxes' rows are
         // 128 bytes whose 16-byte chunk k sits at k ^ (row & 7), and (fr + 8) & 7 == fr
+        if constexpr (FP8) dequant_acc<BN>(acc, p.a_scale, p.w_scale, brow, p.M, n_blk * BN, lane);
         const int q = lane & 3, fr = lane >> 2;
         const uint32_t rowa = (uint32_t)fr * 128u, rowb = rowa + 1024u;
         // the next free 2 KB box of the warp's tile: the store two boxes back has read it

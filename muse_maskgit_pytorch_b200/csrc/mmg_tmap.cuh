@@ -28,6 +28,9 @@ inline int make_tmap(CUtensorMap* m, CUtensorMapDataType dt, const void* base, i
 inline int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
   return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box);
 }
+inline int make_tmap_u8(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box);     // e4m3 operands: TMA moves bytes
+}
 inline int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
   return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box);
 }

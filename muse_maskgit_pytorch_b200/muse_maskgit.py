@@ -37,6 +37,30 @@ class LayerNorm(nn.Module):
         self.register_buffer("beta", torch.zeros(dim))
 
 
+def _geglu_interleave(w1, Fp):
+    """(2F, K) feed-forward weight (rows [0, F) gelu arm, [F, 2F) gate) -> (2 Fp, K) in the GEGLU epilogue's row order: arm unit u at row
+    64 (u // 32) + u % 32, its gate 32 rows further; the padding rows past F are zero.  Works on a trailing-dim-free (2F,) vector too."""
+    F_ = w1.shape[0] // 2
+    out = torch.zeros((2 * Fp,) + tuple(w1.shape[1:]), device=w1.device, dtype=w1.dtype)
+    xi = torch.arange(Fp, device=w1.device).view(-1, 32)
+    dst_x = (xi // 32 * 64 + xi % 32).reshape(-1)                       # unit u -> row 64*(u//32) + u%32 ; gate -> +32
+    valid = torch.arange(Fp, device=w1.device) < F_
+    out[dst_x[valid]] = w1[:F_]
+    out[dst_x[valid] + 32] = w1[F_:]
+    return out
+
+
+def quantize_rows_e4m3(w):
+    """Per-row e4m3 quantisation of an fp32 matrix (precision="fp8" weights, and the rounding of mmg_layernorm_fp8):
+    amax = max |w[r]|, q[r] = rne_satfinite_e4m3(w[r] * (448 / amax)) (0 where amax == 0), scale[r] = amax / 448, so q * scale ~= w.
+    Returns (q float8_e4m3fn, scale fp32)."""
+    w = w.float()
+    amax = w.abs().amax(dim=1)
+    inv = torch.where(amax > 0, 448.0 / torch.where(amax > 0, amax, torch.ones_like(amax)), torch.zeros_like(amax))
+    q = (w * inv[:, None]).clamp(-448.0, 448.0).to(torch.float8_e4m3fn)     # clamp first: the cast of a value past 448 is NaN
+    return q.contiguous(), (amax / 448.0).contiguous()
+
+
 def _ff_params(dim, mult=4):
     inner = int(dim * mult * 2 / 3)                       # ref: muse_maskgit_pytorch.py:82
     return nn.Sequential(LayerNorm(dim), nn.Linear(dim, inner * 2, bias=False), nn.Identity(), LayerNorm(inner),
@@ -89,6 +113,8 @@ class Transformer(nn.Module):
         self.self_cond = self_cond
         self.self_cond_to_init_embed = _ff_params(dim)
         self.precision = precision or "bf16"
+        if self.precision == "fp8" and dim % 128 != 0:
+            raise ValueError(f'precision="fp8" needs dim % 128 == 0 (one 128-element e4m3 k-block per wgmma step); got dim = {dim}')
         self._pack = None
         # nn.Module.load_state_dict on a PARENT never calls a child's load_state_dict override, but it does run the child's
         # post hooks: the packed weights are dropped whichever module the load was started from
@@ -114,10 +140,11 @@ class Transformer(nn.Module):
         return sig
 
     def _adt(self):
-        return torch.bfloat16 if self.precision == "bf16" else torch.float32
+        """operand dtype of every product that is not e4m3: bf16 for "bf16" and "fp8", fp32 (3-way bf16 splits) otherwise"""
+        return torch.bfloat16 if self.precision in ("bf16", "fp8") else torch.float32
 
     def _packed(self):
-        if self._pack is not None and self._pack["adt"] == self._adt():
+        if self._pack is not None and self._pack["adt"] == self._adt() and self._pack.get("fp8", False) == (self.precision == "fp8"):
             return self._pack
         dev = self.token_emb.weight.device
         assert dev.type == "cuda", "Transformer runs on CUDA only (libmmg.so); there is no CPU path"
@@ -132,18 +159,13 @@ class Transformer(nn.Module):
         tb = self.transformer_blocks
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
         wa = lambda t: t.detach().to(dev, adt).contiguous()
-        P = dict(adt=adt, layers=[])
+        fp8 = self.precision == "fp8"
+        P = dict(adt=adt, fp8=fp8, layers=[])
 
         def ff_pack(ff):
             F_ = ff[3].gamma.shape[0]
             Fp = _round_up(F_, 64)
-            w1 = ff[1].weight.detach().to(dev, torch.float32)                  # (2F, dim): rows [0,F) -> gelu arm, [F,2F) -> gate
-            w1p = torch.zeros((2 * Fp, w1.shape[1]), device=dev)
-            xi = torch.arange(Fp, device=dev).view(-1, 32)
-            dst_x = (xi // 32 * 64 + xi % 32).reshape(-1)                       # unit u -> row 64*(u//32) + u%32 ; gate -> +32
-            valid = torch.arange(Fp, device=dev) < F_
-            w1p[dst_x[valid]] = w1[:F_]
-            w1p[dst_x[valid] + 32] = w1[F_:]
+            w1p = _geglu_interleave(ff[1].weight.detach().to(dev, torch.float32), Fp)   # (2F, dim): rows [0,F) -> gelu arm, [F,2F) -> gate
             g3 = torch.zeros(Fp, device=dev); g3[:F_] = ff[3].gamma.detach().float()
             w2 = torch.zeros((ff[4].weight.shape[0], Fp), device=dev); w2[:, :F_] = ff[4].weight.detach().float()
             out = dict(F=F_, Fp=Fp, g0=f32(ff[0].gamma), w1=w1p.to(adt).contiguous(), g3=g3.contiguous(), w2=w2.to(adt).contiguous())
@@ -151,6 +173,9 @@ class Transformer(nn.Module):
                 # LayerNorm(inner) folded through the second linear: LN(h) W2^T = rstd * (h (W2*gamma)^T - mean * cvec), cvec = rowsum(W2*gamma)
                 w2f = (w2 * g3[None, :]).to(adt).contiguous()
                 out["w2f"], out["cvec"] = w2f, w2f.float().sum(dim=1).contiguous()
+            if fp8:      # FF1 on e4m3: rows quantised after the interleave, so the scales follow it
+                out["w1_8"], out["s1"] = quantize_rows_e4m3(w1p)
+                del out["w1"]
             return out
 
         for attn, cross, ff in tb.layers:
@@ -169,6 +194,9 @@ class Transformer(nn.Module):
                         # cross-attention output when every context key is masked: to_out(null_v)  (weight 1.0 on the null key)
                         null_out=f32(cross.null_kv[1].detach().float().reshape(1, -1) @ cross.to_out.weight.detach().float().t()).reshape(-1)),
                 ff=ff_pack(ff))
+            if fp8:      # self QKV and cross q on e4m3, one scale per output row
+                lay["sa"]["wqkv_8"], lay["sa"]["s_qkv"] = quantize_rows_e4m3(lay["sa"].pop("wqkv"))
+                lay["ca"]["wq_8"], lay["ca"]["s_q"] = quantize_rows_e4m3(lay["ca"].pop("wq"))
             P["layers"].append(lay)
         P["gf"] = f32(tb.norm.gamma)
         P["tok"], P["pos"] = f32(self.token_emb.weight), f32(self.pos_emb.weight)
@@ -225,7 +253,7 @@ class Transformer(nn.Module):
 
     # ----- the block stack over R = nb*b*n rows -------------------------------------------------------------------------
     def _workspace(self, nb, b, n, dev):
-        key = (nb, b, n, str(dev), self._adt())
+        key = (nb, b, n, str(dev), self._adt(), self.precision == "fp8")
         cache = self.__dict__.setdefault("_ws", {})        # a few shapes stay resident (e.g. 2-branch decode + 1-branch self-critic)
         if key in cache:
             return cache[key]
@@ -245,6 +273,9 @@ class Transformer(nn.Module):
                   h=torch.empty((R, Fp), device=dev, dtype=adt),
                   hn=torch.empty((R, Fp), device=dev, dtype=adt),
                   stats=torch.zeros((R, Fp // 32, 2), device=dev, dtype=torch.float32))   # per-chunk (sum, sumsq) of the GEGLU output
+        if P["fp8"]:     # the quantising LayerNorm's output: e4m3 rows and one scale per row (the A operand of the fp8 products)
+            ws["xq"] = torch.empty((R, dim), device=dev, dtype=torch.float8_e4m3fn)
+            ws["xs"] = torch.empty((R,), device=dev, dtype=torch.float32)
         if len(cache) >= 4:
             cache.pop(next(iter(cache)))
         cache[key] = ws
@@ -272,13 +303,24 @@ class Transformer(nn.Module):
         else:
             ops.embed(ids.contiguous(), P["tok"], P["pos"], x, n=n, copies=nb)
         live = [j for j in range(nb) if not ctx["all_masked"][j]]
+
+        def norm(rows, g, fp8, **kw):
+            """LayerNorm of x[rows] into the A operand of the next product (xn; fp8: e4m3 rows + row scales)"""
+            if fp8:
+                ops.layernorm_fp8(x[rows], g, ws["xq"][rows], ws["xs"][rows], **kw)
+            else:
+                ops.layernorm(x[rows], g, xn[rows], **kw)
+
         for li, lay in enumerate(P["layers"]):
             sa, ca, ff = lay["sa"], lay["ca"], lay["ff"]
             # --- self attention (all branches) ---
-            ops.layernorm(x, sa["g"], xn)
+            norm(slice(None), sa["g"], "wqkv_8" in sa)
             epi = ops.qkv_epilogue(adt, heads, n, q=q, k=k, v=v, q_scale=sa["qs"], k_scale=sa["ks"], key_off=1,
                                    null_k=sa["nk"], null_v=sa["nv"])
-            ops.linear(xn, sa["wqkv"], None, epilogue=ops.EPI_QKV, epi=epi)
+            if "wqkv_8" in sa:
+                ops.linear_fp8(ws["xq"], ws["xs"], sa["wqkv_8"], sa["s_qkv"], None, epilogue=ops.EPI_QKV, epi=epi)
+            else:
+                ops.linear(xn, sa["wqkv"], None, epilogue=ops.EPI_QKV, epi=epi)
             ops.attention(q, k, v, ao, nb * b, heads, n + 1, logit_bound=sa["bound"])
             ops.linear(ao, sa["wo"], x, epilogue=ops.EPI_RESIDUAL, resid=x)
             # --- cross attention ---
@@ -287,25 +329,29 @@ class Transformer(nn.Module):
             if live:
                 assert live == list(range(len(live))), "live branches must come first"
                 Rl = len(live) * bn
-                ops.layernorm(x[:Rl], ca["g"], xn[:Rl])
+                norm(slice(0, Rl), ca["g"], "wq_8" in ca)
                 epi = ops.qkv_epilogue(adt, heads, n, q=q[:len(live) * b * heads], q_scale=ca["qs"])
-                ops.linear(xn[:Rl], ca["wq"], None, epilogue=ops.EPI_QKV, epi=epi)
+                if "wq_8" in ca:
+                    ops.linear_fp8(ws["xq"][:Rl], ws["xs"][:Rl], ca["wq_8"], ca["s_q"], None, epilogue=ops.EPI_QKV, epi=epi)
+                else:
+                    ops.linear(xn[:Rl], ca["wq"], None, epilogue=ops.EPI_QKV, epi=epi)
                 ops.attention(q[:len(live) * b * heads], kc[:len(live) * b * heads], vc[:len(live) * b * heads], ao[:Rl], len(live) * b, heads,
                               ctx["m"] + 1, key_mask=ctx["key_mask"][:len(live) * b], logit_bound=ca["bound"])
                 ops.linear(ao[:Rl], ca["wo"], x[:Rl], epilogue=ops.EPI_RESIDUAL, resid=x[:Rl])
             # --- feed forward (the constant null-branch cross-attention term is folded into this LayerNorm) ---
+            ff8 = "w1_8" in ff
             if pending_add and sorted(pending_add) == list(range(min(pending_add), nb)):
                 # one launch for all branches: rows of the all-masked (null) branches get += to_out(null_v) before the norm
-                ops.layernorm(x, ff["g0"], xn, add=ca["null_out"], x_out=x, add_from=min(pending_add) * bn)
+                norm(slice(None), ff["g0"], ff8, add=ca["null_out"], x_out=x, add_from=min(pending_add) * bn)
             elif not pending_add:
-                ops.layernorm(x, ff["g0"], xn)
+                norm(slice(None), ff["g0"], ff8)
             else:
                 for j in range(nb):
-                    xs = x[j * bn:(j + 1) * bn]
+                    rows = slice(j * bn, (j + 1) * bn)
                     if j in pending_add:
-                        ops.layernorm(xs, ff["g0"], xn[j * bn:(j + 1) * bn], add=pending_add[j], x_out=xs)
+                        norm(rows, ff["g0"], ff8, add=pending_add[j], x_out=x[rows])
                     else:
-                        ops.layernorm(xs, ff["g0"], xn[j * bn:(j + 1) * bn])
+                        norm(rows, ff["g0"], ff8)
             self._ff_tail(xn, ff, x, ws, R)
         return x
 
@@ -317,7 +363,10 @@ class Transformer(nn.Module):
             stats = ws["stats"][:R, :ff["Fp"] // 32]     # per-chunk (sum, sumsq) partials written by FF1's epilogue, added in order by FF2's
             if stats.shape[1] != ws["stats"].shape[1]:
                 stats = stats.contiguous()
-            ops.linear(xn[:R], ff["w1"], h, epilogue=ops.EPI_GEGLU, row_stats=stats)
+            if "w1_8" in ff:     # fp8: the quantising LayerNorm left e4m3 rows [0, R) and their scales in the workspace
+                ops.linear_fp8(ws["xq"][:R], ws["xs"][:R], ff["w1_8"], ff["s1"], h, epilogue=ops.EPI_GEGLU, row_stats=stats)
+            else:
+                ops.linear(xn[:R], ff["w1"], h, epilogue=ops.EPI_GEGLU, row_stats=stats)
             ops.linear(h, ff["w2f"], x[:R], epilogue=ops.EPI_LNFOLD_RESIDUAL, bias=ff["cvec"], resid=x[:R], row_stats=stats, ln_width=ff["F"])
             return
         ops.linear(xn[:R], ff["w1"], h, epilogue=ops.EPI_GEGLU)
@@ -327,7 +376,10 @@ class Transformer(nn.Module):
     def _ff(self, inp, ff, x_acc, ws, R):
         """x_acc += FeedForward(inp)   (self-conditioning embed, muse_maskgit_pytorch.py:325-328)"""
         xn = ws["xn"][:R]
-        ops.layernorm(inp, ff["g0"], xn)
+        if "w1_8" in ff:
+            ops.layernorm_fp8(inp, ff["g0"], ws["xq"][:R], ws["xs"][:R])
+        else:
+            ops.layernorm(inp, ff["g0"], xn)
         self._ff_tail(xn, ff, x_acc, ws, R)
 
     # ----- public API ---------------------------------------------------------------------------------------------------
@@ -544,6 +596,9 @@ class MaskGit(nn.Module):
                  fmap_size=None, temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False,
                  force_not_use_token_critic=False, timesteps=18, cond_scale=3, critic_noise_scale=1, return_ids=False):
         """ref: muse_maskgit_pytorch.py:491-621.  Returns fp32 NCHW images (b, 3, H, W), unclamped."""
+        if self.use_native_step and self.transformer.precision == "fp8":
+            raise ValueError('use_native_step=True runs mmg_decode_step, whose weights carry no fp8 scales: it cannot run precision="fp8"; '
+                             "set use_native_step = False")
         was_training = self.training
         self.eval()
         try:

@@ -90,6 +90,39 @@ def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, 
     return out
 
 
+def linear_fp8(a, a_scale, w, w_scale, out, epilogue=EPI_GEGLU, epi=None, row_stats=None):
+    """e4m3 product with per-row scales: out = epilogue((a @ w.T) * a_scale[:, None] * w_scale[None, :]).  a [M, K], w [N, K] float8_e4m3fn,
+    a_scale [M], w_scale [N] fp32; epilogue EPI_QKV (pass `epi` from qkv_epilogue) or EPI_GEGLU (bf16 `out`, optional row_stats)."""
+    _chk(a, "a"); _chk(w, "w"); _chk(a_scale, "a_scale"); _chk(w_scale, "w_scale")
+    assert a.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn and w.shape[1] == a.shape[1]
+    assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    assert a_scale.numel() >= a.shape[0] and w_scale.numel() >= w.shape[0]
+    args = L.LinearFp8Args()
+    args.a = a.data_ptr(); args.w = w.data_ptr(); args.a_scale = a_scale.data_ptr(); args.w_scale = w_scale.data_ptr()
+    args.M, args.K = a.shape; args.N = w.shape[0]; args.lda = a.stride(0); args.ldw = w.stride(0)
+    args.dtype = L.E4M3; args.epilogue = epilogue
+    if epi is None:
+        assert out is not None and out.shape[-1] * 2 >= args.N, "GEGLU writes N / 2 columns per row: `out` is too narrow"
+        epi = _epi(out, out.stride(0), row_stats=row_stats)
+    args.epi = epi
+    L.call("mmg_linear_fp8", args)
+    return out
+
+
+def layernorm_fp8(x, gamma, y, row_scale, add=None, x_out=None, add_from=0):
+    """Quantising LayerNorm: y (float8_e4m3fn [rows, >= width]) * row_scale[:, None] ~= LN(x (+ add on rows >= add_from)) * gamma, with
+    the rounding of mmg_layernorm_fp8 (per-row scale max|y| / 448, round to nearest even, saturating).  x fp32 [rows, width]."""
+    _chk(x, "x"); _chk(y, "y"); _chk(row_scale, "row_scale")
+    assert x.dtype == torch.float32 and y.dtype == torch.float8_e4m3fn and row_scale.dtype == torch.float32
+    assert y.shape[0] >= x.shape[0] and row_scale.numel() >= x.shape[0]
+    a = L.LayerNormFp8Args()
+    a.x = x.data_ptr(); a.y = y.data_ptr(); a.row_scale = row_scale.data_ptr(); a.gamma = gamma.data_ptr()
+    a.add = L.ptr(add); a.x_out = L.ptr(x_out); a.add_from = add_from
+    a.rows, a.width = x.shape; a.ldx = x.stride(0); a.ldy = y.stride(0)
+    L.call("mmg_layernorm_fp8", a)
+    return y
+
+
 def qkv_epilogue(dtype_t, heads, tokens, q=None, k=None, v=None, q_scale=None, k_scale=None, key_off=0, null_k=None, null_v=None):
     """Epilogue block for MMG_EPI_QKV.  q [BH, q_rows, 64]; k, v [BH, kv_rows, 64]."""
     e = L.EpilogueArgs()

@@ -124,6 +124,8 @@ class VQGanVAE(nn.Module):
         self.use_vgg_and_gan = False          # no discriminator / VGG in this inference build (dropped by copy_for_eval in the reference)
         self.discr, self._vgg = None, None
         self.precision = precision or "bf16"
+        if self.precision == "fp8":
+            raise ValueError('VQGanVAE has no fp8 mode: use precision="bf16" (the transformer\'s precision="fp8" runs over a bf16 VAE)')
         self._pack = None
         # both hooks also fire when a PARENT module (MaskGit, Muse) loads a checkpoint: checkpoints written by the reference carry
         # discriminator / VGG tensors (vqgan_vae.py:344-348, dropped by copy_for_eval :394-403) that are not part of inference
