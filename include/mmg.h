@@ -261,6 +261,23 @@ typedef struct {
 } mmg_remask_frozen_args;
 int mmg_remask_frozen(const mmg_remask_frozen_args* a, void* stream);
 
+/* selection of one mask-free editing iteration (MaskGit.edit).  Row b takes one uniform key per position: u[b, p] when u != NULL,
+ * else Philox4x32-10(counter = (0xFFFFFFFE, iteration, row_offset + b*n + p), key = seed + *seed_dev) >> 8 * 2^-24 (disjoint from
+ * the gumbel stream, c0 = vocabulary index, and the critic stream, c0 = 0xFFFFFFFF).  Among its editable positions (keep == 0)
+ * it selects the num_select[b] largest keys (ties: lowest position first), writes frozen_out[b, p] = 1 at every other position
+ * and 0 at the selected ones, mask_id at the selected ids and 0 into every score of the row.  A following mmg_remask_frozen
+ * with frozen = frozen_out and count num_select[b] re-masks exactly the selected positions.  num_select is read on the device. */
+typedef struct {
+  int64_t* ids; float* scores; uint8_t* frozen_out;   /* [B, n], [B, n], [B, n] (1 = keep)                         */
+  const uint8_t* keep;                                /* [B, n], 1 = not editable                                  */
+  const int32_t* num_select;                          /* [B] device counts, each <= n                              */
+  const float* u;                                     /* [B, n] injected keys or NULL                              */
+  uint64_t seed; const uint64_t* seed_dev;            /* seed_dev optional, as in mmg_logits_sample_args          */
+  int64_t row_offset;                                 /* global position of this call's first token                */
+  int32_t B, n, iteration, _pad; int64_t mask_id;
+} mmg_edit_select_args;
+int mmg_edit_select(const mmg_edit_select_args* a, void* stream);
+
 /* Final LayerNorm + classifier-free-guidance combine on the masked rows only, in embedding space:
  *   e[j] = LN(x_null[r]) + (LN(x_cond[r]) - LN(x_null[r])) * cond_scale,  r = b*n + masked_pos[b, j]
  * (to_logits is linear and bias-free, so W e == null + (cond - null) * scale of muse_maskgit_pytorch.py:254).    */

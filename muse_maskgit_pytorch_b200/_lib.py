@@ -84,6 +84,11 @@ class RemaskFrozenArgs(C.Structure):
                 ("mask_id", i64)]
 
 
+class EditSelectArgs(C.Structure):
+    _fields_ = [("ids", vp), ("scores", vp), ("frozen_out", vp), ("keep", vp), ("num_select", vp), ("u", vp), ("seed", u64), ("seed_dev", vp),
+                ("row_offset", i64), ("B", i32), ("n", i32), ("iteration", i32), ("_pad", i32), ("mask_id", i64)]
+
+
 class FinalEmbedArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("masked_pos", vp), ("e", vp), ("e_dtype", i32),
                 ("B", i32), ("n", i32), ("num_masked", i32), ("dim", i32), ("cond_scale", f32)]
@@ -177,7 +182,7 @@ EXPORTS = {
     "mmg_logits_sample": LogitsSampleArgs, "mmg_vq_lfq_encode": LfqEncodeArgs, "mmg_vq_l2_argmin": L2ArgminArgs,
     "mmg_vq_decode_codes": DecodeCodesArgs, "mmg_cast": CastArgs, "mmg_split3": Split3Args, "mmg_critic_score": CriticScoreArgs,
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,
-    "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs,
+    "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs, "mmg_edit_select": EditSelectArgs,
     "mmg_logits_xent": LogitsXentArgs, "mmg_logits_xent_rows": LogitsXentRowsArgs,
     "mmg_linear_fp8": LinearFp8Args, "mmg_layernorm_fp8": LayerNormFp8Args,
 }

@@ -13,7 +13,7 @@ extern "C" int mmg_sizeof(const char* name) {
 #define SZ(n) if (!strcmp(name, "mmg_" #n)) return (int)sizeof(mmg_##n##_args)
   SZ(linear); SZ(conv2d); SZ(conv_transpose2d); SZ(conv_in); SZ(groupnorm); SZ(layernorm); SZ(embed); SZ(attention);
   SZ(remask); SZ(final_embed); SZ(logits_sample); SZ(vq_lfq_encode); SZ(vq_l2_argmin); SZ(vq_decode_codes); SZ(cast); SZ(split3); SZ(critic_score); SZ(ff_geglu); SZ(decode_step); SZ(logits_fused);
-  SZ(t5_attention); SZ(rmsnorm); SZ(remask_frozen); SZ(logits_xent); SZ(logits_xent_rows); SZ(linear_fp8); SZ(layernorm_fp8);
+  SZ(t5_attention); SZ(rmsnorm); SZ(remask_frozen); SZ(edit_select); SZ(logits_xent); SZ(logits_xent_rows); SZ(linear_fp8); SZ(layernorm_fp8);
 #undef SZ
   if (!strcmp(name, "mmg_epilogue")) return (int)sizeof(mmg_epilogue_args);
   if (!strcmp(name, "mmg_attn_weights")) return (int)sizeof(mmg_attn_weights);

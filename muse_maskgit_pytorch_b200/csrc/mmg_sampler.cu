@@ -368,6 +368,24 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// rank selection of one batch row held in shared memory: flag[i] = 1 for the num_masked largest sc[i] (ties: lowest
+// position).  FROZEN: positions with fz[i] != 0 are neither ranked nor selected.  Thread tid writes flag[tid + 256 k].
+// ---------------------------------------------------------------------------------------------------------------
+template <bool FROZEN>
+__device__ __forceinline__ void rank_select(const float* sc, const uint8_t* fz, int* flag, int n, int num_masked, int tid) {
+  for (int i = tid; i < n; i += 256) {
+    const float s = sc[i]; int rank = 0;
+    if (FROZEN) {
+      for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += !fz[j] && ((t > s) || (t == s && j < i)); }
+      flag[i] = !fz[i] && rank < num_masked;
+    } else {
+      for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += (t > s) || (t == s && j < i); }
+      flag[i] = rank < num_masked;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // re-mask: per batch row pick the num_masked largest scores (ties: lowest position), scatter mask_id, reset scores.
 // FROZEN (inpainting): positions with frozen[b, i] != 0 are neither ranked nor selected; row b selects
 // min(num_masked_dev[b], rows) positions and pads masked_pos[b, c_b .. rows) with its first frozen position.
@@ -380,16 +398,7 @@ __device__ __forceinline__ void remask_row(int64_t* __restrict__ ids, float* __r
   for (int i = tid; i < n; i += 256) sc[i] = scores[(int64_t)b * n + i];
   if (FROZEN) for (int i = tid; i < n; i += 256) fz[i] = frozen[(int64_t)b * n + i] != 0;
   __syncthreads();
-  for (int i = tid; i < n; i += 256) {
-    const float s = sc[i]; int rank = 0;
-    if (FROZEN) {
-      for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += !fz[j] && ((t > s) || (t == s && j < i)); }
-      flag[i] = !fz[i] && rank < num_masked;
-    } else {
-      for (int j = 0; j < n; ++j) { const float t = sc[j]; rank += (t > s) || (t == s && j < i); }
-      flag[i] = rank < num_masked;
-    }
-  }
+  rank_select<FROZEN>(sc, fz, flag, n, num_masked, tid);
   __syncthreads();
   // ordered compaction: each thread owns a contiguous chunk
   const int per = (n + 255) / 256, lo = tid * per, hi = min(n, lo + per);
@@ -438,6 +447,43 @@ remask_frozen_kernel(const mmg_remask_frozen_args a) {
   const int limit = count < a.rows ? (count > 0 ? count : 0) : a.rows;
   remask_row<true>(a.ids, a.scores, a.masked_pos, a.frozen, a.n, limit, a.rows, a.mask_id, sc, reinterpret_cast<int*>(sc + a.n),
                    reinterpret_cast<uint8_t*>(sc + 2 * a.n), woff);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// mask-free editing (MaskGit.edit): row b draws one uniform key per position (injected, or Philox with counter
+// (0xFFFFFFFE, iteration, global position) next to the gumbel (c0 = vocabulary index) and critic (c0 = 0xFFFFFFFF) streams),
+// selects the num_select[b] largest keys among its editable positions (keep == 0; ties: lowest position), writes
+// frozen_out = !selected, mask_id at the selected ids and 0 into every score of the row.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+edit_select_kernel(const mmg_edit_select_args a) {
+  extern __shared__ float sc[];                       // [n] keys, [n] flags (as int), [n] keep bytes
+  pdl_wait(); pdl_trigger();
+  const int b = blockIdx.x, tid = threadIdx.x, n = a.n;
+  int* flag = reinterpret_cast<int*>(sc + n);
+  uint8_t* fz = reinterpret_cast<uint8_t*>(sc + 2 * n);
+  const int64_t base = (int64_t)b * n;
+  const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  for (int i = tid; i < n; i += 256) {
+    float u;
+    if (a.u) u = a.u[base + i];
+    else {
+      const int64_t grow = a.row_offset + base + i;
+      u = (float)(philox_first(0xFFFFFFFEu, (uint32_t)a.iteration, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed,
+                               (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
+    }
+    sc[i] = u;
+    fz[i] = a.keep[base + i] != 0;
+  }
+  __syncthreads();
+  const int count = a.num_select[b];
+  rank_select<true>(sc, fz, flag, n, count > 0 ? count : 0, tid);
+  for (int i = tid; i < n; i += 256) {                // flag[i] was written by this thread
+    const bool sel = flag[i] != 0;
+    a.frozen_out[base + i] = !sel;
+    if (sel) a.ids[base + i] = a.mask_id;
+    a.scores[base + i] = 0.f;
+  }
 }
 
 
@@ -537,6 +583,19 @@ extern "C" int mmg_remask_frozen(const mmg_remask_frozen_args* a, void* stream) 
   static const cudaError_t attr = cudaFuncSetAttribute(remask_frozen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 9);
   if (attr != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(remask_frozen): %s", cudaGetErrorString(attr));
   MMG_CUDA(launch_pdl(remask_frozen_kernel, dim3(a->B), dim3(256), smem, st, *a));
+  MMG_LAUNCHED();
+  return MMG_OK;
+}
+
+extern "C" int mmg_edit_select(const mmg_edit_select_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->ids && a->scores && a->frozen_out && a->keep && a->num_select, "mmg_edit_select: NULL pointer");
+  MMG_CHECK_ARG(a->B >= 0 && a->n > 0 && a->n <= 16384 && a->iteration >= 0, "mmg_edit_select: B=%d n=%d iteration=%d", a->B, a->n, a->iteration);
+  if (a->B == 0) return MMG_OK;
+  const size_t smem = (size_t)a->n * 9;                 // keys, flags, keep bytes
+  static const cudaError_t attr = cudaFuncSetAttribute(edit_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 9);
+  if (attr != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(edit_select): %s", cudaGetErrorString(attr));
+  MMG_CUDA(launch_pdl(edit_select_kernel, dim3(a->B), dim3(256), smem, st, *a));
   MMG_LAUNCHED();
   return MMG_OK;
 }

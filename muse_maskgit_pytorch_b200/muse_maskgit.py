@@ -626,9 +626,7 @@ class MaskGit(nn.Module):
         b = len(texts)
         device = next(self.parameters()).device
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
-        if not isinstance(images, torch.Tensor) or tuple(images.shape) != (b, self.vae.channels, self.image_size, self.image_size):
-            raise ValueError(f"images must be a (b, {self.vae.channels}, {self.image_size}, {self.image_size}) tensor for b = {b} texts, got "
-                             f"{tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__}")
+        self._check_images(images, b)
         regen = regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1)
         counts = [int(c) for c in regen.sum(dim=1).tolist()]                      # N_b: the call's one device-to-host read for a GPU mask
         n_max = max(counts, default=0)
@@ -644,6 +642,64 @@ class MaskGit(nn.Module):
                                   force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, inpaint=inp)
         finally:
             self.train(was_training)
+
+    @torch.no_grad()
+    def edit(self, texts: List[str], images: torch.Tensor, mask: Optional[torch.Tensor] = None, iterations=8, fraction=0.1, timesteps=4,
+             cond_images: Optional[torch.Tensor] = None, temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False,
+             force_not_use_token_critic=False, cond_scale=3, critic_noise_scale=1, return_ids=False):
+        """Mask-free editing (an extension, as inpaint() is; the Muse paper's third editing mode): moves `images` towards the prompts while
+        keeping their layout, by repeatedly re-masking a random subset of their tokens and resampling it.
+
+        images: fp32 NCHW (b, C, image_size, image_size), encoded once as ids0 = vae.encode_ids(images).  mask: the editable region in any
+        form inpaint() takes (True = editable); None = the whole image.  E_b is image b's editable tokens, N_b = |E_b|, and
+        r_b = max(int(fraction * N_b), 1) when N_b > 0, else 0 (host Python floats, the same in every iteration).
+        Iteration i (0 <= i < iterations):
+          1. image b draws one key per position and selects the r_b editable positions with the largest keys (ties: lowest position);
+          2. exactly inpaint()'s token loop with the selection as the regenerated region: `timesteps` decode steps, image b on the schedule
+             max(int(noise_schedule(t) * r_b), 1), the temperature annealed over the iteration's steps, scores and the self-conditioning
+             embedding reset at the start of the iteration.  Decode step s has the global step index i * timesteps + s, which keys the
+             sampler's Philox stream and is the step passed to `sampler_noise_fn`.
+        Keys: libmmg's Philox with counter (0xFFFFFFFE, i, global position) and the call's seed (disjoint from the gumbel and critic noise,
+        independent of how the batch is sharded over `row_offset`); with `sampler_noise_fn` set, sampler_noise_fn(i * timesteps, (b, n)),
+        drawn before that iteration's first gumbel draw.  sampler_rng = "aten" has no reference stream for the keys and raises ValueError.
+        Tokens outside the selections keep their ids bit for bit; the token grid stays on the device for the whole call (one encode, one
+        decode).  iterations = 1, fraction = 1 is inpaint(mask) (generate() for mask=None) under the same seed; iterations = 0 returns
+        ids0 and its decode.  The defaults (8 iterations of 4 steps on 10 % of the tokens) are this project's provisional choice, not
+        settings from the paper.  Returns what generate() returns.  `use_native_step` does not apply here, as for inpaint()."""
+        if isinstance(iterations, bool) or not isinstance(iterations, int) or iterations < 0:
+            raise ValueError(f"iterations must be an int >= 0, got {iterations!r}")
+        if not 0 < fraction <= 1:
+            raise ValueError(f"fraction must lie in (0, 1], got {fraction!r}")
+        if isinstance(timesteps, bool) or not isinstance(timesteps, int) or timesteps < 1:
+            raise ValueError(f"timesteps must be an int >= 1, got {timesteps!r}")
+        if self.sampler_rng == "aten":
+            raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
+        b = len(texts)
+        device = next(self.parameters()).device
+        fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
+        self._check_images(images, b)
+        editable = (torch.ones((b, fmap_size ** 2), dtype=torch.bool) if mask is None
+                    else regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1))
+        counts = [int(c) for c in editable.sum(dim=1).tolist()]                   # N_b
+        select = [max(int(fraction * c), 1) if c else 0 for c in counts]          # r_b
+        table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in select]
+        inp = dict(n_max=max(select, default=0), iterations=iterations,
+                   dev=dict(images=images.to(device, torch.float32).contiguous(),
+                            keep=(~editable).to(device=device, dtype=torch.uint8).contiguous(),
+                            num_select=torch.tensor(select, dtype=torch.int32).to(device),
+                            counts=torch.tensor(table, dtype=torch.int32).t().contiguous().to(device)))       # [timesteps, b]
+        was_training = self.training
+        self.eval()
+        try:
+            return self._generate(texts, None, cond_images, None, temperature, topk_filter_thres, can_remask_prev_masked,
+                                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, inpaint=inp)
+        finally:
+            self.train(was_training)
+
+    def _check_images(self, images, b):
+        if not isinstance(images, torch.Tensor) or tuple(images.shape) != (b, self.vae.channels, self.image_size, self.image_size):
+            raise ValueError(f"images must be a (b, {self.vae.channels}, {self.image_size}, {self.image_size}) tensor for b = {b} texts, got "
+                             f"{tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__}")
 
     def _generate(self, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
                   force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, seed=None, inpaint=None):
@@ -684,7 +740,7 @@ class MaskGit(nn.Module):
                        timesteps=timesteps, cond_scale=cond_scale, b=b, use_critic=use_critic, critic_noise_scale=critic_noise_scale,
                        score_all=bool(can_remask_prev_masked) and not use_critic, aten=aten)
         if inpaint is not None:
-            body = partial(body, inpaint_rows=inpaint["n_max"])
+            body = partial(body, inpaint_rows=inpaint["n_max"], edit_iterations=inpaint.get("iterations"))
         inp_dev = None if inpaint is None else inpaint["dev"]
         inp_kw = lambda d: {} if inpaint is None else dict(inpaint=d)
         rerun = lambda: self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres,
@@ -701,7 +757,9 @@ class MaskGit(nn.Module):
                float(temperature), float(topk_filter_thres), int(timesteps), float(cond_scale), int(self.row_offset), tr.precision, self.vae.precision,
                use_critic, float(critic_noise_scale), bool(can_remask_prev_masked), None if aten is None else aten["key"], bool(self.use_native_step),
                id(self.noise_schedule), bool(self.use_fused_tail))
-        if inpaint is not None:
+        if inpaint is not None and "iterations" in inpaint:
+            key += (("edit", inpaint["iterations"], inpaint["n_max"]),)
+        elif inpaint is not None:
             key += (("inpaint", inpaint["n_max"]),)
         pack_ids = lambda: (id(tr._pack), id(self.vae._pack), id(self.cond_vae._pack), id(critic_net._pack) if critic_net is not None else 0,
                             id(self.token_critic._head_cache) if isinstance(self.token_critic, SelfCritic) else 0)
@@ -748,8 +806,8 @@ class MaskGit(nn.Module):
         return overflow != 0
 
     def _generate_unfused(self, seed, *args, **kw):
-        """Repeats a generate() / inpaint() call whose fused tail overflowed on the materialised path, with the same noise: the same libmmg
-        seed, or the ATen generator position the failed attempt started from."""
+        """Repeats a generate() / inpaint() / edit() call whose fused tail overflowed on the materialised path, with the same noise: the same
+        libmmg seed, or the ATen generator position the failed attempt started from."""
         saved = self.use_fused_tail
         self.use_fused_tail = False
         try:
@@ -850,10 +908,12 @@ class MaskGit(nn.Module):
         ops.logits_sample(lg, pos, ids, scores, rows_b, k_keep, temp, **kw)
 
     def _generate_body(self, text_embeds, cond_images, *, fmap_size, temperature, topk_filter_thres, timesteps, cond_scale, b,
-                       use_critic=False, critic_noise_scale=1., score_all=False, aten=None, inpaint=None, inpaint_rows=None):
+                       use_critic=False, critic_noise_scale=1., score_all=False, aten=None, inpaint=None, inpaint_rows=None, edit_iterations=None):
         """The device-side work of generate(): no host synchronisation, no data-dependent host control flow.
         inpaint (inpaint()): dict(images, frozen uint8 [b, n], counts int32 [timesteps, b]) device tensors; inpaint_rows = the largest
-        number of regenerated tokens of an image, whose schedule gives the rows sampled per step (pad rows fill the smaller counts)."""
+        number of regenerated tokens of an image, whose schedule gives the rows sampled per step (pad rows fill the smaller counts).
+        edit_iterations (edit()): inpaint holds dict(images, keep uint8 [b, n] (1 = not editable), num_select int32 [b], counts) instead,
+        and the token loop runs edit_iterations times, each preceded by mmg_edit_select, which writes that iteration's frozen map."""
         tr = self.transformer
         device = text_embeds.device
         n = fmap_size ** 2
@@ -863,10 +923,14 @@ class MaskGit(nn.Module):
         ctx = tr._prepare_context(text_embeds, cond_ids, [False, True][:nb])
         P = tr._packed()
         adt = P["adt"]
+        iterations = 1 if edit_iterations is None else edit_iterations
         if inpaint is None:
             ids = torch.full((b, n), self.mask_id, dtype=torch.long, device=device)
-        else:
+        elif edit_iterations is None:
             ids = self.vae.encode_ids(inpaint["images"]).reshape(b, n).masked_fill(inpaint["frozen"] == 0, self.mask_id)
+        else:
+            ids = self.vae.encode_ids(inpaint["images"]).reshape(b, n)
+            frozen = torch.empty((b, n), dtype=torch.uint8, device=device)
         scores = torch.zeros((b, n), dtype=torch.float32, device=device)
         masked_pos = torch.empty((b, n), dtype=torch.int32, device=device)
         k_keep = math.ceil((1 - topk_filter_thres) * V)                        # muse_maskgit_pytorch.py:414
@@ -893,7 +957,16 @@ class MaskGit(nn.Module):
                 assert whead is not None, "token_critic must have dim_out == 1"
             gcrit = cnet._packed()["gf"]
         nvtx = os.environ.get("MMG_NVTX", "0") == "1"            # host-side NVTX ranges per decode step / stage (visible in nsys / ncu --nvtx)
-        for step, (num_masked, steps_until_x0) in enumerate(zip(sched, reversed(range(timesteps)))):
+        # edit(): `iterations` rounds of the token loop, step = the global step index (iteration * timesteps + s); one round otherwise
+        for step, (num_masked, steps_until_x0) in enumerate(zip(sched * iterations, list(reversed(range(timesteps))) * iterations)):
+            s = step % timesteps
+            if edit_iterations is not None and s == 0:
+                it = step // timesteps
+                ukey = None
+                if self.sampler_noise_fn is not None:
+                    ukey = self.sampler_noise_fn(step, (b, n)).to(device=device, dtype=torch.float32).contiguous()
+                ops.edit_select(ids, scores, frozen, inpaint["keep"], inpaint["num_select"], self.mask_id, it, u=ukey,
+                                seed_dev=self._seed_dev, row_offset=self.row_offset * n)
             if nvtx:
                 if step:
                     torch.cuda.nvtx.range_pop()
@@ -912,8 +985,9 @@ class MaskGit(nn.Module):
             if inpaint is None:
                 ops.remask(ids, scores, masked_pos, num_masked, self.mask_id)
             else:      # each image re-masks among its own regenerated tokens; num_masked rows per image, the surplus padded
-                ops.remask_frozen(ids, scores, masked_pos, inpaint["frozen"], inpaint["counts"][step], num_masked, self.mask_id)
-            x = tr._run_blocks(ids, ctx, nb, sc_embed if (self.self_cond and step > 0) else None)
+                ops.remask_frozen(ids, scores, masked_pos, inpaint["frozen"] if edit_iterations is None else frozen, inpaint["counts"][s],
+                                  num_masked, self.mask_id)
+            x = tr._run_blocks(ids, ctx, nb, sc_embed if (self.self_cond and s > 0) else None)
             if self.self_cond:                                                 # embed of the conditional forward, fed back next step (:574)
                 ops.layernorm(x[:bn], P["gf"], sc_embed)
             # rows that are sampled: the masked ones; every position when already-decoded tokens may be re-masked by confidence

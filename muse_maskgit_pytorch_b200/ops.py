@@ -275,6 +275,24 @@ def remask_frozen(ids, scores, masked_pos, frozen, num_masked, rows, mask_id):
     L.call("mmg_remask_frozen", a)
 
 
+def edit_select(ids, scores, frozen_out, keep, num_select, mask_id, iteration, u=None, seed=0, seed_dev=None, row_offset=0):
+    """One mask-free editing selection: each sequence selects its num_select (int32 [B]) largest keys among the positions with keep == 0
+    (uint8 [B, n]); keys are u (fp32 [B, n]) or libmmg's Philox stream for `iteration`.  Writes frozen_out (uint8 [B, n], 1 = not
+    selected), mask_id at the selected ids and 0 into every score."""
+    for t, name in ((ids, "ids"), (scores, "scores"), (frozen_out, "frozen_out"), (keep, "keep"), (num_select, "num_select")):
+        _chk(t, name)
+    assert frozen_out.dtype == keep.dtype == torch.uint8 and frozen_out.shape == keep.shape == ids.shape == scores.shape
+    assert num_select.dtype == torch.int32 and num_select.numel() == ids.shape[0]
+    if u is not None:
+        _chk(u, "u")
+        assert u.dtype == torch.float32 and u.shape == ids.shape
+    a = L.EditSelectArgs()
+    a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.frozen_out = frozen_out.data_ptr(); a.keep = keep.data_ptr()
+    a.num_select = num_select.data_ptr(); a.u = L.ptr(u); a.seed = seed; a.seed_dev = L.ptr(seed_dev); a.row_offset = row_offset
+    a.B, a.n = ids.shape; a.iteration = iteration; a.mask_id = mask_id
+    L.call("mmg_edit_select", a)
+
+
 def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_scale):
     a = L.FinalEmbedArgs()
     a.x_cond = x_cond.data_ptr(); a.x_null = L.ptr(x_null); a.gamma = gamma.data_ptr(); a.masked_pos = masked_pos.data_ptr()

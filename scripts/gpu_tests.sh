@@ -25,6 +25,7 @@ runall full_config 900 tests/test_gpu_full_config.py
 runall fused_tail 600 tests/test_gpu_fused_tail.py
 runall t5 900 tests/test_gpu_t5.py
 runall inpaint 900 tests/test_gpu_inpaint.py
+runall edit 900 tests/test_gpu_edit.py
 runall maskgit_loss 900 tests/test_gpu_maskgit_loss.py
 runall fp8 1200 tests/test_gpu_fp8.py
 cat $OUT/summary.txt
