@@ -177,6 +177,9 @@ int mmg_groupnorm(const mmg_groupnorm_args* a, void* stream);
  * LayerNorm (eps 1e-5, gamma only — beta is a zero buffer): muse_maskgit_pytorch.py:63-70.
  *   y[r, :] = LN(x[r, :width] (+ add[:]) ) * gamma, columns >= width are written as 0 up to ldy.
  *   If x_out != NULL the (x + add) sum is also written back (fp32) — used for the constant null-CFG cross-attn term.
+ *   Mean, then the centred variance, in fp32 (two passes over the row, as F.layer_norm).  width <= 4096 when x and y are 16-byte aligned,
+ *   ldx and ldy are multiples of 4 (fp32 x) / 8 (bf16 x), ldy <= 4096 and, with add or x_out, width is such a multiple too; otherwise
+ *   width <= 2048 (any ldy).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
   const void*  x;  int32_t x_dtype;  int32_t y_dtype;

@@ -4,10 +4,12 @@
 namespace mmg {
 
 // ---------------------------------------------------------------------------------------------------------------
-// LayerNorm: one warp per row, the row is held in registers (width <= 32*4*MAXV), two-pass mean/variance in fp32
-// exactly as F.layer_norm (biased variance, eps 1e-5).  ref: muse_maskgit_pytorch.py:63-70
+// LayerNorm: one warp per row, the row is held in registers, two-pass mean/variance in fp32 exactly as F.layer_norm
+// (biased variance, eps 1e-5).  Widths up to LN_MAXV * 128 on the scalar kernel, up to LN_VEC_MAXW on the vectorised ones.
+// ref: muse_maskgit_pytorch.py:63-70
 // ---------------------------------------------------------------------------------------------------------------
-constexpr int LN_MAXV = 16;   // float4 chunks per lane -> width <= 2048
+constexpr int LN_MAXV = 16;        // float4 chunks per lane -> width <= 2048 (scalar LayerNorm, final_embed, fp8 LayerNorm)
+constexpr int LN_VEC_MAXW = 4096;  // vectorised LayerNorm: 32 chunks of 4 fp32 or 16 chunks of 8 bf16 columns per lane
 
 template <typename TX, typename TY>
 __global__ void __launch_bounds__(256)
@@ -56,6 +58,7 @@ layernorm_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* __re
       }
     }
   }
+  for (int64_t c = LN_MAXV * 128 + lane; c < ldy; c += 32) yr[c] = from_f<TY>(0.f);     // padding past the register-held columns
 }
 
 // Vectorised LayerNorm: every lane moves 16 bytes per access (4 fp32 or 8 bf16 columns), CH chunks per lane cover the row,
@@ -122,29 +125,16 @@ layernorm_vec_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* 
       for (int j = 0; j < VN; ++j) v[i][j] = 0.f;
     }
   }
-  float mean, rstd;
-  if (sizeof(TY) == 2) {
-    // bf16 output: one fused reduction of (sum, sum of squares) — the E[x^2] - mean^2 form is far inside bf16 output precision
-    float sq = 0.f;
+  // centred second pass for every output type: E[x^2] - mean^2 in fp32 loses the variance once |mean| / std reaches a few hundred
+  const float mean = warp_sum(sum) / (float)width;
+  float sq = 0.f;
 #pragma unroll
-    for (int i = 0; i < CH; ++i)
+  for (int i = 0; i < CH; ++i) {
+    const int c = (i * 32 + lane) * VN;
 #pragma unroll
-      for (int j = 0; j < VN; ++j) sq = fmaf(v[i][j], v[i][j], sq);       // padded / out-of-width entries are 0
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { sum += __shfl_xor_sync(0xffffffffu, sum, o); sq += __shfl_xor_sync(0xffffffffu, sq, o); }
-    mean = sum / (float)width;
-    rstd = rsqrtf(fmaxf(sq / (float)width - mean * mean, 0.f) + 1e-5f);
-  } else {
-    mean = warp_sum(sum) / (float)width;
-    float sq = 0.f;
-#pragma unroll
-    for (int i = 0; i < CH; ++i) {
-      const int c = (i * 32 + lane) * VN;
-#pragma unroll
-      for (int j = 0; j < VN; ++j) if (c + j < width) { const float d = v[i][j] - mean; sq += d * d; }
-    }
-    rstd = rsqrtf(warp_sum(sq) / (float)width + 1e-5f);
+    for (int j = 0; j < VN; ++j) if (c + j < width) { const float d = v[i][j] - mean; sq += d * d; }
   }
+  const float rstd = rsqrtf(warp_sum(sq) / (float)width + 1e-5f);
   TY* yr = y + row * ldy;
 #pragma unroll
   for (int i = 0; i < CH; ++i) {
@@ -198,16 +188,19 @@ layernorm_rows2_kernel(const float* __restrict__ x, bf16* __restrict__ y, const 
         if (x_out) reinterpret_cast<float4*>(x_out + row * W)[i * 32 + lane] = v[q][i];
       }
     }
-    float sum = 0.f, sq = 0.f;
+    // two passes over the registers (mean, then the centred sum of squares), as F.layer_norm: the one-pass E[x^2] - mean^2 form
+    // cancels catastrophically on rows whose |mean| / std is in the hundreds
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < CH; ++i) sum += (v[q][i].x + v[q][i].y) + (v[q][i].z + v[q][i].w);
+    const float mean = warp_sum(sum) * (1.0f / W);
+    float sq = 0.f;
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
-      sum += (v[q][i].x + v[q][i].y) + (v[q][i].z + v[q][i].w);
-      sq = fmaf(v[q][i].x, v[q][i].x, fmaf(v[q][i].y, v[q][i].y, fmaf(v[q][i].z, v[q][i].z, fmaf(v[q][i].w, v[q][i].w, sq))));
+      const float dx = v[q][i].x - mean, dy = v[q][i].y - mean, dz = v[q][i].z - mean, dw = v[q][i].w - mean;
+      sq = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, sq))));
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { sum += __shfl_xor_sync(0xffffffffu, sum, o); sq += __shfl_xor_sync(0xffffffffu, sq, o); }
-    const float mean = sum * (1.0f / W);
-    const float rstd = rsqrtf(fmaxf(sq * (1.0f / W) - mean * mean, 0.f) + 1e-5f);
+    const float rstd = rsqrtf(warp_sum(sq) * (1.0f / W) + 1e-5f);
 #pragma unroll
     for (int i = 0; i < CH; ++i) {
       const float o0 = (v[q][i].x - mean) * rstd * g[i].x, o1 = (v[q][i].y - mean) * rstd * g[i].y;
@@ -491,23 +484,41 @@ __global__ void split3_kernel(const float* __restrict__ src, bf16* __restrict__ 
 
 using namespace mmg;
 
+// the vectorised LayerNorm with the fewest 16-byte chunks per lane that cover `span` columns (CH = 32 exists for fp32 input only: bf16
+// input reaches LN_VEC_MAXW at CH = 16)
+template <typename TX, typename TY>
+static cudaError_t launch_layernorm_vec(const mmg_layernorm_args* a, int64_t span, unsigned grid, cudaStream_t st) {
+  constexpr int VN = VecIO<TX>::N;
+  const int ch = (int)((span + 32 * VN - 1) / (32 * VN));
+  auto go = [&](auto kern) {
+    return launch_pdl(kern, dim3(grid), dim3(256), 0, st, (const TX*)a->x, (TY*)a->y, a->gamma, a->add, a->x_out, a->zero_stats, a->add_from,
+                      a->rows, (int)a->width, a->ldx, a->ldy);
+  };
+  if (ch <= 4) return go(layernorm_vec_kernel<TX, TY, 4>);
+  if (ch <= 6) return go(layernorm_vec_kernel<TX, TY, 6>);
+  if (ch <= 8) return go(layernorm_vec_kernel<TX, TY, 8>);
+  if constexpr (VN == 4) { if (ch > 16) return go(layernorm_vec_kernel<TX, TY, 32>); }
+  return go(layernorm_vec_kernel<TX, TY, 16>);
+}
+
 extern "C" int mmg_layernorm(const mmg_layernorm_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->x && a->y && a->gamma, "mmg_layernorm: NULL pointer");
-  MMG_CHECK_ARG(a->width > 0 && a->width <= LN_MAXV * 128, "mmg_layernorm: width %lld not in (0, %d]", (long long)a->width, LN_MAXV * 128);
+  MMG_CHECK_ARG(a->width > 0 && a->width <= LN_VEC_MAXW, "mmg_layernorm: width %lld not in (0, %d]", (long long)a->width, LN_VEC_MAXW);
   MMG_CHECK_ARG(a->ldy >= a->width && a->ldx >= a->width, "mmg_layernorm: leading dims");
   MMG_CHECK_ARG(!a->x_out || a->x_dtype == MMG_F32, "mmg_layernorm: x_out requires fp32 x");
-  if (a->rows == 0) return MMG_OK;
   const unsigned grid = (unsigned)((a->rows + 7) / 8);
   const int w = (int)a->width;
   const int vn = a->x_dtype == MMG_BF16 ? 8 : 4;                      // columns per 16-byte access of the input
   const int64_t span = a->ldy > w ? a->ldy : w;
   const bool vec = (a->ldx % vn == 0) && (a->ldy % vn == 0) && ((reinterpret_cast<uintptr_t>(a->x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(a->y) & 15) == 0) &&
                    (!a->add || (w % vn == 0 && (reinterpret_cast<uintptr_t>(a->add) & 15) == 0)) && (!a->x_out || w % vn == 0) &&
-                   ((w + vn - 1) / vn * vn <= a->ldx) && span <= 16 * 32 * vn;
-#define LNV(TX, TY, CH) launch_pdl(layernorm_vec_kernel<TX, TY, CH>, dim3(grid), dim3(256), 0, st, (const TX*)a->x, (TY*)a->y, a->gamma, a->add, a->x_out, a->zero_stats, a->add_from, a->rows, w, a->ldx, a->ldy)
-#define LNV_DISPATCH(TX, TY) do { const int64_t per = 32 * vn; const int ch = (int)((span + per - 1) / per); \
-    if (ch <= 4) LNV(TX, TY, 4); else if (ch <= 6) LNV(TX, TY, 6); else if (ch <= 8) LNV(TX, TY, 8); else LNV(TX, TY, 16); } while (0)
+                   ((w + vn - 1) / vn * vn <= a->ldx) && span <= LN_VEC_MAXW;
+  // the scalar kernel holds LN_MAXV * 128 columns in registers (any ldy: it zeroes the padding past them in a loop)
+  MMG_CHECK_ARG(vec || w <= LN_MAXV * 128, "mmg_layernorm: width %d > %d needs the vectorised kernel (16-byte aligned x / y / add, ldx and ldy "
+                "multiples of %d, width %% %d == 0 with add / x_out, ldy <= %d)", w, LN_MAXV * 128, vn, vn, LN_VEC_MAXW);
+  if (a->rows == 0) return MMG_OK;
+#define LNV_DISPATCH(TX, TY) MMG_CUDA((launch_layernorm_vec<TX, TY>(a, span, grid, st)))
 #define LN_LAUNCH(TX, TY) layernorm_kernel<TX, TY><<<grid, 256, 0, st>>>((const TX*)a->x, (TY*)a->y, a->gamma, a->add, a->x_out, a->zero_stats, a->add_from, a->rows, w, a->ldx, a->ldy)
   // dense fp32 -> bf16 rows of exactly CH * 128 columns: two rows per warp
   const bool rows2 = a->x_dtype == MMG_F32 && a->y_dtype == MMG_BF16 && vec && a->ldx == w && a->ldy == w && (w == 512 || w == 256 || w == 128) &&
@@ -524,7 +535,6 @@ extern "C" int mmg_layernorm(const mmg_layernorm_args* a, void* stream) {
   else if (a->x_dtype == MMG_F32 && a->y_dtype == MMG_BF16) { if (vec) LNV_DISPATCH(float, bf16); else LN_LAUNCH(float, bf16); }
   else if (a->x_dtype == MMG_BF16 && a->y_dtype == MMG_BF16) { if (vec) LNV_DISPATCH(bf16, bf16); else LN_LAUNCH(bf16, bf16); }
   else return fail(MMG_EINVAL, "mmg_layernorm: unsupported dtype pair %d -> %d", a->x_dtype, a->y_dtype);
-#undef LNV
 #undef LNV_DISPATCH
 #undef LN_LAUNCH
   MMG_LAUNCHED();
