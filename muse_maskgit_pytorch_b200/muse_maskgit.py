@@ -9,12 +9,13 @@ Both CFG branches of a decode step run as one batch of 2B sequences; the null br
 constant to_out(null_v) (every text key masked -> softmax puts weight exactly 1 on the null key, SURVEY.md 8a T3).
 """
 import ctypes
+import dataclasses
 import math
 import os
 import random
 from functools import partial
 from pathlib import Path
-from typing import Callable, List, Optional
+from typing import Callable, List, NamedTuple, Optional
 
 import torch
 from torch import nn
@@ -237,6 +238,10 @@ class Transformer(nn.Module):
                 tm = torch.cat((tm, torch.ones((b, m - m_text), dtype=torch.bool, device=dev)), dim=1)
             masks.append(tm)
         key_mask = torch.cat(masks, 0).to(torch.uint8).contiguous()                # [len(branches)*b, m]
+        # a branch whose keys are all masked has the constant cross-attention output to_out(null_v): _run_blocks attends over the others
+        all_masked = [bool(d) and cond_ids is None for d in branches]
+        live = all_masked.count(False)
+        assert all_masked == [False] * live + [True] * (len(branches) - live), "live CFG branches must come first"
         heads = tb.heads
         tk_alloc = _round_up(m + 1, 8)
         kvs = []
@@ -249,7 +254,7 @@ class Transformer(nn.Module):
             if len(branches) > 1:
                 k, v = k.repeat(len(branches), 1, 1), v.repeat(len(branches), 1, 1)
             kvs.append((k, v))
-        return dict(kv=kvs, key_mask=key_mask, m=m, all_masked=[bool(d) and cond_ids is None for d in branches])
+        return dict(kv=kvs, key_mask=key_mask, m=m, live=live)
 
     # ----- the block stack over R = nb*b*n rows -------------------------------------------------------------------------
     def _workspace(self, nb, b, n, dev):
@@ -302,7 +307,8 @@ class Transformer(nn.Module):
                 x[j * bn:(j + 1) * bn].copy_(x[:bn])
         else:
             ops.embed(ids.contiguous(), P["tok"], P["pos"], x, n=n, copies=nb)
-        live = [j for j in range(nb) if not ctx["all_masked"][j]]
+        live = min(ctx["live"], nb)
+        Rl, ql = live * bn, live * b * heads          # rows and attention batches of the live branches
 
         def norm(rows, g, fp8, **kw):
             """LayerNorm of x[rows] into the A operand of the next product (xn; fp8: e4m3 rows + row scales)"""
@@ -325,33 +331,19 @@ class Transformer(nn.Module):
             ops.linear(ao, sa["wo"], x, epilogue=ops.EPI_RESIDUAL, resid=x)
             # --- cross attention ---
             kc, vc = ctx["kv"][li]
-            pending_add = {j: ca["null_out"] for j in range(nb) if ctx["all_masked"][j]}
             if live:
-                assert live == list(range(len(live))), "live branches must come first"
-                Rl = len(live) * bn
                 norm(slice(0, Rl), ca["g"], "wq_8" in ca)
-                epi = ops.qkv_epilogue(adt, heads, n, q=q[:len(live) * b * heads], q_scale=ca["qs"])
+                epi = ops.qkv_epilogue(adt, heads, n, q=q[:ql], q_scale=ca["qs"])
                 if "wq_8" in ca:
                     ops.linear_fp8(ws["xq"][:Rl], ws["xs"][:Rl], ca["wq_8"], ca["s_q"], None, epilogue=ops.EPI_QKV, epi=epi)
                 else:
                     ops.linear(xn[:Rl], ca["wq"], None, epilogue=ops.EPI_QKV, epi=epi)
-                ops.attention(q[:len(live) * b * heads], kc[:len(live) * b * heads], vc[:len(live) * b * heads], ao[:Rl], len(live) * b, heads,
-                              ctx["m"] + 1, key_mask=ctx["key_mask"][:len(live) * b], logit_bound=ca["bound"])
+                ops.attention(q[:ql], kc[:ql], vc[:ql], ao[:Rl], live * b, heads, ctx["m"] + 1, key_mask=ctx["key_mask"][:live * b],
+                              logit_bound=ca["bound"])
                 ops.linear(ao[:Rl], ca["wo"], x[:Rl], epilogue=ops.EPI_RESIDUAL, resid=x[:Rl])
-            # --- feed forward (the constant null-branch cross-attention term is folded into this LayerNorm) ---
-            ff8 = "w1_8" in ff
-            if pending_add and sorted(pending_add) == list(range(min(pending_add), nb)):
-                # one launch for all branches: rows of the all-masked (null) branches get += to_out(null_v) before the norm
-                norm(slice(None), ff["g0"], ff8, add=ca["null_out"], x_out=x, add_from=min(pending_add) * bn)
-            elif not pending_add:
-                norm(slice(None), ff["g0"], ff8)
-            else:
-                for j in range(nb):
-                    rows = slice(j * bn, (j + 1) * bn)
-                    if j in pending_add:
-                        norm(rows, ff["g0"], ff8, add=pending_add[j], x_out=x[rows])
-                    else:
-                        norm(rows, ff["g0"], ff8)
+            # --- feed forward: one LayerNorm over every branch, which first adds to_out(null_v) to the rows of the masked branches ---
+            null_add = dict(add=ca["null_out"], x_out=x, add_from=Rl) if live < nb else {}
+            norm(slice(None), ff["g0"], "w1_8" in ff, **null_add)
             self._ff_tail(xn, ff, x, ws, R)
         return x
 
@@ -493,6 +485,19 @@ def _aten_uniform_geometry(device, numel):
     return stride, ((numel - 1) // (stride * 4) + 1) * 4
 
 
+def _cuda_generator(device):
+    return torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
+
+
+def _reserve_aten_offsets(device, increment):
+    """Takes `increment` Philox offsets of torch's CUDA generator on `device` for uniforms our kernels draw in place of ATen uniform_
+    calls: returns (seed, first offset) and advances the generator past them, as those calls would have."""
+    gen = _cuda_generator(device)
+    seed, off = gen.initial_seed(), gen.get_offset()
+    gen.set_offset(off + increment)
+    return seed, off
+
+
 def _mask_subset_prob(mask, prob, draw, min_mask=0):
     """ref: muse_maskgit_pytorch.py:46-60 (get_mask_subset_prob) with its torch.rand drawn through `draw`."""
     num_to_mask = (mask.sum(dim=-1, keepdim=True) * prob).clamp(min=min_mask)
@@ -526,6 +531,43 @@ def regen_tokens(mask, b, image_size, fmap_size):
     if p * f != image_size:
         raise ValueError(f"image_size {image_size} is not a multiple of fmap_size {f}: pass the mask at token resolution")
     return mask.reshape(b, f, p, f, p).any(dim=4).any(dim=2)
+
+
+@dataclasses.dataclass(frozen=True)
+class _Region:
+    """The tokens inpaint() regenerates or edit() resamples.  n_max: the most an image regenerates per round (its schedule gives the rows
+    sampled per step); iterations: None for inpaint(), else edit()'s rounds, each opened by an mmg_edit_select that writes its frozen map;
+    tensors: images, counts int32 [timesteps, b], and frozen uint8 [b, n] or keep uint8 [b, n] (1 = not editable) + num_select int32 [b]."""
+    n_max: int
+    iterations: Optional[int]
+    tensors: dict
+
+
+@dataclasses.dataclass(frozen=True)
+class _DecodeRequest:
+    """One validated generate() / inpaint() / edit() call.  seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs)."""
+    texts: List[str]
+    cond_images: Optional[torch.Tensor]
+    fmap_size: int
+    temperature: float
+    topk_filter_thres: float
+    timesteps: int
+    cond_scale: float
+    critic_noise_scale: float
+    can_remask_prev_masked: bool
+    use_critic: bool
+    return_ids: bool
+    region: Optional[_Region] = None
+    seed: Optional[int] = None
+
+
+class _CapturedCall(NamedTuple):
+    """A whole-call CUDA graph of MaskGit._generate_body and the static tensors it reads and writes."""
+    graph: "torch.cuda.CUDAGraph"
+    inputs: tuple               # (text_embeds, cond_images or None, region tensors or None), copied in before each replay
+    outputs: tuple              # (images, ids, fused-tail status or None)
+    pack_ids: tuple             # identities of the packed weights at capture: a re-pack re-captures
+    keep_alive: tuple           # packed weights and workspaces the captured kernels point at
 
 
 # ------------------------------------------------------------------------------------------------ MaskGit
@@ -599,13 +641,11 @@ class MaskGit(nn.Module):
         if self.use_native_step and self.transformer.precision == "fp8":
             raise ValueError('use_native_step=True runs mmg_decode_step, whose weights carry no fp8 scales: it cannot run precision="fp8"; '
                              "set use_native_step = False")
-        was_training = self.training
-        self.eval()
-        try:
-            return self._generate(texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres,
-                                  can_remask_prev_masked, force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids)
-        finally:
-            self.train(was_training)
+        if negative_texts is not None:
+            raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
+        return self._decode(self._request(texts, cond_images=cond_images, fmap_size=fmap_size, temperature=temperature, timesteps=timesteps,
+                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
 
     @torch.no_grad()
     def inpaint(self, texts: List[str], images: torch.Tensor, mask: torch.Tensor, cond_images: Optional[torch.Tensor] = None, temperature=1.,
@@ -624,24 +664,14 @@ class MaskGit(nn.Module):
         caller's job.  With every token masked the result equals generate() under the same seed or injected noise.
         Returns what generate() returns.  `use_native_step` does not apply here (mmg_decode_step has no frozen positions)."""
         b = len(texts)
-        device = next(self.parameters()).device
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
         self._check_images(images, b)
         regen = regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1)
         counts = [int(c) for c in regen.sum(dim=1).tolist()]                      # N_b: the call's one device-to-host read for a GPU mask
-        n_max = max(counts, default=0)
-        table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in counts]
-        inp = dict(n_max=n_max,
-                   dev=dict(images=images.to(device, torch.float32).contiguous(),
-                            frozen=(~regen).to(device=device, dtype=torch.uint8).contiguous(),
-                            counts=torch.tensor(table, dtype=torch.int32).t().contiguous().to(device)))       # [timesteps, b]
-        was_training = self.training
-        self.eval()
-        try:
-            return self._generate(texts, None, cond_images, None, temperature, topk_filter_thres, can_remask_prev_masked,
-                                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, inpaint=inp)
-        finally:
-            self.train(was_training)
+        region = self._region(images, counts, timesteps, frozen=(~regen).to(torch.uint8))
+        return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=timesteps, region=region,
+                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
 
     @torch.no_grad()
     def edit(self, texts: List[str], images: torch.Tensor, mask: Optional[torch.Tensor] = None, iterations=8, fraction=0.1, timesteps=4,
@@ -675,127 +705,148 @@ class MaskGit(nn.Module):
         if self.sampler_rng == "aten":
             raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
         b = len(texts)
-        device = next(self.parameters()).device
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
         self._check_images(images, b)
         editable = (torch.ones((b, fmap_size ** 2), dtype=torch.bool) if mask is None
                     else regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1))
         counts = [int(c) for c in editable.sum(dim=1).tolist()]                   # N_b
         select = [max(int(fraction * c), 1) if c else 0 for c in counts]          # r_b
-        table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in select]
-        inp = dict(n_max=max(select, default=0), iterations=iterations,
-                   dev=dict(images=images.to(device, torch.float32).contiguous(),
-                            keep=(~editable).to(device=device, dtype=torch.uint8).contiguous(),
-                            num_select=torch.tensor(select, dtype=torch.int32).to(device),
-                            counts=torch.tensor(table, dtype=torch.int32).t().contiguous().to(device)))       # [timesteps, b]
-        was_training = self.training
-        self.eval()
-        try:
-            return self._generate(texts, None, cond_images, None, temperature, topk_filter_thres, can_remask_prev_masked,
-                                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, inpaint=inp)
-        finally:
-            self.train(was_training)
+        region = self._region(images, select, timesteps, iterations, keep=(~editable).to(torch.uint8), num_select=torch.tensor(select, dtype=torch.int32))
+        return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=timesteps, region=region,
+                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
 
     def _check_images(self, images, b):
         if not isinstance(images, torch.Tensor) or tuple(images.shape) != (b, self.vae.channels, self.image_size, self.image_size):
             raise ValueError(f"images must be a (b, {self.vae.channels}, {self.image_size}, {self.image_size}) tensor for b = {b} texts, got "
                              f"{tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__}")
 
-    def _generate(self, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres, can_remask_prev_masked,
-                  force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale, return_ids, seed=None, inpaint=None):
-        tr = self.transformer
-        if negative_texts is not None:
-            raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
+    def _region(self, images, counts, timesteps, iterations=None, **tensors):
+        """The _Region of a call whose image b regenerates counts[b] tokens per round, on the schedule of that count (none: 0 throughout)."""
+        table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in counts]
+        tensors.update(images=images.to(torch.float32), counts=torch.tensor(table, dtype=torch.int32).t())        # counts: [timesteps, b]
+        device = next(self.parameters()).device
+        return _Region(max(counts, default=0), iterations, {k: v.to(device).contiguous() for k, v in tensors.items()})
+
+    def _request(self, texts, *, force_not_use_token_critic, fmap_size=None, **settings):
         use_critic = self.token_critic is not None and not force_not_use_token_critic
-        if can_remask_prev_masked and not use_critic:      # the reference only reaches this assert in the no-critic branch (:611-612)
+        if settings["can_remask_prev_masked"] and not use_critic:      # the reference only reaches this assert in the no-critic branch (:611-612)
             assert self.no_mask_token_prob > 0., "without training with some of the non-masked tokens forced to predict, not sure if the logits will be meaningful for these token"
         fmap_size = fmap_size if fmap_size is not None else self.vae.get_encoded_fmap_size(self.image_size)
-        device = next(self.parameters()).device
-        b = len(texts)
-        for net in (tr, self.vae, self.cond_vae, self.token_critic if isinstance(self.token_critic, Transformer) else None):
+        return _DecodeRequest(texts=texts, fmap_size=fmap_size, use_critic=use_critic, **settings)
+
+    def _check_weights(self):          # in-place parameter edits since the last call drop the packed copies (and the captured graphs)
+        for net in (self.transformer, self.vae, self.cond_vae, self.token_critic if isinstance(self.token_critic, Transformer) else None):
             if net is not None:
-                net._check_weights()          # in-place parameter edits since the last call drop the packed copies (and the graphs below)
-        text_embeds = tr.encode_text(texts).to(device, non_blocking=True)
+                net._check_weights()
+
+    def _injected_noise(self, step, shape, device):
+        """sampler_noise_fn's U[0, 1) tensor for (step, shape) as contiguous fp32 on `device`; None when no noise is injected."""
+        if self.sampler_noise_fn is None:
+            return None
+        return self.sampler_noise_fn(step, shape).to(device=device, dtype=torch.float32).contiguous()
+
+    def _resolve_critic(self, text_embeds, cond_ids, branches, ctx=None):
+        """(net, CFG branches, context, head weight, head bias, final LayerNorm gamma) of the token critic.  A SelfCritic is the generator's
+        conditional branch (muse_maskgit_pytorch.py:352-361), over `ctx` when given; a TokenCritic runs `branches` over its own context."""
+        if isinstance(self.token_critic, SelfCritic):
+            net, nb = self.transformer, 1
+            whead, bhead = self.token_critic._head()
+            whead = whead.to(text_embeds.device)
+            ctx = ctx if ctx is not None else net._prepare_context(text_embeds, cond_ids, branches)
+        else:
+            net, nb = self.token_critic, len(branches)
+            ctx = net._prepare_context(text_embeds, cond_ids, branches)
+            whead, bhead = net._packed()["whead"], 0.
+            assert whead is not None, "token_critic must have dim_out == 1"
+        return net, nb, ctx, whead, bhead, net._packed()["gf"]
+
+    def _decode(self, req):
+        """Runs a generate() / inpaint() / edit() request in eval mode.  A call whose fused tail overflowed is repeated on the materialised
+        path with the same noise: the same libmmg seed, or the ATen generator position the failed attempt started from."""
+        was_training, saved = self.training, self.use_fused_tail
+        self.eval()
+        try:
+            images, ids, status, seed = self._decode_once(req)
+            if not self._fused_tail_overflowed(status):
+                return (images, ids) if req.return_ids else images
+            self.use_fused_tail = False
+            if self.sampler_rng == "aten" and self.sampler_noise_fn is None:       # re-read the generator position the failed attempt consumed
+                _cuda_generator(next(self.parameters()).device).set_offset(self._aten_start_offset)
+            return self._decode(dataclasses.replace(req, seed=seed))
+        finally:
+            self.train(was_training)
+            self.use_fused_tail = saved
+
+    def _decode_once(self, req):
+        """One attempt at a request: (images, ids, the fused tail's status word or None, the libmmg seed it sampled with)."""
+        tr = self.transformer
+        device = next(self.parameters()).device
+        b = len(req.texts)
+        self._check_weights()
+        text_embeds = tr.encode_text(req.texts).to(device, non_blocking=True)
         if self.use_cuda_graph and text_embeds.shape[1] % 32:
             # T5 pads to the longest prompt of the batch: bucket the length (multiples of 32) so that prompt lengths share captured
             # graphs; all-zero rows are padding to the reference too (masked keys, muse_maskgit_pytorch.py:304)
             text_embeds = torch.nn.functional.pad(text_embeds, (0, 0, 0, 32 - text_embeds.shape[1] % 32))
         if self.resize_image_for_cond_image:
-            assert cond_images is not None, "conditioning image must be passed in to generate for super res maskgit"
-            cond_images = cond_images.to(device, torch.float32)
+            assert req.cond_images is not None, "conditioning image must be passed in to generate for super res maskgit"
+            cond_images = req.cond_images.to(device, torch.float32)
         else:
             cond_images = None
         # per-call seed: explicit sampler_seed, else one draw from torch's global generator (reproducible under manual_seed)
         assert self.sampler_rng in ("mmg", "aten"), self.sampler_rng
         if getattr(self, "_seed_dev", None) is None or self._seed_dev.device != device:
             self._seed_dev = torch.zeros((1,), dtype=torch.int64, device=device)
-        aten = None
+        aten, seed = None, req.seed
         if self.sampler_rng == "aten" and self.sampler_noise_fn is None:
-            aten = self._aten_plan(device, b, fmap_size ** 2, tr.num_tokens, timesteps, use_critic)
+            aten = self._aten_plan(device, b, req.fmap_size ** 2, tr.num_tokens, req.timesteps, req.use_critic)
         elif self.sampler_noise_fn is None:      # (injected noise: the host generator is the caller's stream — nothing is drawn from it here)
             if seed is None:                     # (a rerun on the materialised path keeps the seed of the attempt it repeats)
                 seed = self.sampler_seed if self.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
             self._seed_dev.fill_(seed)
-        body = partial(self._generate_body, fmap_size=fmap_size, temperature=temperature, topk_filter_thres=topk_filter_thres,
-                       timesteps=timesteps, cond_scale=cond_scale, b=b, use_critic=use_critic, critic_noise_scale=critic_noise_scale,
-                       score_all=bool(can_remask_prev_masked) and not use_critic, aten=aten)
-        if inpaint is not None:
-            body = partial(body, inpaint_rows=inpaint["n_max"], edit_iterations=inpaint.get("iterations"))
-        inp_dev = None if inpaint is None else inpaint["dev"]
-        inp_kw = lambda d: {} if inpaint is None else dict(inpaint=d)
-        rerun = lambda: self._generate_unfused(seed, texts, negative_texts, cond_images, fmap_size, temperature, topk_filter_thres,
-                                               can_remask_prev_masked, force_not_use_token_critic, timesteps, cond_scale, critic_noise_scale,
-                                               return_ids, **inp_kw(inpaint))
-        critic_net = self.token_critic if isinstance(self.token_critic, Transformer) and use_critic else None
+        region = None if req.region is None else req.region.tensors
         if not self.use_cuda_graph or self.sampler_noise_fn is not None:
-            images, ids, status = body(text_embeds, cond_images, **inp_kw(inp_dev))
-            if self._fused_tail_overflowed(status):
-                return rerun()
-            return (images, ids) if return_ids else images
+            return self._generate_body(req, text_embeds, cond_images, region, aten) + (seed,)
         # ---- whole-call CUDA graph: 18 decode steps + VAE decode replayed as one launch (no per-kernel host work) ----
-        key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), fmap_size,
-               float(temperature), float(topk_filter_thres), int(timesteps), float(cond_scale), int(self.row_offset), tr.precision, self.vae.precision,
-               use_critic, float(critic_noise_scale), bool(can_remask_prev_masked), None if aten is None else aten["key"], bool(self.use_native_step),
-               id(self.noise_schedule), bool(self.use_fused_tail))
-        if inpaint is not None and "iterations" in inpaint:
-            key += (("edit", inpaint["iterations"], inpaint["n_max"]),)
-        elif inpaint is not None:
-            key += (("inpaint", inpaint["n_max"]),)
+        key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), req.fmap_size,
+               float(req.temperature), float(req.topk_filter_thres), int(req.timesteps), float(req.cond_scale), int(self.row_offset),
+               tr.precision, self.vae.precision, req.use_critic, float(req.critic_noise_scale), bool(req.can_remask_prev_masked),
+               None if aten is None else aten["key"], bool(self.use_native_step), id(self.noise_schedule), bool(self.use_fused_tail))
+        if req.region is not None:
+            key += (("inpaint", req.region.n_max) if req.region.iterations is None else ("edit", req.region.iterations, req.region.n_max),)
+        critic_net = self.token_critic if isinstance(self.token_critic, Transformer) and req.use_critic else None
         pack_ids = lambda: (id(tr._pack), id(self.vae._pack), id(self.cond_vae._pack), id(critic_net._pack) if critic_net is not None else 0,
                             id(self.token_critic._head_cache) if isinstance(self.token_critic, SelfCritic) else 0)
         entry = self._graphs.get(key)
-        if entry is not None and entry[5] != pack_ids():
+        if entry is not None and entry.pack_ids != pack_ids():
             entry = None                                       # weights were re-packed (load_state_dict / .to()): re-capture
         if entry is None:
             te_s = text_embeds.clone()
             ci_s = None if cond_images is None else cond_images.clone()
-            inp_s = None if inp_dev is None else {k: v.clone() for k, v in inp_dev.items()}     # images, frozen, count table
-            body(te_s, ci_s, **inp_kw(inp_s))                  # eager warm-up: lazy packing, workspaces, function attributes
+            region_s = None if region is None else {k: v.clone() for k, v in region.items()}
+            self._generate_body(req, te_s, ci_s, region_s, aten)        # eager warm-up: lazy packing, workspaces, function attributes
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                out_images, out_ids, out_status = body(te_s, ci_s, **inp_kw(inp_s))
-            # the entry keeps alive everything the captured kernels point at (packed weights, workspaces)
-            entry = (graph, te_s, ci_s, out_images, (out_ids, out_status), pack_ids(),
-                     (tr._pack, self.vae._pack, self.cond_vae._pack, dict(getattr(tr, "_ws", {})),
-                      None if critic_net is None else (critic_net._pack, dict(getattr(critic_net, "_ws", {}))),
-                      self.token_critic._head_cache if isinstance(self.token_critic, SelfCritic) else None), inp_s)
+                outputs = self._generate_body(req, te_s, ci_s, region_s, aten)
+            entry = _CapturedCall(graph, (te_s, ci_s, region_s), outputs, pack_ids(),
+                                  keep_alive=(tr._pack, self.vae._pack, self.cond_vae._pack, dict(getattr(tr, "_ws", {})),
+                                              None if critic_net is None else (critic_net._pack, dict(getattr(critic_net, "_ws", {}))),
+                                              self.token_critic._head_cache if isinstance(self.token_critic, SelfCritic) else None))
             if len(self._graphs) >= 4:
                 self._graphs.pop(next(iter(self._graphs)))       # least recently used (hits are moved to the end below)
         self._graphs.pop(key, None)
         self._graphs[key] = entry
-        graph, te_s, ci_s, out_images, (out_ids, out_status) = entry[:5]
+        te_s, ci_s, region_s = entry.inputs
         te_s.copy_(text_embeds, non_blocking=True)
         if ci_s is not None:
             ci_s.copy_(cond_images, non_blocking=True)
-        if inp_dev is not None:
-            for k, v in entry[7].items():
-                v.copy_(inp_dev[k], non_blocking=True)
-        graph.replay()
-        images, ids = out_images.clone(), out_ids.clone()
-        if self._fused_tail_overflowed(out_status):
-            return rerun()
-        return (images, ids) if return_ids else images
+        for k, v in (region_s or {}).items():
+            v.copy_(region[k], non_blocking=True)
+        entry.graph.replay()
+        images, ids, status = entry.outputs
+        return images.clone(), ids.clone(), status, seed
 
     def _fused_tail_overflowed(self, status):
         """status[1] != 0: some decode step had more rows whose sampled top-k threshold missed than the fused path's fallback holds (e.g. constant
@@ -805,27 +856,12 @@ class MaskGit(nn.Module):
         self.last_fused_fallback_rows, overflow = (int(v) for v in status.tolist())
         return overflow != 0
 
-    def _generate_unfused(self, seed, *args, **kw):
-        """Repeats a generate() / inpaint() / edit() call whose fused tail overflowed on the materialised path, with the same noise: the same
-        libmmg seed, or the ATen generator position the failed attempt started from."""
-        saved = self.use_fused_tail
-        self.use_fused_tail = False
-        try:
-            if self.sampler_rng == "aten" and self.sampler_noise_fn is None:       # re-read the generator position the failed attempt consumed
-                gen = torch.cuda.default_generators[next(self.parameters()).device.index or 0]
-                gen.set_offset(self._aten_start_offset)
-            return self._generate(*args, seed=seed, **kw)
-        finally:
-            self.use_fused_tail = saved
-
     def _native_step_setup(self, ctx, P, b, n, nb, max_masked, V, device):
         """Argument block of mmg_decode_step for this generate(): the packed weights and the per-call context as raw pointers, plus the
         zero-initialised workspace.  Everything referenced is kept alive by the returned dict (and by `P` / `ctx`)."""
         tr = self.transformer
         tb = tr.transformer_blocks
         depth = len(P["layers"])
-        live = sum(1 for m in ctx["all_masked"][:nb] if not m)
-        assert ctx["all_masked"][:nb] == [False] * live + [True] * (nb - live), "live CFG branches must come first"
         layers = (_lib.LayerWeights * depth)()
         for li, lay in enumerate(P["layers"]):
             sa, ca, ff, lw = lay["sa"], lay["ca"], lay["ff"], layers[li]
@@ -843,7 +879,7 @@ class MaskGit(nn.Module):
         ws = torch.zeros((nbytes,), dtype=torch.uint8, device=device)
         a = _lib.DecodeStepArgs()
         a.depth = depth; a.dim = tr.dim; a.heads = tb.heads; a.n = n; a.V = V; a.F = ff0["F"]; a.Fp = ff0["Fp"]; a.b = b
-        a.branches = nb; a.live_branches = live
+        a.branches = nb; a.live_branches = min(ctx["live"], nb)
         a.layers = ctypes.cast(layers, ctypes.POINTER(_lib.LayerWeights))
         a.tok_emb = P["tok"].data_ptr(); a.pos_emb = P["pos"].data_ptr(); a.final_gamma = P["gf"].data_ptr(); a.w_logits = P["wlog"].data_ptr()
         a.ctx_key_mask = ctx["key_mask"].data_ptr(); a.ctx_keys = ctx["m"]; a.ctx_alloc = ctx["kv"][0][0].shape[1]
@@ -853,23 +889,18 @@ class MaskGit(nn.Module):
 
     def _aten_plan(self, device, b, n, V, timesteps, use_critic):
         """Offsets of the reference's uniform_ calls in torch's CUDA Philox stream (one (b, n, V) gumbel draw, then one (b, n) critic
-        draw per step, muse_maskgit_pytorch.py:407, 598).  Launch geometry as ATen's calc_execution_policy: block 256,
-        grid = min(SMs * maxThreadsPerSM / 256, ceil(numel / 256)), 4 values per thread and round.  The generator is read here and
-        advanced by what the reference would have consumed; seed / offset reach the kernels through device words (graph replay)."""
-        gen = torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
+        draw per step, muse_maskgit_pytorch.py:407, 598) in ATen's launch geometry.  The generator is read here and advanced by what the
+        reference would have consumed; seed / offset reach the kernels through device words (graph replay)."""
         B = self.global_batch if self.global_batch is not None else b
-        ng, nc = B * n * V, B * n
-        stride = lambda numel: _aten_uniform_geometry(device, numel)[0]
-        inc = lambda numel: _aten_uniform_geometry(device, numel)[1]
-        per_step = inc(ng) + (inc(nc) if use_critic else 0)
-        seed, off = gen.initial_seed(), gen.get_offset()
+        (stride_g, inc_g), (stride_c, inc_c) = _aten_uniform_geometry(device, B * n * V), _aten_uniform_geometry(device, B * n)
+        per_step = inc_g + (inc_c if use_critic else 0)
+        seed, off = _reserve_aten_offsets(device, timesteps * per_step)
         self._aten_start_offset = off
-        gen.set_offset(off + timesteps * per_step)
         if getattr(self, "_aten_dev", None) is None or self._aten_dev.device != device:
             self._aten_dev = torch.zeros((2,), dtype=torch.int64, device=device)
         wrap = lambda v: v - (1 << 64) if v >= (1 << 63) else v
         self._aten_dev.copy_(torch.tensor([wrap(seed), off], dtype=torch.int64), non_blocking=False)
-        return dict(key=(B, stride(ng), stride(nc), per_step), stride_g=stride(ng), stride_c=stride(nc), inc_g=inc(ng), per_step=per_step)
+        return dict(key=(B, stride_g, stride_c, per_step), stride_g=stride_g, stride_c=stride_c, inc_g=inc_g, per_step=per_step)
 
     def _tail_buffers(self, b, n, rows_max, V, device, k_keep=None):
         """Scratch of the per-step sampling tail for at most `rows_max` sampled rows per sequence.  bf16 + a supported shape: the workspace of
@@ -907,109 +938,88 @@ class MaskGit(nn.Module):
         ops.linear(e[:R], P["wlog"], lg)
         ops.logits_sample(lg, pos, ids, scores, rows_b, k_keep, temp, **kw)
 
-    def _generate_body(self, text_embeds, cond_images, *, fmap_size, temperature, topk_filter_thres, timesteps, cond_scale, b,
-                       use_critic=False, critic_noise_scale=1., score_all=False, aten=None, inpaint=None, inpaint_rows=None, edit_iterations=None):
-        """The device-side work of generate(): no host synchronisation, no data-dependent host control flow.
-        inpaint (inpaint()): dict(images, frozen uint8 [b, n], counts int32 [timesteps, b]) device tensors; inpaint_rows = the largest
-        number of regenerated tokens of an image, whose schedule gives the rows sampled per step (pad rows fill the smaller counts).
-        edit_iterations (edit()): inpaint holds dict(images, keep uint8 [b, n] (1 = not editable), num_select int32 [b], counts) instead,
-        and the token loop runs edit_iterations times, each preceded by mmg_edit_select, which writes that iteration's frozen map."""
+    def _generate_body(self, req, text_embeds, cond_images, region, aten):
+        """The device-side work of a request: no host synchronisation, no data-dependent host control flow.  region: the device tensors
+        of req.region (or a captured graph's static copies of them)."""
         tr = self.transformer
         device = text_embeds.device
-        n = fmap_size ** 2
-        V = tr.num_tokens
+        b, n, V, timesteps = len(req.texts), req.fmap_size ** 2, tr.num_tokens, req.timesteps
         cond_ids = self.cond_vae.encode_ids(cond_images) if cond_images is not None else None
-        nb = 1 if cond_scale == 1 else 2
+        nb = 1 if req.cond_scale == 1 else 2
         ctx = tr._prepare_context(text_embeds, cond_ids, [False, True][:nb])
         P = tr._packed()
         adt = P["adt"]
-        iterations = 1 if edit_iterations is None else edit_iterations
-        if inpaint is None:
+        edit = req.region is not None and req.region.iterations is not None
+        if req.region is None:
             ids = torch.full((b, n), self.mask_id, dtype=torch.long, device=device)
-        elif edit_iterations is None:
-            ids = self.vae.encode_ids(inpaint["images"]).reshape(b, n).masked_fill(inpaint["frozen"] == 0, self.mask_id)
+        elif edit:
+            ids = self.vae.encode_ids(region["images"]).reshape(b, n)
+            frozen = torch.empty((b, n), dtype=torch.uint8, device=device)          # written by each round's mmg_edit_select
         else:
-            ids = self.vae.encode_ids(inpaint["images"]).reshape(b, n)
-            frozen = torch.empty((b, n), dtype=torch.uint8, device=device)
+            frozen = region["frozen"]
+            ids = self.vae.encode_ids(region["images"]).reshape(b, n).masked_fill(frozen == 0, self.mask_id)
         scores = torch.zeros((b, n), dtype=torch.float32, device=device)
         masked_pos = torch.empty((b, n), dtype=torch.int32, device=device)
-        k_keep = math.ceil((1 - topk_filter_thres) * V)                        # muse_maskgit_pytorch.py:414
-        sched = self.mask_schedule(n if inpaint is None else inpaint_rows, timesteps)
+        k_keep = math.ceil((1 - req.topk_filter_thres) * V)                    # muse_maskgit_pytorch.py:414
+        sched = self.mask_schedule(n if req.region is None else req.region.n_max, timesteps)
+        score_all = bool(req.can_remask_prev_masked) and not req.use_critic
         bn = b * n
         native = None
-        if (self.use_native_step and adt == torch.bfloat16 and not self.self_cond and not use_critic and not score_all and aten is None
-                and inpaint is None and all("w2f" in l["ff"] for l in P["layers"])):
+        if (self.use_native_step and adt == torch.bfloat16 and not self.self_cond and not req.use_critic and not score_all and aten is None
+                and req.region is None and all("w2f" in l["ff"] for l in P["layers"])):
             native = self._native_step_setup(ctx, P, b, n, nb, max(sched), V, device)
         rows_max = n if score_all else max(sched)
         tail = self._tail_buffers(b, n, rows_max, V, device, k_keep) if native is None else None
         all_pos = torch.arange(n, dtype=torch.int32, device=device).repeat(b, 1).contiguous() if score_all else None
         sc_embed = torch.empty((bn, tr.dim), device=device, dtype=torch.float32) if self.self_cond else None
         # token critic (muse_maskgit_pytorch.py:535-538, 590-600): a second stack over the freshly filled ids scores EVERY position
-        if use_critic:
-            if isinstance(self.token_critic, SelfCritic):      # the generator itself; only its conditional embed is used (:352-361)
-                cnet, cnb, cctx = tr, 1, ctx
-                whead, bhead = self.token_critic._head()
-                whead = whead.to(device)
-            else:
-                cnet, cnb = self.token_critic, nb
-                cctx = cnet._prepare_context(text_embeds, cond_ids, [False, True][:nb])
-                whead, bhead = cnet._packed()["whead"], 0.
-                assert whead is not None, "token_critic must have dim_out == 1"
-            gcrit = cnet._packed()["gf"]
+        if req.use_critic:
+            cnet, cnb, cctx, whead, bhead, gcrit = self._resolve_critic(text_embeds, cond_ids, [False, True][:nb], ctx)
+        seed_dev = self._seed_dev if aten is None else self._aten_dev[0:1]
+
+        def aten_draw(step, critic=False):      # (Philox offset, device offset word, stride) of the step's gumbel or critic draw
+            return None if aten is None else (step * aten["per_step"] + (aten["inc_g"] if critic else 0), self._aten_dev[1:2],
+                                              aten["stride_c" if critic else "stride_g"])
+
         nvtx = os.environ.get("MMG_NVTX", "0") == "1"            # host-side NVTX ranges per decode step / stage (visible in nsys / ncu --nvtx)
+        iterations = req.region.iterations if edit else 1
         # edit(): `iterations` rounds of the token loop, step = the global step index (iteration * timesteps + s); one round otherwise
         for step, (num_masked, steps_until_x0) in enumerate(zip(sched * iterations, list(reversed(range(timesteps))) * iterations)):
             s = step % timesteps
-            if edit_iterations is not None and s == 0:
-                it = step // timesteps
-                ukey = None
-                if self.sampler_noise_fn is not None:
-                    ukey = self.sampler_noise_fn(step, (b, n)).to(device=device, dtype=torch.float32).contiguous()
-                ops.edit_select(ids, scores, frozen, inpaint["keep"], inpaint["num_select"], self.mask_id, it, u=ukey,
-                                seed_dev=self._seed_dev, row_offset=self.row_offset * n)
+            if edit and s == 0:
+                ops.edit_select(ids, scores, frozen, region["keep"], region["num_select"], self.mask_id, step // timesteps,
+                                u=self._injected_noise(step, (b, n), device), seed_dev=self._seed_dev, row_offset=self.row_offset * n)
             if nvtx:
                 if step:
                     torch.cuda.nvtx.range_pop()
                 torch.cuda.nvtx.range_push(f"mmg.decode_step[{step}] masked={num_masked}")
+            temp = req.temperature * (steps_until_x0 / timesteps)              # annealed, muse_maskgit_pytorch.py:578
+            u = self._injected_noise(step, (b, n, V), device)
             if native is not None:
-                u = None
-                if self.sampler_noise_fn is not None:
-                    u = self.sampler_noise_fn(step, (b, n, V)).to(device=device, dtype=torch.float32).contiguous()
                 a = native["args"]
                 a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.masked_pos = masked_pos.data_ptr()
                 a.num_masked = num_masked; a.k_keep = k_keep; a.step = step
-                a.temperature = float(temperature * (steps_until_x0 / timesteps)); a.cond_scale = float(cond_scale)
+                a.temperature = float(temp); a.cond_scale = float(req.cond_scale)
                 a.u = None if u is None else u.data_ptr(); a.seed = 0; a.seed_dev = self._seed_dev.data_ptr(); a.row_offset = self.row_offset * n
                 _lib.call("mmg_decode_step", a)
                 continue
-            if inpaint is None:
+            if req.region is None:
                 ops.remask(ids, scores, masked_pos, num_masked, self.mask_id)
             else:      # each image re-masks among its own regenerated tokens; num_masked rows per image, the surplus padded
-                ops.remask_frozen(ids, scores, masked_pos, inpaint["frozen"] if edit_iterations is None else frozen, inpaint["counts"][s],
-                                  num_masked, self.mask_id)
+                ops.remask_frozen(ids, scores, masked_pos, frozen, region["counts"][s], num_masked, self.mask_id)
             x = tr._run_blocks(ids, ctx, nb, sc_embed if (self.self_cond and s > 0) else None)
             if self.self_cond:                                                 # embed of the conditional forward, fed back next step (:574)
                 ops.layernorm(x[:bn], P["gf"], sc_embed)
             # rows that are sampled: the masked ones; every position when already-decoded tokens may be re-masked by confidence
             pos, rows_b = (all_pos, n) if score_all else (masked_pos, num_masked)
-            temp = temperature * (steps_until_x0 / timesteps)                  # annealed, muse_maskgit_pytorch.py:578
-            u = None
-            if self.sampler_noise_fn is not None:
-                u = self.sampler_noise_fn(step, (b, n, V)).to(device=device, dtype=torch.float32).contiguous()
-            seed_dev = self._seed_dev if aten is None else self._aten_dev[0:1]
-            self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(cond_scale), k_keep, tail, seed_dev=seed_dev,
-                              only_masked_id=self.mask_id if score_all or inpaint is not None else None,
-                              aten=None if aten is None else (step * aten["per_step"], self._aten_dev[1:2], aten["stride_g"]))
-            if use_critic:
+            self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(req.cond_scale), k_keep, tail, seed_dev=seed_dev,
+                              only_masked_id=self.mask_id if score_all or req.region is not None else None, aten=aten_draw(step))
+            if req.use_critic:
                 xc = cnet._run_blocks(ids, cctx, cnb)
-                uc = None
-                if self.sampler_noise_fn is not None:
-                    uc = self.sampler_noise_fn(step, (b, n)).to(device=device, dtype=torch.float32).contiguous()
-                ops.critic_score(xc[:bn], xc[bn:2 * bn] if cnb == 2 else None, gcrit, whead, float(bhead), float(cond_scale),
-                                 float(critic_noise_scale * (steps_until_x0 / timesteps)), scores, u=uc, seed=0, seed_dev=seed_dev,
-                                 step=step, row_offset=self.row_offset * n,
-                                 aten=None if aten is None else (step * aten["per_step"] + aten["inc_g"], self._aten_dev[1:2], aten["stride_c"]))
-        ids = ids.view(b, fmap_size, fmap_size)
+                ops.critic_score(xc[:bn], xc[bn:2 * bn] if cnb == 2 else None, gcrit, whead, float(bhead), float(req.cond_scale),
+                                 float(req.critic_noise_scale * (steps_until_x0 / timesteps)), scores, u=self._injected_noise(step, (b, n), device),
+                                 seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, aten=aten_draw(step, critic=True))
+        ids = ids.view(b, req.fmap_size, req.fmap_size)
         if nvtx:
             torch.cuda.nvtx.range_pop()
             torch.cuda.nvtx.range_push("mmg.vae_decode")
@@ -1045,9 +1055,7 @@ class MaskGit(nn.Module):
         if cond_token_ids is not None:
             self._check_ids(cond_token_ids, "cond_token_ids")
         assert (texts is None) != (text_embeds is None), "pass exactly one of texts / text_embeds"
-        for net in (tr, self.vae, self.cond_vae, self.token_critic if isinstance(self.token_critic, Transformer) else None):
-            if net is not None:
-                net._check_weights()
+        self._check_weights()
         if images_or_ids.dtype == torch.float:
             ids = self.vae.encode_ids(images_or_ids.to(device, torch.float32).contiguous())
         else:
@@ -1060,7 +1068,7 @@ class MaskGit(nn.Module):
             cond_token_ids = self.cond_vae.encode_ids(cond_images.to(device, torch.float32).contiguous())
         cond_ids = None if cond_token_ids is None else cond_token_ids.to(device, torch.long).reshape(b, -1).contiguous()
         if self.sampler_noise_fn is not None:
-            draw = lambda shape: self.sampler_noise_fn(0, shape).to(device=device, dtype=torch.float32)
+            draw = lambda shape: self._injected_noise(0, shape, device)
         else:
             draw = lambda shape: torch.zeros(shape, device=device).uniform_(0, 1)
         # ---- masks and labels (:670-686): labels use the mask before the no-mask subset is removed, the input x the mask after it
@@ -1112,12 +1120,10 @@ class MaskGit(nn.Module):
         critic_input = x.clone()
         kw = dict(seed=0, step=0, row_offset=0, only_masked_id=mask_id)
         if self.sampler_noise_fn is not None:
-            kw["u"] = draw((b, n, V)).contiguous()
+            kw["u"] = draw((b, n, V))
         elif self.sampler_rng == "aten":
-            gen = torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
             stride, inc = _aten_uniform_geometry(device, b * n * V)
-            seed, off = gen.initial_seed(), gen.get_offset()
-            gen.set_offset(off + inc)
+            seed, off = _reserve_aten_offsets(device, inc)
             kw.update(seed=seed, aten=(off, None, stride))
         else:
             assert self.sampler_rng == "mmg", self.sampler_rng
@@ -1127,17 +1133,10 @@ class MaskGit(nn.Module):
                           float(temperature), **kw)
         critic_labels = (ids != critic_input).float()
         te_c = self._drop_text(text_embeds, cond_drop_prob, draw)
-        if isinstance(self.token_critic, SelfCritic):
-            cnet = tr
-            whead, bhead = self.token_critic._head()
-            whead = whead.to(device)
-        else:
-            cnet = self.token_critic
-            whead, bhead = cnet._packed()["whead"], 0.
-            assert whead is not None, "token_critic must have dim_out == 1"
-        xc = cnet._run_blocks(critic_input, cnet._prepare_context(te_c, cond_ids, [cond_drop_prob == 1]), 1)
+        cnet, _, cctx, whead, bhead, gcrit = self._resolve_critic(te_c, cond_ids, [cond_drop_prob == 1])
+        xc = cnet._run_blocks(critic_input, cctx, 1)
         critic_logits = torch.empty((b * n,), device=device, dtype=torch.float32)
-        ops.critic_score(xc, None, cnet._packed()["gf"], whead, float(bhead), 1., 0., critic_logits)
+        ops.critic_score(xc, None, gcrit, whead, float(bhead), 1., 0., critic_logits)
         bce_loss = torch.nn.functional.binary_cross_entropy_with_logits(critic_logits.view(b, n), critic_labels)
         return ce_loss + self.critic_loss_weight * bce_loss
 

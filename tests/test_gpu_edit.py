@@ -193,9 +193,9 @@ def test_graph_replay_determinism_and_weight_edit():
     run = lambda: mg.edit(["a"] * 3, img, mask=m, iterations=3, fraction=0.5, timesteps=4, return_ids=True)
     a, ida = run()
     key = list(mg._graphs)[-1]
-    graph_obj = mg._graphs[key][0]
+    graph_obj = mg._graphs[key].graph
     a2, ida2 = run()
-    assert mg._graphs[key][0] is graph_obj and key[-1] == ("edit", 3, 8)
+    assert mg._graphs[key].graph is graph_obj and key[-1] == ("edit", 3, 8)
     mg.use_cuda_graph = False
     b_, idb = run()
     assert torch.equal(ida, ida2) and torch.equal(a, a2) and torch.equal(ida, idb) and torch.equal(a, b_)
@@ -203,7 +203,7 @@ def test_graph_replay_determinism_and_weight_edit():
     mg.use_cuda_graph = True
     mg.transformer.to_logits.weight.mul_(1.5)
     c, idc = run()
-    assert mg._graphs[key][0] is not graph_obj
+    assert mg._graphs[key].graph is not graph_obj
     mg.use_cuda_graph = False
     d, idd = run()
     assert torch.equal(idc, idd) and torch.equal(c, d) and not torch.equal(idc, ida)

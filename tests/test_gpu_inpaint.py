@@ -241,10 +241,10 @@ def test_graph_replay_determinism_and_repack():
     run = lambda m: mg.inpaint(["a"] * 3, img, m.cuda(), timesteps=8, return_ids=True)
     a, ida = run(m1)
     keys = list(mg._graphs)
-    graph_obj = mg._graphs[keys[-1]][0]
+    graph_obj = mg._graphs[keys[-1]].graph
     a2, ida2 = run(m1)
     c, idc = run(m2)                                           # same N_max: the captured graph replays with the new mask
-    assert list(mg._graphs) == keys and mg._graphs[keys[-1]][0] is graph_obj
+    assert list(mg._graphs) == keys and mg._graphs[keys[-1]].graph is graph_obj
     assert keys[-1][-1] == ("inpaint", 16)
     mg.use_cuda_graph = False
     b_, idb = run(m1)

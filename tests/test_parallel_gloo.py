@@ -43,7 +43,7 @@ def _worker(rank, world, port, total, q):
     assert mg.sampler_seed == (None if rank else 4242)
     lo, hi = parallel.shard_bounds(total, rank, world)
     assert mg.seen == ([(4242, total, lo)] if hi > lo else []), mg.seen
-    q.put((rank, out))
+    q.put((rank, out.numpy()))      # by value: a shared tensor's storage would be fetched from this process, which may have exited by then
     dist.barrier()
     dist.destroy_process_group()
 
@@ -54,7 +54,7 @@ def _run(total, port):
     procs = [ctx.Process(target=_worker, args=(r, 2, port, total, q)) for r in range(2)]
     for p in procs:
         p.start()
-    outs = dict(q.get(timeout=120) for _ in range(2))
+    outs = {rank: torch.from_numpy(out) for rank, out in (q.get(timeout=120) for _ in range(2))}
     for p in procs:
         p.join(timeout=60)
         assert p.exitcode == 0
