@@ -283,12 +283,15 @@ int mmg_edit_select(const mmg_edit_select_args* a, void* stream);
 
 /* Final LayerNorm + classifier-free-guidance combine on the masked rows only, in embedding space:
  *   e[j] = LN(x_null[r]) + (LN(x_cond[r]) - LN(x_null[r])) * cond_scale,  r = b*n + masked_pos[b, j]
- * (to_logits is linear and bias-free, so W e == null + (cond - null) * scale of muse_maskgit_pytorch.py:254).    */
+ * (to_logits is linear and bias-free, so W e == null + (cond - null) * scale of muse_maskgit_pytorch.py:254).
+ * cond_scale_dev != NULL: image b combines at cond_scale_dev[b] instead, and an image whose scale is exactly 1 takes LN(x_cond)
+ * alone without reading x_null (bitwise the x_null == NULL launch).                                                 */
 typedef struct {
   const float* x_cond; const float* x_null;  /* [B*n, dim] fp32; x_null may be NULL (cond_scale == 1)             */
   const float* gamma; const int32_t* masked_pos;
   void* e; int32_t e_dtype;
   int32_t B, n, num_masked, dim; float cond_scale;
+  const float* cond_scale_dev;               /* [B] per-image scales or NULL (use cond_scale)                     */
 } mmg_final_embed_args;
 int mmg_final_embed(const mmg_final_embed_args* a, void* stream);
 
@@ -320,6 +323,8 @@ typedef struct {
   /* optional row indirection (the fallback leg of mmg_logits_fused): logits row j belongs to sampled row row_index[j] (the index into
      masked_pos), only the first min(*row_count_dev, row_index_cap) rows are processed; the grid is row_index_cap CTAs               */
   const int32_t* row_index; const int32_t* row_count_dev; int32_t row_index_cap, _pad2;
+  const float* temperature_dev;  /* [B] per-image temperatures or NULL (use `temperature`): sampled row j of image b = j / num_masked
+                                    divides by max(temperature_dev[b], 1e-10)                                                       */
 } mmg_logits_sample_args;
 int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream);
 
@@ -376,7 +381,9 @@ int mmg_logits_xent_rows(const mmg_logits_xent_rows_args* a, void* stream);
  *   s[r] = dot(LayerNorm(x_cond[r]) * gamma, w) + bias;   x_null != NULL: s = s_null + (s - s_null) * cond_scale  (CFG, :257)
  *   scores[r] = s + (u[r] - 0.5) * noise_mul       noise_mul = critic_noise_scale * steps_until_x0 / timesteps
  * x_* are the residual streams after the critic's last block (the final LayerNorm and the 1-wide head are applied here).
- * u == NULL: u = Philox4x32-10(counter = (0xFFFFFFFF, step, row_offset + r), key = seed + *seed_dev) >> 8 * 2^-24.            */
+ * u == NULL: u = Philox4x32-10(counter = (0xFFFFFFFF, step, row_offset + r), key = seed + *seed_dev) >> 8 * 2^-24.
+ * cond_scale_dev / noise_mul_dev != NULL: row r reads its scale / noise multiplier from them instead of the scalars (a host expands
+ * per-image settings over the image's rows); a row whose scale is exactly 1 keeps s from x_cond alone, as the x_null == NULL launch. */
 typedef struct {
   const float* x_cond; const float* x_null;   /* [rows, dim] fp32; x_null may be NULL (cond_scale == 1, SelfCritic)   */
   const float* gamma; const float* w;         /* [dim] final LayerNorm gain, [dim] head weight (to_logits / to_pred)  */
@@ -386,6 +393,7 @@ typedef struct {
   int64_t rows, row_offset; uint64_t seed; const uint64_t* seed_dev; int32_t step;
   int32_t rng_mode;                           /* 1: ATen's `uniform(scores.shape)` stream (:598), see mmg_logits_sample_args */
   uint64_t aten_offset; const uint64_t* aten_offset_dev; uint32_t aten_stride, _pad;
+  const float* cond_scale_dev; const float* noise_mul_dev;   /* [rows] per-row values or NULL (use cond_scale / noise_mul)      */
 } mmg_critic_score_args;
 int mmg_critic_score(const mmg_critic_score_args* a, void* stream);
 
@@ -463,6 +471,8 @@ typedef struct {
   const float* u; uint64_t seed; const uint64_t* seed_dev; int64_t row_offset;   /* noise: see mmg_logits_sample_args        */
   void* workspace; uint64_t workspace_bytes;      /* >= mmg_decode_step_workspace_bytes(...), 256-byte aligned, ZERO-INITIALISED once by
                                                      the caller (the padding rows of the self-attention K/V stay zero)        */
+  const float* cond_scale_dev; const float* temperature_dev;   /* [b] per-image settings or NULL (use cond_scale / temperature): passed
+                                                     to mmg_final_embed_args.cond_scale_dev / mmg_logits_sample_args.temperature_dev */
 } mmg_decode_step_args;
 uint64_t mmg_decode_step_workspace_bytes(int32_t b, int32_t branches, int32_t n, int32_t dim, int32_t heads, int32_t Fp, int32_t V, int32_t max_masked);
 int mmg_decode_step(const mmg_decode_step_args* a, void* stream);

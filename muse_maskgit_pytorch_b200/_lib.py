@@ -91,7 +91,7 @@ class EditSelectArgs(C.Structure):
 
 class FinalEmbedArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("masked_pos", vp), ("e", vp), ("e_dtype", i32),
-                ("B", i32), ("n", i32), ("num_masked", i32), ("dim", i32), ("cond_scale", f32)]
+                ("B", i32), ("n", i32), ("num_masked", i32), ("dim", i32), ("cond_scale", f32), ("cond_scale_dev", vp)]
 
 
 class LogitsSampleArgs(C.Structure):
@@ -99,7 +99,7 @@ class LogitsSampleArgs(C.Structure):
                 ("B", i32), ("n", i32), ("num_masked", i32), ("V", i32), ("k", i32), ("temperature", f32),
                 ("seed", u64), ("step", u64), ("row_offset", i64), ("seed_dev", vp), ("mask_id", i64), ("only_masked", i32), ("rng_mode", i32),
                 ("aten_offset", u64), ("aten_offset_dev", vp), ("aten_stride", C.c_uint32), ("_pad", i32),
-                ("row_index", vp), ("row_count_dev", vp), ("row_index_cap", i32), ("_pad2", i32)]
+                ("row_index", vp), ("row_count_dev", vp), ("row_index_cap", i32), ("_pad2", i32), ("temperature_dev", vp)]
 
 
 class LogitsFusedArgs(C.Structure):
@@ -119,7 +119,8 @@ class LogitsXentRowsArgs(C.Structure):
 class CriticScoreArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("w", vp), ("bias", f32), ("cond_scale", f32), ("noise_mul", f32),
                 ("dim", i32), ("u", vp), ("scores", vp), ("rows", i64), ("row_offset", i64), ("seed", u64), ("seed_dev", vp),
-                ("step", i32), ("rng_mode", i32), ("aten_offset", u64), ("aten_offset_dev", vp), ("aten_stride", C.c_uint32), ("_pad", i32)]
+                ("step", i32), ("rng_mode", i32), ("aten_offset", u64), ("aten_offset_dev", vp), ("aten_stride", C.c_uint32), ("_pad", i32),
+                ("cond_scale_dev", vp), ("noise_mul_dev", vp)]
 
 
 class FfGegluArgs(C.Structure):
@@ -142,7 +143,8 @@ class DecodeStepArgs(C.Structure):
                 ("live_branches", i32), ("layers", C.POINTER(LayerWeights)), ("tok_emb", vp), ("pos_emb", vp), ("final_gamma", vp), ("w_logits", vp),
                 ("ctx_key_mask", vp), ("ctx_keys", i32), ("ctx_alloc", i32), ("ids", vp), ("scores", vp), ("masked_pos", vp), ("mask_id", i64),
                 ("num_masked", i32), ("k_keep", i32), ("step", i32), ("temperature", f32), ("cond_scale", f32), ("_pad", i32),
-                ("u", vp), ("seed", u64), ("seed_dev", vp), ("row_offset", i64), ("workspace", vp), ("workspace_bytes", u64)]
+                ("u", vp), ("seed", u64), ("seed_dev", vp), ("row_offset", i64), ("workspace", vp), ("workspace_bytes", u64),
+                ("cond_scale_dev", vp), ("temperature_dev", vp)]
 
 
 class LfqEncodeArgs(C.Structure):

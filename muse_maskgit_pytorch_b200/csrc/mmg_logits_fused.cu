@@ -469,6 +469,7 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
     const uint2* row_lists = f.lists + r * (int64_t)nseg * f.cap;
     const int64_t grow = a.row_offset + (int64_t)b * a.n + pos;
     const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+    tdiv = image_tdiv(a, b, tdiv);
     const float inv_t = 1.0f / tdiv;
     uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
     if (MODE == 2) {            // flat index of logit (grow, v) in the reference's [B, n, V] noise tensor = grow * V + v = ar0 + v + S * aq0

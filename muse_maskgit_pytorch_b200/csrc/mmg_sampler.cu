@@ -231,7 +231,7 @@ logits_sample_kernel(const mmg_logits_sample_args a, float tdiv) {
 
   // ---------------- phase C: perturbed argmax restricted to the exact top-k ----------------
   int win_v; float win_x;
-  sample_from_list<MODE>(a, tdiv, lval, lidx, n, k, V, b, pos, sc, tid, warp, lane, win_v, win_x);
+  sample_from_list<MODE>(a, image_tdiv(a, b, tdiv), lval, lidx, n, k, V, b, pos, sc, tid, warp, lane, win_v, win_x);
   if (tid == 0) {
     if (win_v < 0) { win_v = 0; win_x = row[0]; }                 // degenerate rows (all -inf / NaN)
     const float p = expf(win_x - s_max) / s_sum;
@@ -253,7 +253,7 @@ __global__ void __launch_bounds__(SMP_THREADS)
 logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   __shared__ SampleScratch sc;
   __shared__ int s_cut;
-  __shared__ float s_m, s_s;
+  __shared__ float s_m, s_s, s_tdiv;
   pdl_wait(); pdl_trigger();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int V = a.V, k = a.k;
@@ -262,6 +262,8 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   if (a.row_index) { if ((int)blockIdx.x >= *a.row_count_dev) return; r = a.row_index[blockIdx.x]; }
   const int b = (int)(r / a.num_masked);
   const int pos = a.masked_pos[r];
+  // the row's temperature, read after the descent loop's barriers.  Held in a register across that loop, it made MODE 2 spill 8 bytes.
+  if (tid == 0) s_tdiv = image_tdiv(a, b, tdiv);
   // 1. k-th largest key
   uint32_t prefix = 0;
   for (int bit = 31; bit >= 0; --bit) {
@@ -301,7 +303,7 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   // 2. statistics + perturbed argmax over the kept set
   const int64_t grow = a.row_offset + (int64_t)b * a.n + pos;
   const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
-  const float inv_t = 1.0f / tdiv;
+  const float inv_t = 1.0f / s_tdiv;
   uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
   if (MODE == 2) {
     const uint64_t base = (uint64_t)grow * (uint64_t)V;
@@ -323,7 +325,7 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
         if (MODE == 1) u = a.u[((int64_t)b * a.n + pos) * V + v];
         else { const uint32_t rr = ar0 + (uint32_t)v, dq = rr / a.aten_stride; u = aten_uniform(rr - dq * a.aten_stride, aq0 + dq, aoff4, seed); }
         const float l1 = logf(fmaxf(u, 1e-20f));
-        p = __fdiv_rn(x, tdiv) - logf(fmaxf(-l1, 1e-20f));
+        p = __fdiv_rn(x, s_tdiv) - logf(fmaxf(-l1, 1e-20f));
       } else {
         const float u = (float)(philox_first((uint32_t)v, (uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed, (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
         const float l1 = __logf(fmaxf(u, 1e-20f));
@@ -509,9 +511,10 @@ critic_score_kernel(mmg_critic_score_args a) {
   const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= a.rows) return;
   float s = critic_head(a.x_cond + row * a.dim, a.gamma, a.w, a.dim, lane) + a.bias;
-  if (a.x_null) {
+  const float cs = a.cond_scale_dev ? a.cond_scale_dev[row] : a.cond_scale;
+  if (a.x_null && !(a.cond_scale_dev && cs == 1.f)) {       // a per-row scale of exactly 1 scores x_cond alone, as x_null == NULL
     const float sn = critic_head(a.x_null + row * a.dim, a.gamma, a.w, a.dim, lane) + a.bias;
-    s = sn + (s - sn) * a.cond_scale;
+    s = sn + (s - sn) * cs;
   }
   if (lane == 0) {
     float u;
@@ -525,7 +528,7 @@ critic_score_kernel(mmg_critic_score_args a) {
       } else
         u = (float)(philox_first(0xFFFFFFFFu, (uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed, (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
     }
-    a.scores[row] = s + (u - 0.5f) * a.noise_mul;
+    a.scores[row] = s + (u - 0.5f) * (a.noise_mul_dev ? a.noise_mul_dev[row] : a.noise_mul);
   }
 }
 

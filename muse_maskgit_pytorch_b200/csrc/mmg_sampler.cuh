@@ -165,6 +165,13 @@ __device__ __forceinline__ float sample_threshold(const uint32_t (&sk)[SMP_SPT],
   return tlo;
 }
 
+// max(temperature, 1e-10) of image b (muse_maskgit_pytorch.py:411): the per-image table when given, else the launcher's clamped scalar
+__device__ __forceinline__ float image_tdiv(const mmg_logits_sample_args& a, int b, float tdiv) {
+  if (!a.temperature_dev) return tdiv;
+  const float t = a.temperature_dev[b];
+  return t < 1e-10f ? 1e-10f : t;
+}
+
 // ---------------- phase C: perturbed argmax restricted to the exact top-k ----------------
 // lval / lidx: the n candidates of the row (every element >= some threshold, n >= k or the complete exact top-k); (b, pos): the row.
 // MODE 1 = injected-noise parity mode, MODE 2 = ATen-compatible in-kernel Philox (the stream a seeded torch.cuda run of the reference

@@ -132,7 +132,7 @@ extern "C" int mmg_decode_step(const mmg_decode_step_args* a, void* stream) {
   }
   {   // final LayerNorm + CFG combine in embedding space, masked rows only (:195, 254)
     mmg_final_embed_args f{}; f.x_cond = x; f.x_null = a->branches == 2 ? x + bn * a->dim : nullptr; f.gamma = a->final_gamma; f.masked_pos = a->masked_pos; f.e = e; f.e_dtype = MMG_BF16;
-    f.B = a->b; f.n = a->n; f.num_masked = a->num_masked; f.dim = a->dim; f.cond_scale = a->cond_scale;
+    f.B = a->b; f.n = a->n; f.num_masked = a->num_masked; f.dim = a->dim; f.cond_scale = a->cond_scale; f.cond_scale_dev = a->cond_scale_dev;
     if ((rc = mmg_final_embed(&f, stream))) return rc;
   }
   const int64_t Rm = (int64_t)a->b * a->num_masked;
@@ -140,7 +140,7 @@ extern "C" int mmg_decode_step(const mmg_decode_step_args* a, void* stream) {
     if ((rc = linear_bf16(e, a->w_logits, Rm, a->V, a->dim, MMG_EPI_STORE, ep, stream))) return rc; }
   {   // top-k filter + gumbel argmax + confidence (:576-609)
     mmg_logits_sample_args s{}; s.logits = logits; s.masked_pos = a->masked_pos; s.ids = a->ids; s.scores = a->scores; s.u = a->u;
-    s.B = a->b; s.n = a->n; s.num_masked = a->num_masked; s.V = a->V; s.k = a->k_keep; s.temperature = a->temperature;
+    s.B = a->b; s.n = a->n; s.num_masked = a->num_masked; s.V = a->V; s.k = a->k_keep; s.temperature = a->temperature; s.temperature_dev = a->temperature_dev;
     s.seed = a->seed; s.step = (uint64_t)a->step; s.row_offset = a->row_offset; s.seed_dev = a->seed_dev;
     if ((rc = mmg_logits_sample(&s, stream))) return rc;
   }

@@ -11,6 +11,7 @@ constant to_out(null_v) (every text key masked -> softmax puts weight exactly 1 
 import ctypes
 import dataclasses
 import math
+import numbers
 import os
 import random
 from functools import partial
@@ -543,28 +544,80 @@ class _Region:
     tensors: dict
 
 
+def _per_image(name, value, b):
+    """A sampling setting of generate() / inpaint() / edit() as a tuple of b Python floats: `value` is a number (every image), or a
+    length-b sequence of numbers or 1-D tensor (image by image).  Raises ValueError on a wrong length or a value that is not finite."""
+    if isinstance(value, torch.Tensor):
+        if value.dim() > 1:
+            raise ValueError(f"{name} must be a number or 1-D, got a tensor of shape {tuple(value.shape)}")
+        value = value.item() if value.dim() == 0 else value.detach().cpu().double().tolist()
+    if isinstance(value, numbers.Real):
+        vals = (float(value),) * b
+    else:
+        try:
+            vals = tuple(float(v) for v in value)
+        except (TypeError, ValueError):
+            raise ValueError(f"{name} must be a number, a sequence of numbers or a 1-D tensor, got {value!r}") from None
+        if len(vals) != b:
+            raise ValueError(f"{name} has {len(vals)} values for {b} texts")
+    if not all(math.isfinite(v) for v in vals):
+        raise ValueError(f"{name} must be finite, got {vals}")
+    return vals
+
+
+def _fill_on_device(t, device):
+    """Host tensor `t` rebuilt on `device` with one fill kernel per run of equal values.  Used when a caller captures the whole call into
+    their own CUDA graph, where a host-to-device copy cannot be recorded; the values are then fixed in that graph, as scalar arguments are."""
+    flat = t.reshape(-1).tolist()
+    out = torch.empty((len(flat),), dtype=t.dtype, device=device)
+    start = 0
+    for i in range(1, len(flat) + 1):
+        if i == len(flat) or flat[i] != flat[start]:
+            out[start:i].fill_(flat[start])
+            start = i
+    return out.view(t.shape)
+
+
 @dataclasses.dataclass(frozen=True)
 class _DecodeRequest:
-    """One validated generate() / inpaint() / edit() call.  seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs)."""
+    """One validated generate() / inpaint() / edit() call.  temperature, cond_scale, critic_noise_scale: one float per image.
+    seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs)."""
     texts: List[str]
     cond_images: Optional[torch.Tensor]
     fmap_size: int
-    temperature: float
+    temperature: tuple
     topk_filter_thres: float
     timesteps: int
-    cond_scale: float
-    critic_noise_scale: float
+    cond_scale: tuple
+    critic_noise_scale: tuple
     can_remask_prev_masked: bool
     use_critic: bool
     return_ids: bool
     region: Optional[_Region] = None
     seed: Optional[int] = None
 
+    @property
+    def branches(self):
+        """CFG branches of the call: 1 when every image's cond_scale is 1 (no null forward, as the reference), else 2."""
+        return 1 if all(c == 1 for c in self.cond_scale) else 2
+
+    def settings(self, n):
+        """The host fp32 tables the sampling kernels read, each value the float64 expression of a scalar call rounded once: temps and
+        crit_noise [timesteps, b] (step s anneals by steps_until_x0 / timesteps, muse_maskgit_pytorch.py:578, 600), cond_scale [b]; with a
+        critic, its per-row copies over the n positions of each image (crit_cond_scale [b*n], crit_noise [timesteps, b*n])."""
+        anneal = [until / self.timesteps for until in reversed(range(self.timesteps))]
+        f32 = lambda v: torch.tensor(v, dtype=torch.float32)
+        out = dict(temps=f32([[t * a for t in self.temperature] for a in anneal]), cond_scale=f32(self.cond_scale))
+        if self.use_critic:
+            out["crit_cond_scale"] = out["cond_scale"].repeat_interleave(n)
+            out["crit_noise"] = f32([[c * a for c in self.critic_noise_scale] for a in anneal]).repeat_interleave(n, dim=1)
+        return out
+
 
 class _CapturedCall(NamedTuple):
     """A whole-call CUDA graph of MaskGit._generate_body and the static tensors it reads and writes."""
     graph: "torch.cuda.CUDAGraph"
-    inputs: tuple               # (text_embeds, cond_images or None, region tensors or None), copied in before each replay
+    inputs: tuple               # (text_embeds, cond_images or None, region tensors or None, settings tables), copied in before each replay
     outputs: tuple              # (images, ids, fused-tail status or None)
     pack_ids: tuple             # identities of the packed weights at capture: a re-pack re-captures
     keep_alive: tuple           # packed weights and workspaces the captured kernels point at
@@ -637,7 +690,12 @@ class MaskGit(nn.Module):
     def generate(self, texts: List[str], negative_texts: Optional[List[str]] = None, cond_images: Optional[torch.Tensor] = None,
                  fmap_size=None, temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False,
                  force_not_use_token_critic=False, timesteps=18, cond_scale=3, critic_noise_scale=1, return_ids=False):
-        """ref: muse_maskgit_pytorch.py:491-621.  Returns fp32 NCHW images (b, 3, H, W), unclamped."""
+        """ref: muse_maskgit_pytorch.py:491-621.  Returns fp32 NCHW images (b, 3, H, W), unclamped.
+
+        temperature, cond_scale and critic_noise_scale are each a number (every image) or per image, a length-b sequence of numbers or a
+        1-D tensor on any device: image i is decoded as if the whole call had been made with its own values (values must be finite,
+        temperature >= 0).  The settings reach the kernels as device data, so one captured CUDA graph replays for any of them; only
+        whether every image has cond_scale == 1 (no null-CFG forward) selects a different graph.  inpaint() and edit() take them alike."""
         if self.use_native_step and self.transformer.precision == "fp8":
             raise ValueError('use_native_step=True runs mmg_decode_step, whose weights carry no fp8 scales: it cannot run precision="fp8"; '
                              "set use_native_step = False")
@@ -733,6 +791,10 @@ class MaskGit(nn.Module):
         if settings["can_remask_prev_masked"] and not use_critic:      # the reference only reaches this assert in the no-critic branch (:611-612)
             assert self.no_mask_token_prob > 0., "without training with some of the non-masked tokens forced to predict, not sure if the logits will be meaningful for these token"
         fmap_size = fmap_size if fmap_size is not None else self.vae.get_encoded_fmap_size(self.image_size)
+        for name in ("temperature", "cond_scale", "critic_noise_scale"):
+            settings[name] = _per_image(name, settings[name], len(texts))
+        if any(t < 0 for t in settings["temperature"]):
+            raise ValueError(f"temperature must be >= 0, got {settings['temperature']}")
         return _DecodeRequest(texts=texts, fmap_size=fmap_size, use_critic=use_critic, **settings)
 
     def _check_weights(self):          # in-place parameter edits since the last call drop the packed copies (and the captured graphs)
@@ -806,12 +868,15 @@ class MaskGit(nn.Module):
                 seed = self.sampler_seed if self.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
             self._seed_dev.fill_(seed)
         region = None if req.region is None else req.region.tensors
+        # per-image sampling settings as device data: a captured graph copies them in like the region, so they are not in its key
+        upload = _fill_on_device if torch.cuda.is_current_stream_capturing() else (lambda t, dev: t.to(dev))
+        settings = {k: upload(v, device) for k, v in req.settings(req.fmap_size ** 2).items()}
         if not self.use_cuda_graph or self.sampler_noise_fn is not None:
-            return self._generate_body(req, text_embeds, cond_images, region, aten) + (seed,)
+            return self._generate_body(req, text_embeds, cond_images, region, settings, aten) + (seed,)
         # ---- whole-call CUDA graph: 18 decode steps + VAE decode replayed as one launch (no per-kernel host work) ----
         key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), req.fmap_size,
-               float(req.temperature), float(req.topk_filter_thres), int(req.timesteps), float(req.cond_scale), int(self.row_offset),
-               tr.precision, self.vae.precision, req.use_critic, float(req.critic_noise_scale), bool(req.can_remask_prev_masked),
+               float(req.topk_filter_thres), int(req.timesteps), req.branches, int(self.row_offset),
+               tr.precision, self.vae.precision, req.use_critic, bool(req.can_remask_prev_masked),
                None if aten is None else aten["key"], bool(self.use_native_step), id(self.noise_schedule), bool(self.use_fused_tail))
         if req.region is not None:
             key += (("inpaint", req.region.n_max) if req.region.iterations is None else ("edit", req.region.iterations, req.region.n_max),)
@@ -825,12 +890,13 @@ class MaskGit(nn.Module):
             te_s = text_embeds.clone()
             ci_s = None if cond_images is None else cond_images.clone()
             region_s = None if region is None else {k: v.clone() for k, v in region.items()}
-            self._generate_body(req, te_s, ci_s, region_s, aten)        # eager warm-up: lazy packing, workspaces, function attributes
+            settings_s = {k: v.clone() for k, v in settings.items()}
+            self._generate_body(req, te_s, ci_s, region_s, settings_s, aten)        # eager warm-up: lazy packing, workspaces, function attributes
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                outputs = self._generate_body(req, te_s, ci_s, region_s, aten)
-            entry = _CapturedCall(graph, (te_s, ci_s, region_s), outputs, pack_ids(),
+                outputs = self._generate_body(req, te_s, ci_s, region_s, settings_s, aten)
+            entry = _CapturedCall(graph, (te_s, ci_s, region_s, settings_s), outputs, pack_ids(),
                                   keep_alive=(tr._pack, self.vae._pack, self.cond_vae._pack, dict(getattr(tr, "_ws", {})),
                                               None if critic_net is None else (critic_net._pack, dict(getattr(critic_net, "_ws", {}))),
                                               self.token_critic._head_cache if isinstance(self.token_critic, SelfCritic) else None))
@@ -838,12 +904,14 @@ class MaskGit(nn.Module):
                 self._graphs.pop(next(iter(self._graphs)))       # least recently used (hits are moved to the end below)
         self._graphs.pop(key, None)
         self._graphs[key] = entry
-        te_s, ci_s, region_s = entry.inputs
+        te_s, ci_s, region_s, settings_s = entry.inputs
         te_s.copy_(text_embeds, non_blocking=True)
         if ci_s is not None:
             ci_s.copy_(cond_images, non_blocking=True)
         for k, v in (region_s or {}).items():
             v.copy_(region[k], non_blocking=True)
+        for k, v in settings_s.items():
+            v.copy_(settings[k], non_blocking=True)
         entry.graph.replay()
         images, ids, status = entry.outputs
         return images.clone(), ids.clone(), status, seed
@@ -918,18 +986,21 @@ class MaskGit(nn.Module):
             bufs["logits"] = torch.empty((b * rows_max, V), device=device, dtype=torch.float32)
         return bufs
 
-    def _sample_tail(self, x, nb, pos, rows_b, ids, scores, temp, step, u, cond_scale, k_keep, tail, seed_dev=None, only_masked_id=None, aten=None):
+    def _sample_tail(self, x, nb, pos, rows_b, ids, scores, temp, step, u, cond_scale, k_keep, tail, seed_dev=None, only_masked_id=None, aten=None,
+                     temp_dev=None, cond_scale_dev=None):
         """The sampling tail of one decode step (muse_maskgit_pytorch.py:576-609) on the rows listed in `pos` (b, rows_b): final LayerNorm +
         CFG combine in embedding space, to_logits, top-k filter, gumbel argmax, confidence score; ids / scores are updated in place.
-        x: residual stream [nb*b*n, dim] after the blocks (cond rows first, then the null-CFG rows)."""
+        x: residual stream [nb*b*n, dim] after the blocks (cond rows first, then the null-CFG rows).  temp_dev / cond_scale_dev: fp32 [b]
+        per-image values the kernels read in place of the scalars `temp` / `cond_scale`."""
         tr = self.transformer
         P = tr._packed()
         b, n = ids.shape
         bn = b * n
         R = b * rows_b
         e = tail["e"]
-        ops.final_embed(x[:bn], x[bn:2 * bn] if nb == 2 else None, P["gf"], pos, e, b, n, rows_b, cond_scale)
-        kw = dict(u=u, seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, only_masked_id=only_masked_id, aten=aten)
+        ops.final_embed(x[:bn], x[bn:2 * bn] if nb == 2 else None, P["gf"], pos, e, b, n, rows_b, cond_scale, cond_scale_dev=cond_scale_dev)
+        kw = dict(u=u, seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, only_masked_id=only_masked_id, aten=aten,
+                  temperature_dev=temp_dev)
         if "fused_ws" in tail:      # logits never reach HBM: candidate lists out of the GEMM epilogue, sampled by the finishing kernel
             ops.logits_fused(e[:R], P["wlog"], pos, ids, scores, rows_b, k_keep, temp, tail["fused_ws"], tail["status"],
                              rows_capacity=b * tail["rows_max"], **kw)
@@ -938,14 +1009,17 @@ class MaskGit(nn.Module):
         ops.linear(e[:R], P["wlog"], lg)
         ops.logits_sample(lg, pos, ids, scores, rows_b, k_keep, temp, **kw)
 
-    def _generate_body(self, req, text_embeds, cond_images, region, aten):
-        """The device-side work of a request: no host synchronisation, no data-dependent host control flow.  region: the device tensors
-        of req.region (or a captured graph's static copies of them)."""
+    def _generate_body(self, req, text_embeds, cond_images, region, settings, aten):
+        """The device-side work of a request: no host synchronisation, no data-dependent host control flow.  region, settings: the device
+        tensors of req.region and req.settings() (or a captured graph's static copies of them)."""
         tr = self.transformer
         device = text_embeds.device
         b, n, V, timesteps = len(req.texts), req.fmap_size ** 2, tr.num_tokens, req.timesteps
         cond_ids = self.cond_vae.encode_ids(cond_images) if cond_images is not None else None
-        nb = 1 if req.cond_scale == 1 else 2
+        nb = req.branches
+        # the kernels read the settings from the device tables; the scalar argument fields carry image 0's values, which are what a call
+        # with one setting for every image passes (so its launch records are those of a scalar call)
+        lead = lambda v: v[0] if v else 0.
         ctx = tr._prepare_context(text_embeds, cond_ids, [False, True][:nb])
         P = tr._packed()
         adt = P["adt"]
@@ -993,13 +1067,15 @@ class MaskGit(nn.Module):
                 if step:
                     torch.cuda.nvtx.range_pop()
                 torch.cuda.nvtx.range_push(f"mmg.decode_step[{step}] masked={num_masked}")
-            temp = req.temperature * (steps_until_x0 / timesteps)              # annealed, muse_maskgit_pytorch.py:578
+            temp = lead(req.temperature) * (steps_until_x0 / timesteps)        # annealed, muse_maskgit_pytorch.py:578
+            temp_dev = settings["temps"][s]
             u = self._injected_noise(step, (b, n, V), device)
             if native is not None:
                 a = native["args"]
                 a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.masked_pos = masked_pos.data_ptr()
                 a.num_masked = num_masked; a.k_keep = k_keep; a.step = step
-                a.temperature = float(temp); a.cond_scale = float(req.cond_scale)
+                a.temperature = float(temp); a.cond_scale = float(lead(req.cond_scale))
+                a.temperature_dev = temp_dev.data_ptr(); a.cond_scale_dev = settings["cond_scale"].data_ptr()
                 a.u = None if u is None else u.data_ptr(); a.seed = 0; a.seed_dev = self._seed_dev.data_ptr(); a.row_offset = self.row_offset * n
                 _lib.call("mmg_decode_step", a)
                 continue
@@ -1012,13 +1088,15 @@ class MaskGit(nn.Module):
                 ops.layernorm(x[:bn], P["gf"], sc_embed)
             # rows that are sampled: the masked ones; every position when already-decoded tokens may be re-masked by confidence
             pos, rows_b = (all_pos, n) if score_all else (masked_pos, num_masked)
-            self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(req.cond_scale), k_keep, tail, seed_dev=seed_dev,
-                              only_masked_id=self.mask_id if score_all or req.region is not None else None, aten=aten_draw(step))
+            self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(lead(req.cond_scale)), k_keep, tail, seed_dev=seed_dev,
+                              only_masked_id=self.mask_id if score_all or req.region is not None else None, aten=aten_draw(step),
+                              temp_dev=temp_dev, cond_scale_dev=settings["cond_scale"])
             if req.use_critic:
                 xc = cnet._run_blocks(ids, cctx, cnb)
-                ops.critic_score(xc[:bn], xc[bn:2 * bn] if cnb == 2 else None, gcrit, whead, float(bhead), float(req.cond_scale),
-                                 float(req.critic_noise_scale * (steps_until_x0 / timesteps)), scores, u=self._injected_noise(step, (b, n), device),
-                                 seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, aten=aten_draw(step, critic=True))
+                ops.critic_score(xc[:bn], xc[bn:2 * bn] if cnb == 2 else None, gcrit, whead, float(bhead), float(lead(req.cond_scale)),
+                                 float(lead(req.critic_noise_scale) * (steps_until_x0 / timesteps)), scores, u=self._injected_noise(step, (b, n), device),
+                                 seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, aten=aten_draw(step, critic=True),
+                                 cond_scale_dev=settings["crit_cond_scale"], noise_mul_dev=settings["crit_noise"][s])
         ids = ids.view(b, req.fmap_size, req.fmap_size)
         if nvtx:
             torch.cuda.nvtx.range_pop()
@@ -1171,6 +1249,7 @@ class Muse(nn.Module):
     @torch.no_grad()
     def forward(self, texts: List[str], cond_scale=3., temperature=1., timesteps=18, superres_timesteps=None,
                 return_lowres=False, return_pil_images=True):
+        """cond_scale / temperature: a number or per image (see MaskGit.generate), used by both stages."""
         lowres = self.base_maskgit.generate(texts=texts, cond_scale=cond_scale, temperature=temperature, timesteps=timesteps)
         superres = self.superres_maskgit.generate(texts=texts, cond_scale=cond_scale, cond_images=lowres, temperature=temperature,
                                                   timesteps=superres_timesteps if superres_timesteps is not None else timesteps)

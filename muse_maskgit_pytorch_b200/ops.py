@@ -293,22 +293,33 @@ def edit_select(ids, scores, frozen_out, keep, num_select, mask_id, iteration, u
     L.call("mmg_edit_select", a)
 
 
-def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_scale):
+def _per_row_table(t, rows, name):
+    """A per-image (or per-row) fp32 device table of `rows` entries, or None."""
+    if t is not None:
+        _chk(t, name)
+        assert t.dtype == torch.float32 and t.numel() == rows, f"{name}: fp32 [{rows}]"
+    return L.ptr(t)
+
+
+def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_scale, cond_scale_dev=None):
+    """cond_scale_dev: fp32 [B] per-image scales (read on the device in place of cond_scale); an image at exactly 1 takes LN(x_cond)."""
     a = L.FinalEmbedArgs()
     a.x_cond = x_cond.data_ptr(); a.x_null = L.ptr(x_null); a.gamma = gamma.data_ptr(); a.masked_pos = masked_pos.data_ptr()
     a.e = e.data_ptr(); a.e_dtype = L.dt(e); a.B = B; a.n = n; a.num_masked = num_masked; a.dim = gamma.shape[0]
-    a.cond_scale = cond_scale
+    a.cond_scale = cond_scale; a.cond_scale_dev = _per_row_table(cond_scale_dev, B, "cond_scale_dev")
     L.call("mmg_final_embed", a)
     return e
 
 
 def logits_sample(logits, masked_pos, ids, scores, num_masked, k, temperature, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
-                  only_masked_id=None, aten=None):
-    """aten = (offset, offset_dev, stride): draw the noise from ATen's CUDA uniform_ stream instead of libmmg's keying."""
+                  only_masked_id=None, aten=None, temperature_dev=None):
+    """aten = (offset, offset_dev, stride): draw the noise from ATen's CUDA uniform_ stream instead of libmmg's keying.
+    temperature_dev: fp32 [B] per-image temperatures, read on the device in place of `temperature`."""
     a = L.LogitsSampleArgs()
     a.logits = _chk(logits).data_ptr(); a.masked_pos = masked_pos.data_ptr(); a.ids = ids.data_ptr(); a.scores = scores.data_ptr()
     a.u = L.ptr(u)
     a.B, a.n = ids.shape; a.num_masked = num_masked; a.V = logits.shape[-1]; a.k = k; a.temperature = temperature
+    a.temperature_dev = _per_row_table(temperature_dev, a.B, "temperature_dev")
     a.seed = seed; a.step = step; a.row_offset = row_offset; a.seed_dev = L.ptr(seed_dev)
     if only_masked_id is not None:
         a.only_masked = 1; a.mask_id = only_masked_id
@@ -323,8 +334,9 @@ def logits_fused_workspace_bytes(rows_capacity, V, K, k):
 
 
 def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, workspace, status, rows_capacity=0, u=None, seed=0, step=0,
-                 row_offset=0, seed_dev=None, only_masked_id=None, aten=None):
-    """to_logits + top-k / gumbel argmax / confidence on the rows listed in masked_pos without a [rows, V] logits buffer."""
+                 row_offset=0, seed_dev=None, only_masked_id=None, aten=None, temperature_dev=None):
+    """to_logits + top-k / gumbel argmax / confidence on the rows listed in masked_pos without a [rows, V] logits buffer.
+    temperature_dev: as for logits_sample."""
     a = L.LogitsFusedArgs()
     a.e = _chk(e).data_ptr(); a.w = _chk(w).data_ptr(); a.K = e.shape[1]; a.rows_capacity = rows_capacity
     assert e.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and w.shape[1] == e.shape[1]
@@ -332,6 +344,7 @@ def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, work
     s = a.s
     s.masked_pos = masked_pos.data_ptr(); s.ids = ids.data_ptr(); s.scores = scores.data_ptr(); s.u = L.ptr(u)
     s.B, s.n = ids.shape; s.num_masked = num_masked; s.V = w.shape[0]; s.k = k; s.temperature = temperature
+    s.temperature_dev = _per_row_table(temperature_dev, s.B, "temperature_dev")
     s.seed = seed; s.step = step; s.row_offset = row_offset; s.seed_dev = L.ptr(seed_dev)
     if only_masked_id is not None:
         s.only_masked = 1; s.mask_id = only_masked_id
@@ -372,11 +385,14 @@ def logits_xent_rows(logits, labels, nll):
 
 
 def critic_score(x_cond, x_null, gamma, w, bias, cond_scale, noise_mul, scores, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
-                 aten=None):
-    """scores[r] = CFG(dot(LN(x[r]) * gamma, w) + bias) + (u[r] - 0.5) * noise_mul   (ref: muse_maskgit_pytorch.py:590-600)"""
+                 aten=None, cond_scale_dev=None, noise_mul_dev=None):
+    """scores[r] = CFG(dot(LN(x[r]) * gamma, w) + bias) + (u[r] - 0.5) * noise_mul   (ref: muse_maskgit_pytorch.py:590-600)
+    cond_scale_dev / noise_mul_dev: fp32 [rows] per-row values read on the device in place of the scalars."""
     a = L.CriticScoreArgs()
     a.x_cond = _chk(x_cond).data_ptr(); a.x_null = L.ptr(x_null); a.gamma = gamma.data_ptr(); a.w = _chk(w).data_ptr()
     a.bias = bias; a.cond_scale = cond_scale; a.noise_mul = noise_mul; a.dim = x_cond.shape[-1]
+    a.cond_scale_dev = _per_row_table(cond_scale_dev, scores.numel(), "cond_scale_dev")
+    a.noise_mul_dev = _per_row_table(noise_mul_dev, scores.numel(), "noise_mul_dev")
     a.u = L.ptr(u); a.scores = scores.data_ptr(); a.rows = scores.numel(); a.row_offset = row_offset
     a.seed = seed; a.seed_dev = L.ptr(seed_dev); a.step = step
     assert x_cond.dtype == torch.float32 and w.dtype == torch.float32 and x_cond.shape[0] >= a.rows

@@ -2,8 +2,12 @@
 of generate(), so rank r generates a contiguous slice of the batch with replicated weights and the decoded images are
 assembled with ONE all-gather at the end.  No collective runs inside the decode loop.  The sampler's Philox counters are
 keyed on the global sequence index (MaskGit.row_offset), so token ids do not depend on the number of ranks."""
+import numbers
+
 import torch
 import torch.distributed as dist
+
+PER_IMAGE_SETTINGS = ("temperature", "cond_scale", "critic_noise_scale")
 
 
 def shard_bounds(total, rank, world):
@@ -50,6 +54,13 @@ def generate_sharded(maskgit, texts, text_embeds=None, cond_images=None, group=N
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     total = len(texts)
     lo, hi = shard_bounds(total, rank, world)
+    for name in PER_IMAGE_SETTINGS:       # per-image settings (a sequence or 1-D tensor of `total` values) are sliced like text_embeds
+        value = generate_kwargs.get(name)
+        if value is None or isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
+            continue
+        if len(value) != total:
+            raise ValueError(f"{name} has {len(value)} values for {total} texts")
+        generate_kwargs[name] = value[lo:hi]
     tr = maskgit.transformer
     saved = (tr.encode_text, maskgit.row_offset, maskgit.global_batch, maskgit.sampler_seed)
     try:
