@@ -223,7 +223,12 @@ int mmg_embed(const mmg_embed_args* a, void* stream);
  * Attention core: out[b, t, h*64:(h+1)*64] = softmax(scale * q.k^T + key_mask) v   with dh = 64.
  * q [BH, Tq, 64], k/v [BH, Tk_alloc, 64] already l2-normalised/scaled (epilogue MMG_EPI_QKV); key 0 is the null key.
  * replaces: Attend.forward / flash_attn (attend.py:66-140) + the head split/merge in Attention.forward
- * (muse_maskgit_pytorch.py:143-161).  key_mask: [B, Tk] uint8 (1 = attend) or NULL; masked logits = -FLT_MAX.     */
+ * (muse_maskgit_pytorch.py:143-161).  key_mask: [B, Tk - 1] uint8 (1 = attend) or NULL: one byte per REAL key, row b at
+ * key_mask + b * (Tk - 1); the null key has no byte and is always attended.  Masked logits = -FLT_MAX.
+ * Precondition: the tensor-core kernels (MMG_BF16 with aligned operands, and split3) multiply zero weights by the k/v rows between Tk
+ * and the end of the last 32-key chunk.  Rows [Tk, Tk_alloc) of k and v must therefore hold finite values (zeros, or stale finite
+ * data): a NaN or Inf there reaches the output.  Where the padding is shorter than the chunk the rows read are the next head's, and
+ * reads past the end of the tensor give zeros.  The CUDA-core kernels never read past row Tk.                        */
 typedef struct {
   const void* q; const void* k; const void* v; void* out;
   const uint8_t* key_mask;
