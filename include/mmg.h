@@ -60,12 +60,14 @@ enum mmg_epilogue {
   MMG_EPI_RESIDUAL   = 1, /* out[r, c] = acc (+bias[c]) + resid[r, c]; out/resid dtype = out_dtype (may alias)      */
   MMG_EPI_GEGLU      = 2, /* W rows interleaved in blocks of 32: [x(32) | gate(32)]; out[r, c/2] = gate*gelu_erf(x) */
   MMG_EPI_GLU        = 3, /* same interleave, with bias: out = (a+ba) * sigmoid(g+bg)         (nn.GLU, vqgan_vae.py:256) */
-  MMG_EPI_QKV        = 4, /* N = (nq+nk+nv)*64 head-columns: l2norm(q)*q_scale, l2norm(k)*k_scale, v -> per-head layouts */
+  MMG_EPI_QKV        = 4, /* N = (nq+nk+nv)*64 head-columns: l2norm(q)*q_scale, l2norm(k)*k_scale, v -> per-head layouts;
+                             q_out / k_out / v_out / null_k / null_v 16-byte aligned (else MMG_EINVAL)                       */
   MMG_EPI_CONVT      = 5, /* conv-transpose parity scatter: out pixel (2y+py, 2x+px) = leaky(acc + bias)             */
   MMG_EPI_CONVT_RGB  = 6, /* CONVT followed by the fused final 1x1 conv (C -> channels<=4), fp32 NCHW output          */
   MMG_EPI_LNFOLD_RESIDUAL = 7, /* LayerNorm folded through the product: with W' = W*gamma, cvec[c] = sum_k W'[c,k] (passed as
                                   `bias`) and per-row (sum, sumsq) of the un-normalised A row in `row_stats`:
-                                  out[r,c] = resid[r,c] + rstd_r * (acc - mean_r * cvec[c])   == resid + LN(a_r) W^T           */
+                                  out[r,c] = resid[r,c] + rstd_r * (acc - mean_r * cvec[c])   == resid + LN(a_r) W^T;
+                                  out and resid 16-byte aligned (else MMG_EINVAL)                                                */
   MMG_EPI_LFQ_IDS    = 8, /* LFQ lookup fused into the projection: W rows = [hi(bits) | mid(bits) | lo(bits)] (a 3-way bf16 split
                              of the fp32 project_in weight, 3*bits <= 64 = N), bias = project_in bias [bits], ln_width = bits:
                              ids[r] = sum_i ((hi+mid+lo)_i + bias_i > 0) << (bits-1-i), written as int64 to out[r]                */
@@ -76,7 +78,7 @@ enum mmg_epilogue {
 };
 
 typedef struct {
-  void*        out;        /* see enum; [M, ldo]                                                                 */
+  void*        out;        /* see enum; [M, ldo]; any element offset (an unaligned out / resid is written element by element) */
   int64_t      ldo;        /* leading dimension of out (elements)                                                */
   int32_t      out_dtype;  /* MMG_F32 / MMG_BF16                                                                 */
   int32_t      act;        /* 0 none, 1 leaky_relu(0.1), 2 relu (STORE of mmg_linear only)                       */
@@ -106,7 +108,9 @@ typedef struct {
   const void* a;           /* [M, lda] operand dtype                                                             */
   const void* w;           /* [N, ldw] operand dtype (nn.Linear weight layout, K contiguous)                     */
   int64_t M, N, K, lda, ldw;
-  int32_t dtype;           /* MMG_BF16: wgmma path (K % 64 == 0, N % 64 == 0, 16B-aligned rows); MMG_F32: CUDA cores */
+  int32_t dtype;           /* MMG_BF16: wgmma path when K % 64 == 0, N % 64 == 0, lda % 8 == 0, ldw % 8 == 0, a and w 16-byte aligned
+                              and epi.ldo % 8 == 0 (not required for QKV, CONVT_RGB, LFQ_IDS, ARGMIN); any other bf16 call runs on the
+                              CUDA-core kernel and counts in mmg_simt_fallback_count.  MMG_F32: CUDA cores                         */
   int32_t epilogue;        /* enum mmg_epilogue                                                                   */
   mmg_epilogue_args epi;
 } mmg_linear_args;
@@ -143,7 +147,11 @@ typedef struct {
 int mmg_conv2d(const mmg_conv2d_args* a, void* stream);
 
 /* ConvTranspose2d(k=4, s=2, p=1) as 4 parity-class GEMMs (K = 4*Cin each).  w: [4 parities][Cout, 4*Cin].
- * replaces: nn.ConvTranspose2d + LeakyReLU at vqgan_vae.py:225 (and, with CONVT_RGB, the 1x1 at vqgan_vae.py:232). */
+ * replaces: nn.ConvTranspose2d + LeakyReLU at vqgan_vae.py:225 (and, with CONVT_RGB, the 1x1 at vqgan_vae.py:232).
+ * CONVT_RGB runs on the bf16 tensor-core kernel only: dtype MMG_BF16, Cout in {64, 128, 256}, Cin % 64 == 0, 16-byte aligned x and w, and
+ * an (H, W) that the conv tile geometry takes (TW = min(W, 128) divides 128 and W; TH = min(128 / TW, H) divides H; TW * TH divides
+ * 128).  Any other CONVT_RGB
+ * call returns MMG_EINVAL and launches nothing.  mmg_conv2d and this call return MMG_EINVAL for B, H, W, Cin or Cout <= 0.           */
 typedef struct {
   const void* x;           /* [B, H, W, Cin]                                                                     */
   const void* w;           /* [4, Cout, 4*Cin]                                                                   */

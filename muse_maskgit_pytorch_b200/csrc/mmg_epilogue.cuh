@@ -13,9 +13,12 @@ struct Epilogue {
   float rgb_acc[4];
   float st_a, st_b;         // LNFOLD: (mean, rstd) of the row
   int r_b, r_t;             // QKV: (batch, token) of the row; CONVT*: (batch, y * W + x)
+  // the 16-byte vector accesses (Vec64, store32_bf16, float4) need a 16-byte aligned address: a row stride that is a multiple of 8 elements
+  // keeps every 64-column chunk as aligned as the base pointer, which the caller may give at any element offset
+  static __device__ __forceinline__ bool al16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
   template <typename T>
   static __device__ __forceinline__ void store_n(T* dst, const float (&v)[64], int n, bool vec_ok) {
-    if (vec_ok && n == 64) {
+    if (vec_ok && n == 64 && al16(dst)) {
       Vec64<T>::store(dst, v);
     } else {
 #pragma unroll
@@ -171,7 +174,7 @@ struct Epilogue {
         }
         const bool vec_ok = (nvalid == 64) && ((p.ldo & 7) == 0);
         if (kind == MMG_EPI_RESIDUAL) {
-          const bool rvec = vec_ok && ((p.ldr & 7) == 0);
+          const bool rvec = vec_ok && ((p.ldr & 7) == 0) && al16(p.resid);
           if (bf) {
             const bf16* r = reinterpret_cast<const bf16*>(p.resid) + row * p.ldr + col0;
             if (rvec) { float t[64]; Vec64<bf16>::load(r, t);
@@ -216,14 +219,14 @@ struct Epilogue {
         const int oc = col0 >> 1;
         if (bf) {
           bf16* d = reinterpret_cast<bf16*>(p.out) + row * p.ldo + oc;
-          if ((p.ldo & 7) == 0) store32_bf16(d, o);
+          if ((p.ldo & 7) == 0 && al16(d)) store32_bf16(d, o);
           else {
 #pragma unroll
             for (int i = 0; i < 32; ++i) d[i] = from_f<bf16>(o[i]);
           }
         } else {
           float* d = reinterpret_cast<float*>(p.out) + row * p.ldo + oc;
-          if ((p.ldo & 3) == 0) {
+          if ((p.ldo & 3) == 0 && al16(d)) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) reinterpret_cast<float4*>(d)[i] = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
           } else {
@@ -247,7 +250,7 @@ struct Epilogue {
       case MMG_EPI_CONVT:
       case MMG_EPI_CONVT_RGB: {
 #pragma unroll
-        for (int i = 0; i < 64; ++i) v[i] = leaky01(v[i] + (p.bias ? __ldg(p.bias + col0 + i) : 0.f));
+        for (int i = 0; i < 64; ++i) v[i] = leaky01(v[i] + (p.bias && i < nvalid ? __ldg(p.bias + col0 + i) : 0.f));
         if (kind == MMG_EPI_CONVT) {
           const int64_t b = r_b; const int rem = r_t; const int y = rem / p.W, x = rem - y * p.W;
           const int64_t opix = (b * 2 * p.H + 2 * y + p.py) * (int64_t)(2 * p.W) + 2 * x + p.px;
@@ -291,7 +294,7 @@ struct Epilogue {
 #pragma unroll
         for (int i = 0; i < 32; ++i) o[i] = v[32 + i] * gelu_tanh(v[i], true);
         bf16* d = reinterpret_cast<bf16*>(p.out) + row * p.ldo + oc;
-        if ((p.ldo & 7) == 0) store32_bf16(d, o);
+        if ((p.ldo & 7) == 0 && al16(d)) store32_bf16(d, o);
         else {
 #pragma unroll
           for (int i = 0; i < 32; ++i) d[i] = from_f<bf16>(o[i]);
@@ -300,7 +303,7 @@ struct Epilogue {
 #pragma unroll
         for (int i = 0; i < 32; ++i) o[i] = v[32 + i] * gelu_tanh(v[i], false);
         float* d = reinterpret_cast<float*>(p.out) + row * p.ldo + oc;
-        if ((p.ldo & 3) == 0) {
+        if ((p.ldo & 3) == 0 && al16(d)) {
 #pragma unroll
           for (int i = 0; i < 8; ++i) reinterpret_cast<float4*>(d)[i] = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
         } else {
@@ -321,7 +324,7 @@ struct Epilogue {
   // ---- residual epilogues with the residual chunk prefetched by the caller (tensor-core kernel) -------------------------
   __device__ __forceinline__ bool can_prefetch_resid() const {
     if (kind == MMG_EPI_LNFOLD_RESIDUAL) return true;
-    return kind == MMG_EPI_RESIDUAL && p.out_dtype == MMG_F32 && (p.ldo & 7) == 0 && (p.ldr & 7) == 0 && p.act == 0;
+    return kind == MMG_EPI_RESIDUAL && p.out_dtype == MMG_F32 && (p.ldo & 7) == 0 && (p.ldr & 7) == 0 && p.act == 0 && al16(p.out) && al16(p.resid);
   }
   __device__ __forceinline__ void load_resid(int64_t row, int col0, float (&r)[64]) const {
     Vec64<float>::load(reinterpret_cast<const float*>(p.resid) + row * p.ldr + col0, r);
@@ -364,6 +367,7 @@ struct Epilogue {
 };
 
 // host-side validation shared by the launchers
+inline bool aligned16_host(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 inline int validate_epilogue(int kind, const mmg_epilogue_args& e, int64_t N) {
   switch (kind) {
     case MMG_EPI_STORE: MMG_CHECK_ARG(e.out && e.act >= 0 && e.act <= 2, "epilogue STORE: out is NULL or act not in {0, 1, 2}"); break;
@@ -374,6 +378,7 @@ inline int validate_epilogue(int kind, const mmg_epilogue_args& e, int64_t N) {
     case MMG_EPI_LNFOLD_RESIDUAL:
       MMG_CHECK_ARG(e.out && e.resid && e.bias && e.row_stats && e.ln_width > 0 && e.stats_slots >= 1, "epilogue LNFOLD_RESIDUAL: out/resid/cvec/row_stats/ln_width/stats_slots");
       MMG_CHECK_ARG(e.out_dtype == MMG_F32 && (N % 64) == 0 && (e.ldo % 4) == 0 && (e.ldr % 4) == 0, "epilogue LNFOLD_RESIDUAL: fp32 out, N %% 64, ld %% 4");
+      MMG_CHECK_ARG(aligned16_host(e.out) && aligned16_host(e.resid), "epilogue LNFOLD_RESIDUAL: out and resid must be 16-byte aligned");
       break;
     case MMG_EPI_GEGLU: case MMG_EPI_GLU:
       MMG_CHECK_ARG(e.out && (N % 64) == 0, "epilogue GEGLU/GLU: N %% 64 != 0 or out NULL");
@@ -383,6 +388,8 @@ inline int validate_epilogue(int kind, const mmg_epilogue_args& e, int64_t N) {
       MMG_CHECK_ARG((N % 64) == 0 && N / 64 == e.nq_heads + e.nk_heads + e.nv_heads, "epilogue QKV: N != 64*(nq+nk+nv)");
       MMG_CHECK_ARG(e.tokens > 0 && e.heads > 0, "epilogue QKV: tokens/heads");
       MMG_CHECK_ARG((!e.nq_heads || (e.q_out && e.q_scale)) && (!e.nk_heads || (e.k_out && e.k_scale)) && (!e.nv_heads || e.v_out), "epilogue QKV: NULL output");
+      MMG_CHECK_ARG(aligned16_host(e.q_out) && aligned16_host(e.k_out) && aligned16_host(e.v_out) && aligned16_host(e.null_k) && aligned16_host(e.null_v),
+                    "epilogue QKV: q / k / v outputs and null rows must be 16-byte aligned");
       break;
     case MMG_EPI_CONVT: MMG_CHECK_ARG(e.out && e.H > 0 && e.W > 0, "epilogue CONVT: geometry"); break;
     case MMG_EPI_CONVT_RGB: MMG_CHECK_ARG(e.out && e.rgb_w && e.rgb_b && e.rgb_channels >= 1 && e.rgb_channels <= 4, "epilogue CONVT_RGB: args"); break;

@@ -300,6 +300,7 @@ extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->x && a->w, "mmg_conv2d: NULL operand");
   MMG_CHECK_ARG(a->kind >= 0 && a->kind <= 3, "mmg_conv2d: kind %d", a->kind);
+  MMG_CHECK_ARG(a->B > 0 && a->H > 0 && a->W > 0 && a->Cin > 0 && a->Cout > 0, "mmg_conv2d: bad geometry");
   MMG_CHECK_ARG(a->kind != 2 || (a->H % 2 == 0 && a->W % 2 == 0), "mmg_conv2d: stride-2 conv needs even H, W");
   ConvGeom g; conv_geom(a->kind, a->B, a->H, a->W, a->Cin, &g);
   const int64_t M = (int64_t)a->B * g.Ho * g.Wo, N = a->Cout, K = (int64_t)g.ntaps * a->Cin;
@@ -352,6 +353,7 @@ extern "C" int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* st
   const bool tc_ok = a->dtype == MMG_BF16 && (a->Cin % 64 == 0) && (N % 64 == 0) && aligned16(a->x) && aligned16(a->w) &&
                      (a->epilogue == MMG_EPI_CONVT_RGB ? (N == 64 || N == 128 || N == 256) : (a->epi.ldo % 8 == 0)) &&
                      tile_geometry(a->H, a->W, &p) == 0;
+  MMG_CHECK_ARG(tc_ok || a->epilogue != MMG_EPI_CONVT_RGB, "mmg_conv_transpose2d: CONVT_RGB needs the bf16 tensor-core path (N in {64, 128, 256}, a tile geometry)");
   const size_t esz = a->dtype == MMG_BF16 ? 2 : 4;
   if (!tc_ok && a->dtype == MMG_BF16) note_simt_fallback("mmg_conv_transpose2d", M, N, K);
   for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {

@@ -20,6 +20,7 @@ runall() { # same but without -x
 runall kernels 900 tests/test_gpu_kernels.py
 runall row_kernels 600 tests/test_gpu_row_kernels.py
 runall attention 600 tests/test_gpu_attention.py
+runall gemm 900 tests/test_gpu_gemm.py          # about 150 s on an H100, of which about 80 s is its profiling child run (timeout 480 s)
 runall gemm_fragment_epilogue 600 tests/test_gpu_gemm_fragment_epilogue.py
 runall models 900 tests/test_gpu_models.py
 runall aten_rng 600 tests/test_gpu_aten_rng.py

@@ -51,19 +51,32 @@ def _profiler_ready():
         kernels_of(lambda: torch.ones(8, device="cuda").sum())
 
 
+CAPTURE_RETAKES = [0]              # captures taken again because they recorded fewer libmmg kernels than were launched
+
+
 def kernels_of(fn):
     """Runs fn() under torch.profiler and returns (its result, the names of the libmmg kernels it launched).  fn must give the same result
-    when called again (in-place operands are built inside it): a capture that recorded no libmmg kernel at all (the CUPTI activity records
-    of a short capture are now and then lost) is taken again, up to twice."""
+    when called again (in-place operands are built inside it).  The CUPTI activity records of a capture are now and then lost, all of them
+    or only some (a split3 product without its GEMM, three of the four conv-transpose launches): a capture that recorded fewer libmmg
+    kernels than mmg_launch_count() rose by during it is taken again, after a pause that grows with each retake, up to five times: the
+    losses come in short bursts, and three captures in a row of the same small kernel have come back empty."""
+    import time
     from torch.profiler import profile, ProfilerActivity
-    for _ in range(3):
+    from muse_maskgit_pytorch_b200 import _lib
+    for attempt in range(6):
+        if attempt:
+            time.sleep(0.05 * attempt)
         torch.cuda.synchronize()
+        launched = _lib.launch_count()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             out = fn()
             torch.cuda.synchronize()
-        names = sorted({e.key for e in prof.key_averages() if e.self_device_time_total > 0 and "mmg::" in e.key})
-        if names:
+        launched = _lib.launch_count() - launched
+        ev = [e for e in prof.key_averages() if e.self_device_time_total > 0 and "mmg::" in e.key]
+        names = sorted({e.key for e in ev})
+        if names and sum(e.count for e in ev) >= launched:
             break
+        CAPTURE_RETAKES[0] += 1
     return out, names
 
 
