@@ -34,7 +34,8 @@ extern "C" {
 /* operand dtypes */
 #define MMG_F32  0
 #define MMG_BF16 1
-#define MMG_E4M3 2   /* fp8 e4m3 (OCP E4M3FN: largest finite 448, no infinities): mmg_linear_fp8 operands, mmg_layernorm_fp8 output */
+#define MMG_E4M3 2   /* fp8 e4m3 (OCP E4M3FN: largest finite 448, no infinities): mmg_linear_fp8 / mmg_conv*_fp8 operands, mmg_layernorm_fp8 /
+                          mmg_quantize_e4m3_images output */
 
 int         mmg_version(void);
 const char* mmg_last_error(void);
@@ -160,6 +161,48 @@ typedef struct {
   mmg_epilogue_args epi;   /* out: [B, 2H, 2W, Cout] (CONVT) or fp32 [B, channels, 2H, 2W] (CONVT_RGB)           */
 } mmg_conv_transpose2d_args;
 int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* stream);
+
+/* The same convolutions with e4m3 operands (VQGanVAE precision="fp8"): one fp32 scale per IMAGE of x (mmg_quantize_e4m3_images) and one
+ * per row of w (output channel; per parity class for the conv-transpose):
+ *   acc[r, c] = sum_k qx[r, k] qw[c, k]  (fp8 tensor cores),  C[r, c] = acc[r, c] * x_scale[image of output row r] * w_scale[c]
+ * then the register epilogue exactly as the bf16 call's: STORE (+ bias, LeakyReLU act = 1), RESIDUAL (bf16 resid), GLU (mmg_conv2d_fp8);
+ * CONVT, CONVT_RGB (mmg_conv_transpose2d_fp8).  One k-block is one tap x 128 channels.  Requires Cin % 128 == 0, Cout % 64 == 0, x and w
+ * 16-byte aligned, w_scale 8-byte aligned, an output (conv) / input (conv-transpose) grid the conv tile geometry takes, kind 0, 1 or 2,
+ * epi.ldo % 8 == 0 (CONVT_RGB: Cout in {64, 128, 256}).  Any other call returns MMG_EINVAL and launches nothing: there is no fallback. */
+typedef struct {
+  const void*  x;          /* [B, H, W, Cin] e4m3                                                                */
+  const void*  w;          /* [Cout, taps*Cin] e4m3                                                              */
+  const float* x_scale;    /* [B]                                                                                */
+  const float* w_scale;    /* [Cout]                                                                             */
+  int32_t B, H, W, Cin, Cout, kind;
+  int32_t dtype, epilogue; /* MMG_E4M3; STORE / RESIDUAL / GLU                                                   */
+  mmg_epilogue_args epi;
+} mmg_conv2d_fp8_args;
+int mmg_conv2d_fp8(const mmg_conv2d_fp8_args* a, void* stream);
+
+typedef struct {
+  const void*  x;          /* [B, H, W, Cin] e4m3                                                                */
+  const void*  w;          /* [4, Cout, 4*Cin] e4m3                                                              */
+  const float* x_scale;    /* [B]                                                                                */
+  const float* w_scale;    /* [4, Cout]                                                                          */
+  int32_t B, H, W, Cin, Cout;
+  int32_t dtype, epilogue; /* MMG_E4M3; CONVT or CONVT_RGB                                                       */
+  mmg_epilogue_args epi;
+} mmg_conv_transpose2d_fp8_args;
+int mmg_conv_transpose2d_fp8(const mmg_conv_transpose2d_fp8_args* a, void* stream);
+
+/* Per-image e4m3 quantisation of a bf16 NHWC map x [B * hw, C] (contiguous) for the calls above:
+ *   amax_b = max |x| over image b (an integer max over the bits of |x|: order-independent, bitwise reproducible);
+ *   inv = amax_b == 0 ? 0 : 448 / amax_b (IEEE division);  q = cvt.rn.satfinite.e4m3(x * inv);  scale[b] = amax_b / 448
+ * An all-zero image gets scale 0 and zero bytes.  C % 8 == 0, x and q 16-byte aligned, B < 65536.                 */
+typedef struct {
+  const void* x;           /* [B * hw, C] bf16                                                                   */
+  void*       q;           /* [B * hw, C] e4m3                                                                   */
+  float*      scale;       /* [B]                                                                                */
+  int64_t B, hw;
+  int32_t C, _pad;
+} mmg_quantize_e4m3_images_args;
+int mmg_quantize_e4m3_images(const mmg_quantize_e4m3_images_args* a, void* stream);
 
 /* First encoder conv: k x k (odd k <= 9, padding k / 2; the reference default is 5), Cin = channels (<= 4), fp32 NCHW image in, NHWC act
  * out.  replaces vqgan_vae.py:231.                                                                                  */

@@ -43,6 +43,20 @@ class ConvTranspose2dArgs(C.Structure):
                 ("dtype", i32), ("epilogue", i32), ("epi", EpilogueArgs)]
 
 
+class Conv2dFp8Args(C.Structure):
+    _fields_ = [("x", vp), ("w", vp), ("x_scale", vp), ("w_scale", vp), ("B", i32), ("H", i32), ("W", i32), ("Cin", i32), ("Cout", i32),
+                ("kind", i32), ("dtype", i32), ("epilogue", i32), ("epi", EpilogueArgs)]
+
+
+class ConvTranspose2dFp8Args(C.Structure):
+    _fields_ = [("x", vp), ("w", vp), ("x_scale", vp), ("w_scale", vp), ("B", i32), ("H", i32), ("W", i32), ("Cin", i32), ("Cout", i32),
+                ("dtype", i32), ("epilogue", i32), ("epi", EpilogueArgs)]
+
+
+class QuantizeE4m3ImagesArgs(C.Structure):
+    _fields_ = [("x", vp), ("q", vp), ("scale", vp), ("B", i64), ("hw", i64), ("C", i32), ("_pad", i32)]
+
+
 class ConvInArgs(C.Structure):
     _fields_ = [("img", vp), ("w", vp), ("bias", vp), ("out", vp), ("B", i32), ("C", i32), ("H", i32), ("W", i32),
                 ("Cout", i32), ("out_dtype", i32), ("ksize", i32), ("_pad", i32)]
@@ -187,6 +201,7 @@ EXPORTS = {
     "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs, "mmg_edit_select": EditSelectArgs,
     "mmg_logits_xent": LogitsXentArgs, "mmg_logits_xent_rows": LogitsXentRowsArgs,
     "mmg_linear_fp8": LinearFp8Args, "mmg_layernorm_fp8": LayerNormFp8Args,
+    "mmg_conv2d_fp8": Conv2dFp8Args, "mmg_conv_transpose2d_fp8": ConvTranspose2dFp8Args, "mmg_quantize_e4m3_images": QuantizeE4m3ImagesArgs,
 }
 PLAIN_EXPORTS = ("mmg_version", "mmg_last_error", "mmg_launch_count", "mmg_sizeof", "mmg_decode_step_workspace_bytes", "mmg_logits_fused_workspace_bytes",
                  "mmg_logits_xent_workspace_bytes", "mmg_simt_fallback_count", "mmg_simt_launch_count")

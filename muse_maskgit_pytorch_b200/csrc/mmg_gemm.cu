@@ -341,6 +341,112 @@ extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
   return dispatch_tc(p, bn, a->w, N, K, K, st);
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// e4m3 convolutions: the conv mode of tc_gemm_kernel<BN, TC_EPI_REGS, fp8e4> at the tile geometry, tile width and tile order the bf16
+// convolution of the same shape takes.  A k-block is one tap x 128 channels (Cin % 128 == 0); the register epilogue first dequantises
+// with x_scale[image] * w_scale[col].  Shapes the kernel does not take are argument errors: there is no other e4m3 convolution kernel.
+// ------------------------------------------------------------------------------------------------------------------
+static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+
+static int launch_conv_fp8(TcGemmParams& p, const void* w, int64_t N, int64_t K, cudaStream_t st) {
+  int bn = pick_bn(p.num_m_tiles, N, p.epi.kind);
+  if (bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;        // dispatch_tc's register-epilogue width
+  p.num_n_tiles = (int)((N + bn - 1) / bn);
+  p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;   // the bf16 product's tile order
+  uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)K}; uint32_t box[2] = {128, (uint32_t)bn};
+  int rc = make_tmap_u8(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
+  switch (bn) {
+    case 64: return launch_tc<64, TC_EPI_REGS, fp8e4>(p, st);
+    case 128: return launch_tc<128, TC_EPI_REGS, fp8e4>(p, st);
+    case 256: return launch_tc<256, TC_EPI_REGS, fp8e4>(p, st);      // CONVT_RGB: the whole 256-column row in one tile
+  }
+  return fail(MMG_EINVAL, "e4m3 convolution: unsupported tile width %d", bn);
+}
+
+// the A tensor map(s) of an e4m3 NHWC map: one 4-D map (stride 1), or one per input parity over the (H/2, W/2) grid (stride 2)
+static int fp8_image_maps(TcGemmParams& p, const void* x, int B, int H, int W, int Cin, bool stride2) {
+  const uint64_t C = Cin, Wd = W, Hd = H;
+  uint32_t box[4] = {128, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TB};
+  if (!stride2) {
+    uint64_t dims[4] = {C, Wd, Hd, (uint64_t)B}; uint64_t str[3] = {C, Wd * C, Hd * Wd * C};
+    return make_tmap_u8(&p.tma_a[0], x, 4, dims, str, box);
+  }
+  for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
+    const uint8_t* base = reinterpret_cast<const uint8_t*>(x) + ((uint64_t)py * Wd + px) * C;
+    uint64_t dims[4] = {C, Wd / 2, Hd / 2, (uint64_t)B}; uint64_t str[3] = {2 * C, 2 * Wd * C, Hd * Wd * C};
+    const int rc = make_tmap_u8(&p.tma_a[py * 2 + px], base, 4, dims, str, box); if (rc) return rc;
+  }
+  return MMG_OK;
+}
+
+extern "C" int mmg_conv2d_fp8(const mmg_conv2d_fp8_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->x && a->w && a->x_scale && a->w_scale, "mmg_conv2d_fp8: NULL operand or scale");
+  MMG_CHECK_ARG(a->dtype == MMG_E4M3, "mmg_conv2d_fp8: dtype %d is not MMG_E4M3", a->dtype);
+  MMG_CHECK_ARG(a->kind >= 0 && a->kind <= 2, "mmg_conv2d_fp8: kind %d (1x1, 3x3 or 4x4 stride 2 only)", a->kind);
+  MMG_CHECK_ARG(a->B > 0 && a->H > 0 && a->W > 0 && a->Cin > 0 && a->Cout > 0, "mmg_conv2d_fp8: bad geometry");
+  MMG_CHECK_ARG(a->kind != 2 || (a->H % 2 == 0 && a->W % 2 == 0), "mmg_conv2d_fp8: stride-2 conv needs even H, W");
+  MMG_CHECK_ARG(a->Cin % 128 == 0 && a->Cout % 64 == 0, "mmg_conv2d_fp8: Cin %% 128 == 0 and Cout %% 64 == 0 (Cin=%d Cout=%d)", a->Cin, a->Cout);
+  MMG_CHECK_ARG(aligned16(a->x) && aligned16(a->w) && aligned8(a->w_scale) && a->epi.ldo % 8 == 0,
+                "mmg_conv2d_fp8: x and w need 16-byte alignment, w_scale 8-byte alignment, epi.ldo %% 8 == 0");
+  MMG_CHECK_ARG(a->epilogue == MMG_EPI_STORE || a->epilogue == MMG_EPI_RESIDUAL || a->epilogue == MMG_EPI_GLU,
+                "mmg_conv2d_fp8: epilogue %d (STORE, RESIDUAL or GLU)", a->epilogue);
+  MMG_CHECK_ARG(a->epi.act != 2, "mmg_conv2d_fp8: ReLU epilogues are offered by mmg_linear only");
+  ConvGeom g; conv_geom(a->kind, a->B, a->H, a->W, a->Cin, &g);
+  const int64_t M = (int64_t)a->B * g.Ho * g.Wo, N = a->Cout, K = (int64_t)g.ntaps * a->Cin;
+  int rc = validate_epilogue(a->epilogue, a->epi, N); if (rc) return rc;
+  TcGemmParams p{};
+  MMG_CHECK_ARG(tile_geometry(g.Ho, g.Wo, &p) == 0, "mmg_conv2d_fp8: no conv tile geometry for a %d x %d output", g.Ho, g.Wo);
+  p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 128; p.ntaps = g.ntaps; p.num_kb = p.ntaps * p.cchunks;
+  p.Ho = g.Ho; p.Wo = g.Wo; p.B = a->B;
+  p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
+  p.epi.p = a->epi; p.epi.kind = a->epilogue; p.epi.fast = 1; p.epi.M = M; p.epi.N = N;
+  p.a_scale = a->x_scale; p.w_scale = a->w_scale;
+  rc = fp8_image_maps(p, a->x, a->B, a->H, a->W, a->Cin, a->kind == 2); if (rc) return rc;
+  if (a->kind != 2) {
+    for (int t = 0; t < g.ntaps; ++t) { p.tap_map[t] = 0; p.tap_dy[t] = g.tdy[t]; p.tap_dx[t] = g.tdx[t]; }
+  } else {
+    for (int r = 0; r < 4; ++r) for (int s = 0; s < 4; ++s) {
+      const int oy = r - 1, ox = s - 1;
+      const int py = ((oy % 2) + 2) % 2, px = ((ox % 2) + 2) % 2;
+      p.tap_map[r * 4 + s] = (int8_t)(py * 2 + px); p.tap_dy[r * 4 + s] = (int8_t)((oy - py) / 2); p.tap_dx[r * 4 + s] = (int8_t)((ox - px) / 2);
+    }
+  }
+  return launch_conv_fp8(p, a->w, N, K, st);
+}
+
+extern "C" int mmg_conv_transpose2d_fp8(const mmg_conv_transpose2d_fp8_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->x && a->w && a->x_scale && a->w_scale, "mmg_conv_transpose2d_fp8: NULL operand or scale");
+  MMG_CHECK_ARG(a->dtype == MMG_E4M3, "mmg_conv_transpose2d_fp8: dtype %d is not MMG_E4M3", a->dtype);
+  MMG_CHECK_ARG(a->epilogue == MMG_EPI_CONVT || a->epilogue == MMG_EPI_CONVT_RGB, "mmg_conv_transpose2d_fp8: epilogue must be CONVT/CONVT_RGB");
+  MMG_CHECK_ARG(a->B > 0 && a->H > 0 && a->W > 0 && a->Cin > 0 && a->Cout > 0, "mmg_conv_transpose2d_fp8: bad geometry");
+  MMG_CHECK_ARG(a->Cin % 128 == 0 && a->Cout % 64 == 0, "mmg_conv_transpose2d_fp8: Cin %% 128 == 0 and Cout %% 64 == 0 (Cin=%d Cout=%d)", a->Cin, a->Cout);
+  MMG_CHECK_ARG(aligned16(a->x) && aligned16(a->w) && aligned8(a->w_scale), "mmg_conv_transpose2d_fp8: x and w need 16-byte alignment, w_scale 8-byte alignment");
+  MMG_CHECK_ARG(a->epilogue == MMG_EPI_CONVT_RGB ? (a->Cout == 64 || a->Cout == 128 || a->Cout == 256) : (a->epi.ldo % 8 == 0),
+                "mmg_conv_transpose2d_fp8: CONVT_RGB needs Cout in {64, 128, 256}, CONVT epi.ldo %% 8 == 0");
+  const int64_t M = (int64_t)a->B * a->H * a->W, N = a->Cout, K = 4 * (int64_t)a->Cin;
+  int rc;
+  { mmg_epilogue_args e = a->epi; e.H = a->H; e.W = a->W; rc = validate_epilogue(a->epilogue, e, N); if (rc) return rc; }
+  TcGemmParams p{};
+  MMG_CHECK_ARG(tile_geometry(a->H, a->W, &p) == 0, "mmg_conv_transpose2d_fp8: no conv tile geometry for a %d x %d input", a->H, a->W);
+  p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 128; p.ntaps = 4; p.num_kb = 4 * p.cchunks;
+  p.Ho = a->H; p.Wo = a->W; p.B = a->B;
+  p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
+  p.a_scale = a->x_scale;
+  rc = fp8_image_maps(p, a->x, a->B, a->H, a->W, a->Cin, false); if (rc) return rc;
+  for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
+    TcGemmParams q = p;
+    q.epi.p = a->epi; q.epi.kind = a->epilogue; q.epi.fast = 1; q.epi.M = M; q.epi.N = N;
+    q.epi.p.H = a->H; q.epi.p.W = a->W; q.epi.p.py = py; q.epi.p.px = px;
+    q.w_scale = a->w_scale + (size_t)(py * 2 + px) * N;
+    for (int t = 0; t < 4; ++t) { q.tap_map[t] = 0; q.tap_dy[t] = (int8_t)CT_D[py][t >> 1]; q.tap_dx[t] = (int8_t)CT_D[px][t & 1]; }
+    const uint8_t* wp = reinterpret_cast<const uint8_t*>(a->w) + (size_t)(py * 2 + px) * N * K;
+    rc = launch_conv_fp8(q, wp, N, K, st); if (rc) return rc;
+  }
+  return MMG_OK;
+}
+
 extern "C" int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->x && a->w, "mmg_conv_transpose2d: NULL operand");

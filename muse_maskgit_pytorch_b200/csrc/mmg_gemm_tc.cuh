@@ -94,8 +94,9 @@ template <int BN> struct TcCfg {
 // TC_EPI_QKV: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 16 rows are 16 consecutive tokens of one
 // sequence and land on 16 consecutive rows of one head of q / k / v): one box and one TMA store per warp and head chunk.
 // TC_EPI_GEGLU: the GEGLU epilogue (bf16 out, BN == 256): two 64-column chunks make 64 outputs = one box per warp.
-// e4m3 operands (TA = __nv_fp8_e4m3; QKV and GEGLU tile epilogues only): a k-block is 128 elements, four m64nBNk32 wgmma, and the tile
-// epilogue starts by dequantising the fragment with dequant_acc; everything after it is the bf16 code.
+// e4m3 operands (TA = __nv_fp8_e4m3; the dense QKV and GEGLU tile epilogues, and the register epilogues of the convolutions): a k-block
+// is 128 elements, four m64nBNk32 wgmma, and the epilogue starts by dequantising the fragment with dequant_acc (per-row A scales) or
+// dequant_acc_images (per-image A scales, conv mode); everything after it is the bf16 code.
 template <int BN>
 __device__ __forceinline__ void dequant_acc(float (&acc)[BN / 2], const float* __restrict__ a_scale, const float* __restrict__ w_scale,
                                             int64_t brow, int64_t M, int col0, int lane) {
@@ -110,6 +111,24 @@ __device__ __forceinline__ void dequant_acc(float (&acc)[BN / 2], const float* _
   }
 }
 
+// e4m3 convolutions (mode 1, register epilogues): A holds one scale per IMAGE (mmg_quantize_e4m3_images), which factors out of the sum
+// over taps and channels because an output pixel reads only pixels of its own image.  The warp's fragment rows r0 + l / 4 and + 8 of
+// the tile belong to image bt * TB + row / (TW * TH); rows of images past B hold zero accumulators and are never stored.
+template <int BN>
+__device__ __forceinline__ void dequant_acc_images(float (&acc)[BN / 2], const TcGemmParams& p, int m_blk, int r0, int col0, int lane) {
+  const int q = lane & 3, fr = lane >> 2;
+  const int per = p.TW * p.TH, bbase = (m_blk / (p.tiles_x * p.tiles_y)) * p.TB;
+  const int b0 = bbase + (r0 + fr) / per, b1 = bbase + (r0 + fr + 8) / per;
+  const float sa0 = b0 < p.B ? __ldg(p.a_scale + b0) : 0.f;
+  const float sa1 = b1 < p.B ? __ldg(p.a_scale + b1) : 0.f;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const float2 ws = __ldg(reinterpret_cast<const float2*>(p.w_scale + col0 + 8 * j + 2 * q));
+    acc[4 * j] *= sa0 * ws.x; acc[4 * j + 1] *= sa0 * ws.y;
+    acc[4 * j + 2] *= sa1 * ws.x; acc[4 * j + 3] *= sa1 * ws.y;
+  }
+}
+
 template <int BN, int EPI_MODE, typename TA = bf16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
@@ -117,7 +136,11 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   using Cfg = TcCfg<BN>;
   constexpr bool FP8 = sizeof(TA) == 1;
   constexpr int BK = 128 / (int)sizeof(TA);           // elements per k-block: one 128-byte row
-  static_assert(!FP8 || EPI_MODE == TC_EPI_QKV || EPI_MODE == TC_EPI_GEGLU, "e4m3 operands are dequantised by the QKV / GEGLU tile epilogues only");
+  static_assert(!FP8 || EPI_MODE == TC_EPI_QKV || EPI_MODE == TC_EPI_GEGLU || EPI_MODE == TC_EPI_REGS,
+                "e4m3 operands are dequantised by the QKV / GEGLU tile epilogues (dense) or the register epilogues (convolutions) only");
+  // e4m3 convolutions: a k-block is one tap x 128 channels.  The dense e4m3 instantiations never run mode 1 and keep the bf16 channel step.
+  constexpr bool FP8_CONV = FP8 && EPI_MODE == TC_EPI_REGS;
+  constexpr int CBK = FP8_CONV ? BK : TC_BK;
   constexpr bool RED = EPI_MODE == TC_EPI_REDUCE || EPI_MODE == TC_EPI_TSTORE, RED_ADD = EPI_MODE == TC_EPI_REDUCE;   // TSTORE: same tiles, plain TMA store
   constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
   constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
@@ -180,7 +203,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
             tma_load_2d(sa, &p.tma_a[0], full_bar + stage, kb * BK, m_blk * TC_BM);
           } else {
             const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
-            tma_load_4d(sa, &p.tma_a[p.tap_map[tap]], full_bar + stage, cc * TC_BK, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], b0);
+            tma_load_4d(sa, &p.tma_a[p.tap_map[tap]], full_bar + stage, cc * CBK, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], b0);
           }
           tma_load_2d(sb, &p.tma_b, full_bar + stage, kb * BK, n_blk * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -231,6 +254,14 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         epi.ln_row_stats(brow + (lane >> 2) + 8 * (lane & 3), ln_a, ln_b);
 
       // ---- main loop: 4 wgmma (K = 16, e4m3: 32) per k-block; a ring slot goes back to the producer once the wgmma group after it was issued ----
+      // e4m3 convolutions promote instead: the fp8 tensor core adds each k32 step into its accumulator with fewer bits than fp32, so every
+      // k-block starts a fresh accumulator, waits for its own group, and is added into the fp32 sum `tot` (one promotion per 128 elements
+      // of K, BN / 2 more registers per thread).  The dense e4m3 products (K = 512: four k-blocks) accumulate in place.
+      float tot[FP8_CONV ? BN / 2 : 1];
+      if constexpr (FP8_CONV) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+      }
       int prev_stage = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(full_bar + stage, phase);
@@ -240,18 +271,31 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          if constexpr (FP8) WgmmaE4m3<BN>::mma(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+          if constexpr (FP8_CONV) WgmmaE4m3<BN>::mma(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), k ? 1u : 0u);
+          else if constexpr (FP8) WgmmaE4m3<BN>::mma(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
           else Wgmma<BN>::template mma<0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
         }
         wgmma_commit();
-        wgmma_wait<1>();
-        if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
-        prev_stage = stage;
+        if constexpr (FP8_CONV) {
+          wgmma_wait<0>();
+          reg_fence(acc);
+          __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + stage);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) tot[i] += acc[i];
+        } else {
+          wgmma_wait<1>();
+          if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
+          prev_stage = stage;
+        }
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
       reg_fence(acc);
       if (prev_stage >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar + prev_stage); }
+      if constexpr (FP8_CONV) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = tot[i];
+      }
 
       if constexpr (TILES) {
         // ---- tile epilogues, from the accumulator fragments (layout above the kernel) ----
@@ -403,6 +447,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
         }
       } else {
         // ---- register epilogues: columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread ----
+        if constexpr (FP8_CONV) dequant_acc_images<BN>(acc, p, m_blk, wg * 64 + 16 * wq, n_blk * BN, lane);
         // the epilogue of one 64-column accumulator chunk held in v
         auto chunk = [&](const int c, float (&v)[64]) {
           const int col0 = n_blk * BN + c * 64;

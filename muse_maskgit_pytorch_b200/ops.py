@@ -173,6 +173,60 @@ def conv_transpose2d(x, w, out, B, H, W, Cin, Cout, bias=None, rgb_w=None, rgb_b
     return out
 
 
+def quantize_e4m3_images(x, B, q=None, scale=None):
+    """Per-image e4m3 quantisation of a bf16 NHWC map x [B * hw, C]: q (float8_e4m3fn, x's shape) * scale[b] ~= x on image b, with
+    scale[b] = max |x_b| / 448 and round-to-nearest-even, saturating (mmg_quantize_e4m3_images).  Returns (q, scale)."""
+    _chk(x, "x")
+    assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.shape[0] % B == 0
+    q = torch.empty(x.shape, device=x.device, dtype=torch.float8_e4m3fn) if q is None else q
+    scale = torch.empty((B,), device=x.device, dtype=torch.float32) if scale is None else scale
+    _chk(q, "q"); _chk(scale, "scale")
+    assert q.dtype == torch.float8_e4m3fn and q.shape == x.shape and scale.dtype == torch.float32 and scale.numel() == B
+    a = L.QuantizeE4m3ImagesArgs()
+    a.x = x.data_ptr(); a.q = q.data_ptr(); a.scale = scale.data_ptr(); a.B = B; a.hw = x.shape[0] // B; a.C = x.shape[1]
+    L.call("mmg_quantize_e4m3_images", a)
+    return q, scale
+
+
+def conv2d_fp8(x, x_scale, w, w_scale, out, B, H, W, Cin, Cout, kind, epilogue=EPI_STORE, bias=None, act=0, resid=None):
+    """e4m3 conv2d: x [B*H*W, Cin] float8_e4m3fn with per-image scales x_scale [B] (quantize_e4m3_images), w packed [Cout, taps*Cin]
+    float8_e4m3fn with per-output-channel scales w_scale [Cout]; the epilogue as conv2d's (bf16 / fp32 out, bf16 resid)."""
+    for t, n in ((x, "x"), (x_scale, "x_scale"), (w, "w"), (w_scale, "w_scale")):
+        _chk(t, n)
+    assert x.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn and x_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    assert x_scale.numel() >= B and w_scale.numel() >= Cout
+    a = L.Conv2dFp8Args()
+    a.x = x.data_ptr(); a.w = w.data_ptr(); a.x_scale = x_scale.data_ptr(); a.w_scale = w_scale.data_ptr()
+    a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.kind = kind
+    a.dtype = L.E4M3; a.epilogue = epilogue
+    a.epi = _epi(out, out.shape[-1], bias, act, resid, resid.shape[-1] if resid is not None else 0)
+    L.call("mmg_conv2d_fp8", a)
+    return out
+
+
+def conv_transpose2d_fp8(x, x_scale, w, w_scale, out, B, H, W, Cin, Cout, bias=None, rgb_w=None, rgb_b=None):
+    """e4m3 ConvTranspose2d(4,2,1) + LeakyReLU(0.1): w [4, Cout, 4*Cin] float8_e4m3fn, w_scale [4, Cout]; with rgb_w: the fused trailing
+    1x1 conv (fp32 weights), out fp32 [B, ch, 2H, 2W]."""
+    for t, n in ((x, "x"), (x_scale, "x_scale"), (w, "w"), (w_scale, "w_scale")):
+        _chk(t, n)
+    assert x.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn and x_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
+    assert x_scale.numel() >= B and w_scale.numel() >= 4 * Cout
+    a = L.ConvTranspose2dFp8Args()
+    a.x = x.data_ptr(); a.w = w.data_ptr(); a.x_scale = x_scale.data_ptr(); a.w_scale = w_scale.data_ptr()
+    a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.dtype = L.E4M3
+    e = L.EpilogueArgs()
+    e.out = out.data_ptr(); e.bias = L.ptr(bias)
+    if rgb_w is not None:
+        a.epilogue = EPI_CONVT_RGB
+        e.out_dtype = L.F32; e.rgb_w = rgb_w.data_ptr(); e.rgb_b = rgb_b.data_ptr(); e.rgb_channels = rgb_w.shape[0]
+    else:
+        a.epilogue = EPI_CONVT
+        e.out_dtype = L.dt(out); e.ldo = Cout
+    a.epi = e
+    L.call("mmg_conv_transpose2d_fp8", a)
+    return out
+
+
 def conv_in(img, w, bias, out, ksize=5):
     a = L.ConvInArgs()
     a.ksize = ksize

@@ -3,7 +3,8 @@
 Same constructor keywords, attribute names, state_dict keys and method signatures as the reference for the inference
 surface (encode / decode / decode_from_ids / forward without losses / get_encoded_fmap_size / copy_for_eval / save / load).
 The modules below only HOLD parameters under the reference's key names; all arithmetic happens in the sm_90a kernels:
-convolutions are implicit GEMMs over NHWC activations (wgmma + TMA in bf16 precision), the quantizer is the LFQ sign
+convolutions are implicit GEMMs over NHWC activations (wgmma + TMA in bf16 precision, or e4m3 operands with per-image and per-row
+scales under precision="fp8"), the quantizer is the LFQ sign
 scan / explicit L2 argmin scan.  Training losses (GAN, VGG; vqgan_vae.py:350-385, 465-534) are out of scope.
 """
 import copy
@@ -125,7 +126,12 @@ class VQGanVAE(nn.Module):
         self.discr, self._vgg = None, None
         self.precision = precision or "bf16"
         if self.precision == "fp8":
-            raise ValueError('VQGanVAE has no fp8 mode: use precision="bf16" (the transformer\'s precision="fp8" runs over a bf16 VAE)')
+            # e4m3 convolutions take one k-block per tap and 128 input channels: every conv / conv-transpose input width must be a multiple
+            # of 128 (the stem conv_in and the final 1x1 RGB conv stay as they are)
+            for w in self._conv_input_widths():
+                if w % 128:
+                    raise ValueError(f'VQGanVAE precision="fp8" needs every conv input width to be a multiple of 128; this model has a conv '
+                                     f'with {w} input channels (use precision="bf16")')
         self._pack = None
         # both hooks also fire when a PARENT module (MaskGit, Muse) loads a checkpoint: checkpoints written by the reference carry
         # discriminator / VGG tensors (vqgan_vae.py:344-348, dropped by copy_for_eval :394-403) that are not part of inference
@@ -136,6 +142,11 @@ class VQGanVAE(nn.Module):
     def _drop_training_only_keys(state_dict, prefix, *_):
         for k in [k for k in state_dict if k.startswith((prefix + "discr.", prefix + "_vgg."))]:
             del state_dict[k]
+
+    def _conv_input_widths(self):
+        """input channels of every conv and conv-transpose the implicit-GEMM kernels run (not the stem conv_in nor the final 1x1)"""
+        ed = self.enc_dec
+        return [e[2] for e in ed.enc_plan + ed.dec_plan if e[0] in ("down", "res", "glu", "up")]
 
     def _weights_sig(self):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
@@ -180,10 +191,11 @@ class VQGanVAE(nn.Module):
 
     # ----- weight packing ---------------------------------------------------------------------------------------
     def _adt(self):
-        return torch.bfloat16 if self.precision == "bf16" else torch.float32
+        """activation dtype: bf16 for "bf16" and "fp8" (e4m3 is only the operand type of the convolutions), fp32 for "fp32\""""
+        return torch.bfloat16 if self.precision in ("bf16", "fp8") else torch.float32
 
     def _packed(self):
-        if self._pack is not None and self._pack["adt"] == self._adt():
+        if self._pack is not None and self._pack["adt"] == self._adt() and self._pack.get("fp8", False) == (self.precision == "fp8"):
             return self._pack
         dev = self.device
         assert dev.type == "cuda", "VQGanVAE runs on CUDA only (libmmg.so); there is no CPU path"
@@ -194,10 +206,19 @@ class VQGanVAE(nn.Module):
 
     def _build_pack(self):
         adt, dev = self._adt(), self.device
-        P = {"adt": adt}
+        fp8 = self.precision == "fp8"
+        P = {"adt": adt, "fp8": fp8}
         ed, L = self.enc_dec, self.enc_dec.layers
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
-        conv_w = lambda w: w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).to(dev, adt).contiguous()   # (Cout,kh,kw,Cin)
+        # (Cout,kh,kw,Cin); fp8 keeps fp32 here and quantises the finished row layout in `wq`
+        conv_w = lambda w: w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).to(dev, torch.float32 if fp8 else adt).contiguous()
+
+        def wq(w2d):
+            """the operand the conv kernels take: the packed weight itself, or (fp8) its e4m3 rows and one fp32 scale per output row"""
+            if not fp8:
+                return w2d
+            from .muse_maskgit import quantize_rows_e4m3
+            return quantize_rows_e4m3(w2d)
 
         def glu_interleave(w2d, bias):         # rows [a(32) | gate(32)] per block so the epilogue sees both halves of a unit
             C2 = w2d.shape[0]; Cc = C2 // 2
@@ -211,19 +232,19 @@ class VQGanVAE(nn.Module):
         P["enc"], P["dec"] = {}, {}                                     # module index -> packed tensors, following enc_plan / dec_plan
         for kind, i, *_ in ed.enc_plan:
             if kind == "down":
-                P["enc"][i] = (conv_w(ed.encoders[i][0].weight), f32(ed.encoders[i][0].bias))
+                P["enc"][i] = (wq(conv_w(ed.encoders[i][0].weight)), f32(ed.encoders[i][0].bias))
             elif kind == "res":
                 n = ed.encoders[i].net
-                P["enc"][i] = dict(w1=conv_w(n[0].weight), b1=f32(n[0].bias), g1=f32(n[1].weight), be1=f32(n[1].bias),
-                                   w2=conv_w(n[3].weight), b2=f32(n[3].bias), g2=f32(n[4].weight), be2=f32(n[4].bias),
-                                   w3=conv_w(n[6].weight), b3=f32(n[6].bias))
+                P["enc"][i] = dict(w1=wq(conv_w(n[0].weight)), b1=f32(n[0].bias), g1=f32(n[1].weight), be1=f32(n[1].bias),
+                                   w2=wq(conv_w(n[3].weight)), b2=f32(n[3].bias), g2=f32(n[4].weight), be2=f32(n[4].bias),
+                                   w3=wq(conv_w(n[6].weight)), b3=f32(n[6].bias))
         for kind, i, *_ in ed.dec_plan:
             if kind == "glu":
                 n = ed.decoders[i].net
                 w1, b1 = glu_interleave(conv_w(n[0].weight), f32(n[0].bias))
                 w2, b2 = glu_interleave(conv_w(n[3].weight), f32(n[3].bias))
-                P["dec"][i] = dict(w1=w1, b1=b1, g1=f32(n[2].weight), be1=f32(n[2].bias), w2=w2, b2=b2, g2=f32(n[5].weight),
-                                   be2=f32(n[5].bias), w3=conv_w(n[6].weight), b3=f32(n[6].bias))
+                P["dec"][i] = dict(w1=wq(w1), b1=b1, g1=f32(n[2].weight), be1=f32(n[2].bias), w2=wq(w2), b2=b2, g2=f32(n[5].weight),
+                                   be2=f32(n[5].bias), w3=wq(conv_w(n[6].weight)), b3=f32(n[6].bias))
             elif kind == "up":
                 ct = ed.decoders[i][0]
                 w = ct.weight.detach().to(dev, torch.float32)                 # (Cin, Cout, 4, 4)
@@ -232,7 +253,12 @@ class VQGanVAE(nn.Module):
                     for px in range(2):
                         taps = [w[:, :, CT_R[py][a], CT_R[px][b]].t() for a in range(2) for b in range(2)]   # each (Cout, Cin)
                         packs.append(torch.cat(taps, dim=1))
-                P["dec"][i] = (torch.stack(packs).to(adt).contiguous(), f32(ct.bias))
+                st = torch.stack(packs)                                        # [4 parities, Cout, 4 Cin]
+                if fp8:                                                        # one scale per row of each parity stack: [4, Cout]
+                    q, s = wq(st.reshape(-1, st.shape[2]))
+                    P["dec"][i] = ((q.view(st.shape).contiguous(), s.view(4, -1).contiguous()), f32(ct.bias))
+                else:
+                    P["dec"][i] = (st.to(adt).contiguous(), f32(ct.bias))
         last = ed.decoders[-1]
         P["rgb_w"], P["rgb_b"] = f32(last.weight.reshape(last.weight.shape[0], -1)), f32(last.bias)
         P["rgb_w_adt"] = P["rgb_w"].to(adt).contiguous()
@@ -265,6 +291,24 @@ class VQGanVAE(nn.Module):
         return P
 
     # ----- NHWC pipelines (all arithmetic in libmmg) ---------------------------------------------------------------
+    @staticmethod
+    def _conv(x, w, out, B, H, W, Cin, Cout, kind, **epi):
+        """one convolution of the pipelines; w is a packed bf16 / fp32 weight, or (fp8) the pair (e4m3 rows, row scales): the input map is
+        then quantised per image for this conv alone"""
+        if isinstance(w, tuple):
+            VQGanVAE._check_fp8_grid(*((H // 2, W // 2) if kind == 2 else (H, W)))
+            q, s = ops.quantize_e4m3_images(x, B)
+            return ops.conv2d_fp8(q, s, w[0], w[1], out, B, H, W, Cin, Cout, kind, **epi)
+        return ops.conv2d(x, w, out, B, H, W, Cin, Cout, kind, **epi)
+
+    @staticmethod
+    def _conv_t(x, w, out, B, H, W, Cin, Cout, **epi):
+        if isinstance(w, tuple):
+            VQGanVAE._check_fp8_grid(H, W)
+            q, s = ops.quantize_e4m3_images(x, B)
+            return ops.conv_transpose2d_fp8(q, s, w[0], w[1], out, B, H, W, Cin, Cout, **epi)
+        return ops.conv_transpose2d(x, w, out, B, H, W, Cin, Cout, **epi)
+
     def _encode_nhwc(self, img):
         """img (B,C,H,W) fp32 -> fmap NHWC [B*f*f, D] in activation dtype.  ref: vqgan_vae.py:241-244"""
         P, ed = self._packed(), self.enc_dec
@@ -279,16 +323,16 @@ class VQGanVAE(nn.Module):
                 cin, cout = cc
                 cw, cb = P["enc"][i]
                 y = torch.empty((B * (h // 2) * (w // 2), cout), device=dev, dtype=adt)
-                ops.conv2d(x, cw, y, B, h, w, cin, cout, kind=2, bias=cb, act=1)
+                self._conv(x, cw, y, B, h, w, cin, cout, kind=2, bias=cb, act=1)
                 x, h, w = y, h // 2, w // 2
             else:                                   # ResBlock (vqgan_vae.py:267-281)
                 R, D = P["enc"][i], cc[0]
                 t1 = torch.empty_like(x); t2 = torch.empty_like(x); out = torch.empty_like(x)
-                ops.conv2d(x, R["w1"], t1, B, h, w, D, D, kind=1, bias=R["b1"])
+                self._conv(x, R["w1"], t1, B, h, w, D, D, kind=1, bias=R["b1"])
                 ops.groupnorm_(t1, R["g1"], R["be1"], B, h * w, D, ed.groups, act=1)
-                ops.conv2d(t1, R["w2"], t2, B, h, w, D, D, kind=1, bias=R["b2"])
+                self._conv(t1, R["w2"], t2, B, h, w, D, D, kind=1, bias=R["b2"])
                 ops.groupnorm_(t2, R["g2"], R["be2"], B, h * w, D, ed.groups, act=1)
-                ops.conv2d(t2, R["w3"], out, B, h, w, D, D, kind=0, epilogue=ops.EPI_RESIDUAL, bias=R["b3"], resid=x)
+                self._conv(t2, R["w3"], out, B, h, w, D, D, kind=0, epilogue=ops.EPI_RESIDUAL, bias=R["b3"], resid=x)
                 x = out
         return x, h, w
 
@@ -301,11 +345,11 @@ class VQGanVAE(nn.Module):
             if kind == "glu":                       # GLUResBlock (vqgan_vae.py:251-265)
                 R, D = P["dec"][i], cc[0]
                 t1 = torch.empty_like(x); t2 = torch.empty_like(x); out = torch.empty_like(x)
-                ops.conv2d(x, R["w1"], t1, B, h, w, D, 2 * D, kind=1, epilogue=ops.EPI_GLU, bias=R["b1"])
+                self._conv(x, R["w1"], t1, B, h, w, D, 2 * D, kind=1, epilogue=ops.EPI_GLU, bias=R["b1"])
                 ops.groupnorm_(t1, R["g1"], R["be1"], B, h * w, D, ed.groups)
-                ops.conv2d(t1, R["w2"], t2, B, h, w, D, 2 * D, kind=1, epilogue=ops.EPI_GLU, bias=R["b2"])
+                self._conv(t1, R["w2"], t2, B, h, w, D, 2 * D, kind=1, epilogue=ops.EPI_GLU, bias=R["b2"])
                 ops.groupnorm_(t2, R["g2"], R["be2"], B, h * w, D, ed.groups)
-                ops.conv2d(t2, R["w3"], out, B, h, w, D, D, kind=0, epilogue=ops.EPI_RESIDUAL, bias=R["b3"], resid=x)
+                self._conv(t2, R["w3"], out, B, h, w, D, D, kind=0, epilogue=ops.EPI_RESIDUAL, bias=R["b3"], resid=x)
                 x = out
                 continue
             cin, cout = cc                          # ConvTranspose2d(4, 2, 1) + LeakyReLU
@@ -314,14 +358,23 @@ class VQGanVAE(nn.Module):
             fuse_rgb = last and adt == torch.bfloat16 and cout in (64, 128, 256) and cin % 64 == 0 and self._tc_tile_ok(h, w)
             if fuse_rgb:
                 img = torch.empty((B, self.channels, 2 * h, 2 * w), device=dev, dtype=torch.float32)
-                ops.conv_transpose2d(x, cw, img, B, h, w, cin, cout, bias=cb, rgb_w=P["rgb_w"], rgb_b=P["rgb_b"])
+                self._conv_t(x, cw, img, B, h, w, cin, cout, bias=cb, rgb_w=P["rgb_w"], rgb_b=P["rgb_b"])
                 return img
             y = torch.empty((B * 4 * h * w, cout), device=dev, dtype=adt)
-            ops.conv_transpose2d(x, cw, y, B, h, w, cin, cout, bias=cb)
+            self._conv_t(x, cw, y, B, h, w, cin, cout, bias=cb)
             x, h, w = y, 2 * h, 2 * w
         rgb = torch.empty((B * h * w, self.channels), device=dev, dtype=torch.float32)
         ops.linear(x, P["rgb_w_adt"], rgb, bias=P["rgb_b"])
         return rgb.view(B, h, w, self.channels).permute(0, 3, 1, 2).contiguous()
+
+    @staticmethod
+    def _check_fp8_grid(h, w):
+        """the e4m3 convolutions have no CUDA-core kernel behind them: each conv's output grid (conv-transpose: input grid) must have a
+        conv tile geometry, which holds for square power-of-two image sizes and for most multiples of 128 pixels"""
+        if not VQGanVAE._tc_tile_ok(h, w):
+            raise ValueError(f'VQGanVAE precision="fp8": a {h} x {w} feature map has no tile geometry for the e4m3 convolutions (the tile '
+                             f'width min(W, 128) must divide 128 and W, and min(128 / width, H) must divide H); use precision="bf16" for '
+                             f'this image size')
 
     @staticmethod
     def _tc_tile_ok(h, w):
