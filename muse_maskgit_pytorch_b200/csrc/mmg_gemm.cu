@@ -9,11 +9,11 @@ int linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* stream)
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// persistent grid of min(tiles, #SM) CTAs; the tile epilogues keep 32 KB of per-warp output tiles next to the operand ring instead of
-// the register epilogues' 66 KB staging buffer
+// persistent grid of min(tiles, #SM) CTAs; every mode but TC_EPI_ACT keeps 32 KB of per-warp output boxes next to the operand ring
+// instead of TC_EPI_ACT's 66 KB staging buffer
 template <int BN, int EPI_MODE, typename TA = bf16>
 static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
-  constexpr int smem = tc_tile_epilogue(EPI_MODE) ? TcCfg<BN>::SMEM_BYTES_RED : TcCfg<BN>::SMEM_BYTES;
+  constexpr int smem = tc_staged_epilogue(EPI_MODE) ? TcCfg<BN>::SMEM_BYTES : TcCfg<BN>::SMEM_BYTES_RED;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, EPI_MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
@@ -70,8 +70,8 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
   const bool geglu_tiles = p.epi.kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && bn == 256 && (e.ldo % 8) == 0 && aligned16(e.out);
   const int epi_mode = in_place ? TC_EPI_REDUCE : (plain_f32 && (bn == 256 || bn == 128)) ? TC_EPI_TSTORE : qkv_tiles ? TC_EPI_QKV :
                        geglu_tiles ? TC_EPI_GEGLU : TC_EPI_REGS;
-  // the register epilogue keeps 128 accumulator registers per thread at BN = 256 next to its 64-column chunk and spills; the
-  // tile epilogues at BN = 256 and every epilogue at BN = 128 fit the consumer warpgroups' registers
+  // 128 accumulator registers per thread at BN = 256 next to a 64-column row chunk would spill, so <256, TC_EPI_REGS> compiles only
+  // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128
   if (epi_mode == TC_EPI_REGS && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
   // the tile epilogues write whole 32- / 64-column boxes: pick_bn's widths divide N (N % 64 == 0 on this path)
   MMG_CHECK_ARG(epi_mode == TC_EPI_REGS || N % bn == 0, "tile epilogue: tile width %d does not divide N = %lld", bn, (long long)N);
@@ -350,7 +350,7 @@ static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7
 
 static int launch_conv_fp8(TcGemmParams& p, const void* w, int64_t N, int64_t K, cudaStream_t st) {
   int bn = pick_bn(p.num_m_tiles, N, p.epi.kind);
-  if (bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;        // dispatch_tc's register-epilogue width
+  if (bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;        // dispatch_tc's register-epilogue width (<256, REGS>: RGB only)
   p.num_n_tiles = (int)((N + bn - 1) / bn);
   p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;   // the bf16 product's tile order
   uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)K}; uint32_t box[2] = {128, (uint32_t)bn};

@@ -3,11 +3,11 @@
 //   warp 0      : TMA producer  (one elected lane) — A tile 128x64 and W tile BNx64 per k-block, SWIZZLE_128B, STAGES-deep ring
 //                 (e4m3 operands: 128 x 128 and BN x 128 — the same 128-byte rows, so the ring, boxes and descriptors are unchanged)
 //   warps 4..11 : two consumer warpgroups.  Warpgroup g multiplies rows [64 g, 64 g + 64) of the tile (wgmma m64nBNk16, 4 per k-block,
-//                 accumulators in registers), then runs the fused Epilogue on those rows (EPI_MODE below): either from the accumulator
-//                 registers into per-warp shared-memory boxes and a TMA store / TMA reduction, or through a shared-memory staging buffer
-//                 (128 columns at a time) so that one thread owns one output row, 64 columns per chunk; two warps then share a 32-row
-//                 quarter and take alternate 64-column chunks.  setmaxnreg moves registers from warpgroup 0 (40/thread) to the consumers
-//                 (232/thread).
+//                 accumulators in registers), then runs the fused Epilogue on those rows (EPI_MODE below): from the accumulator
+//                 registers into per-warp shared-memory boxes, then a TMA store / TMA reduction (tile epilogues) or one lane per row and
+//                 64-column chunk (TC_EPI_REGS); TC_EPI_ACT goes through a shared-memory staging buffer (128 columns at a time), where two
+//                 warps share a 32-row quarter and take alternate 64-column chunks.  setmaxnreg moves registers from warpgroup 0
+//                 (40/thread) to the consumers (232/thread).
 //   persistent grid (<= #SM CTAs), static tile schedule (M- or N-fastest); the producer runs ahead into the next tile while the consumers
 //   finish the epilogue of the current one.
 //
@@ -31,15 +31,17 @@ constexpr int TC_SMEM_LIMIT = 227 * 1024;
 
 // How the epilogue's results leave the CTA (the EPI_MODE of tc_gemm_kernel; described above the kernel).  The launcher picks one per product.
 enum TcEpiMode : int {
-  TC_EPI_REGS = 0,      // from registers, one thread per row
+  TC_EPI_REGS = 0,      // every Epilogue kind: fragments -> per-warp box -> one lane per row (CONVT_RGB: a quad reduction of the fragments)
   TC_EPI_REDUCE = 2,    // in-place residual: per-warp tiles + TMA reduction
   TC_EPI_TSTORE = 3,    // plain fp32: per-warp tiles + TMA store
   TC_EPI_QKV = 4,       // QKV heads: per-warp tiles + TMA stores
   TC_EPI_GEGLU = 5,     // GEGLU, BN = 256: per-warp tiles + TMA store
-  TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: from registers, one thread per row
+  TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: staging buffer, one thread per row
 };
-// the modes whose epilogue runs from the accumulator fragments through per-warp output boxes (no staging buffer)
+// the modes whose epilogue runs from the accumulator fragments through per-warp output boxes
 constexpr bool tc_tile_epilogue(int mode) { return mode != TC_EPI_REGS && mode != TC_EPI_ACT; }
+// the modes that keep the shared-memory staging buffer (and its shallower operand ring); every other mode uses the 32 KB of per-warp boxes
+constexpr bool tc_staged_epilogue(int mode) { return mode == TC_EPI_ACT; }
 
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
@@ -62,9 +64,9 @@ struct alignas(64) TcGemmParams {
   const float* w_scale;
 };
 
-// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][register epilogues: staging, 2 x 64 x 132 fp32 | tile epilogues: per-warp
-// output tiles, 32 KB].  Without the staging buffer the tile epilogues get 4 operand stages at BN = 256 and 6 at BN <= 128 (register
-// epilogues: 3, 4 and 6 at BN = 256, 128, 64); the 512 B static s_scale fits in what the 227 KB limit leaves over.
+// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][TC_EPI_ACT: staging, 2 x 64 x 132 fp32 | every other mode: per-warp
+// output boxes, 32 KB].  Without the staging buffer a kernel gets 4 operand stages at BN = 256 and 6 at BN <= 128 (TC_EPI_ACT, BN = 128:
+// 4); the 512 B static s_scale fits in what the 227 KB limit leaves over.
 template <int BN> struct TcCfg {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;
   static constexpr int B_BYTES = BN * TC_BK * 2;
@@ -82,12 +84,16 @@ template <int BN> struct TcCfg {
   static_assert(SMEM_BYTES + 512 <= TC_SMEM_LIMIT && SMEM_BYTES_RED + 512 <= TC_SMEM_LIMIT, "dynamic + static shared memory over the opt-in limit");
 };
 
-// Register epilogues (TC_EPI_REGS, TC_EPI_ACT) need one thread to own a whole output row, so the accumulators go through the staging
-// buffer.  The tile epilogues need no such thing: each of their terms is elementwise, or (GEGLU) pairs column i with column 32 + i, which
-// the wgmma fragment keeps in the same thread.  They go from the accumulator registers straight into the warp's output boxes, and the
-// TMA engine writes the boxes out.  Thread t of a warpgroup (warp w, lane l) holds rows 16 w + l / 4 and + 8 at columns 8 j + 2 (l % 4)
-// and + 1, so a warp owns 16 whole rows; a box is 16 rows x 128 bytes (TMA 128-byte swizzle), and the warp's 4 KB tile double-buffers two.
-// The launcher takes a tile epilogue only at a tile width BN that divides N, so every box lies inside the N columns.
+// The Epilogue kinds (mmg_epilogue.cuh) are written for one thread that owns a 64-column chunk of a row.  TC_EPI_ACT gets such chunks
+// through the staging buffer.  The tile epilogues need no such thing: each of their terms is elementwise, or (GEGLU) pairs column i with
+// column 32 + i, which the wgmma fragment keeps in the same thread.  They go from the accumulator registers straight into the warp's output
+// boxes, and the TMA engine writes the boxes out.  Thread t of a warpgroup (warp w, lane l) holds rows 16 w + l / 4 and + 8 at columns
+// 8 j + 2 (l % 4) and + 1, so a warp owns 16 whole rows; a box is 16 rows x 128 bytes (TMA 128-byte swizzle), and the warp's 4 KB tile
+// double-buffers two.  The launcher takes a tile epilogue only at a tile width BN that divides N, so every box lies inside the N columns.
+// TC_EPI_REGS uses the same 4 KB per warp as one fp32 box of its 16 rows x 64 columns: each 64-column chunk of the fragments goes into it,
+// and lane r < 16 reads row r back and runs the Epilogue kind on it, so every kind computes what it computes elsewhere, element for
+// element.  CONVT_RGB never forms a row: each thread projects its own fragment columns onto the (<= 4) RGB weights and two shuffles
+// finish the sum over the lane quad that shares a row.
 // TC_EPI_REDUCE: in-place residual epilogues (out == resid, fp32) push the term they add with a TMA reduction
 // (cp.reduce.async.bulk.tensor .add), 32 columns per box: the residual is never read and the adds happen in L2.
 // TC_EPI_TSTORE: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same boxes with a TMA store.
@@ -147,7 +153,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   constexpr bool ACTT = EPI_MODE == TC_EPI_ACT;
   constexpr bool TILES = tc_tile_epilogue(EPI_MODE);
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
-  constexpr int STAGES = TILES ? Cfg::STAGES_RED : Cfg::STAGES;
+  constexpr int STAGES = tc_staged_epilogue(EPI_MODE) ? Cfg::STAGES : Cfg::STAGES_RED;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
   constexpr int ROUNDS = (BN + 127) / 128;
   // residual rows are fetched one chunk ahead (the first one during the main loop) only at BN <= 128: at BN = 256 the 128 accumulator
@@ -243,10 +249,10 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
       }
       const bool mine = !whole_row || half == 0;
       const int c_first = whole_row ? 0 : half, c_step = whole_row ? 1 : 2, c_end = BN / 64;
-      const bool pre = EARLY_RESID && !TILES && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
+      const bool pre = EARLY_RESID && ACTT && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
       float rbuf[64];
       if (pre) epi.load_resid(row, n_blk * BN + c_first * 64, rbuf);      // in flight during the main loop
-      if (!TILES && valid && mine) epi.begin_row(row);                     // row geometry / folded-LayerNorm statistics: independent of the accumulator
+      if (ACTT && valid && mine) epi.begin_row(row);                       // row geometry / folded-LayerNorm statistics: independent of the accumulator
       // tile epilogues: the warp's 16 fragment rows start at brow; LNFOLD statistics of row brow + l / 4 + 8 (l % 4) in lanes l % 4 < 2
       const int64_t brow = (int64_t)m_blk * TC_BM + wg * 64 + 16 * wq;
       float ln_a = 0.f, ln_b = 0.f;
@@ -445,9 +451,97 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
             }
           }
         }
+      } else if constexpr (!ACTT) {
+        // ---- TC_EPI_REGS, from the accumulator fragments (layout above the kernel) ----
+        const int r0 = wg * 64 + 16 * wq;                          // the warp's 16 rows of the tile
+        if constexpr (FP8_CONV) dequant_acc_images<BN>(acc, p, m_blk, r0, n_blk * BN, lane);
+        const int q = lane & 3, fr = lane >> 2;
+        // global output row of tile row r; false for rows past M (dense) or of images past B (conv), which are never stored
+        auto out_row = [&](int r, int64_t& orow) {
+          if (p.mode == 0) { orow = (int64_t)m_blk * TC_BM + r; return orow < p.M; }
+          const int xt = m_blk % p.tiles_x, yt = (m_blk / p.tiles_x) % p.tiles_y, bt = m_blk / (p.tiles_x * p.tiles_y);
+          const int tx = r % p.TW, ty = (r / p.TW) % p.TH, b = bt * p.TB + r / (p.TW * p.TH);
+          orow = ((int64_t)b * p.Ho + (yt * p.TH + ty)) * p.Wo + xt * p.TW + tx;
+          return b < p.B;
+        };
+        if (epi.kind == MMG_EPI_CONVT_RGB) {
+          // bias + LeakyReLU per element, then the <= 4 channel dot products over this thread's BN / 4 columns of rows fr and fr + 8, and
+          // over the lane quad (shfl.xor 1, 2).  The launcher gives CONVT_RGB one tile of BN = N columns, so n_blk == 0 and every column
+          // is valid.  Lane q = 0 writes row fr's pixel, lane q = 1 row fr + 8's (NCHW fp32).
+          const mmg_epilogue_args& e = epi.p;
+          float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int c = 8 * j + 2 * q;
+            const float b0 = e.bias ? __ldg(e.bias + c) : 0.f, b1 = e.bias ? __ldg(e.bias + c + 1) : 0.f;
+            const float x0 = leaky01(acc[4 * j] + b0), x1 = leaky01(acc[4 * j + 1] + b1);
+            const float y0 = leaky01(acc[4 * j + 2] + b0), y1 = leaky01(acc[4 * j + 3] + b1);
+#pragma unroll
+            for (int ch = 0; ch < 4; ++ch) {
+              if (ch < e.rgb_channels) {
+                const float* w = e.rgb_w + (int64_t)ch * BN + c;
+                const float w0 = __ldg(w), w1 = __ldg(w + 1);
+                s0[ch] = fmaf(x1, w1, fmaf(x0, w0, s0[ch]));
+                s1[ch] = fmaf(y1, w1, fmaf(y0, w0, s1[ch]));
+              }
+            }
+          }
+#pragma unroll
+          for (int ch = 0; ch < 4; ++ch) {
+            s0[ch] += __shfl_xor_sync(0xffffffffu, s0[ch], 1); s0[ch] += __shfl_xor_sync(0xffffffffu, s0[ch], 2);
+            s1[ch] += __shfl_xor_sync(0xffffffffu, s1[ch], 1); s1[ch] += __shfl_xor_sync(0xffffffffu, s1[ch], 2);
+          }
+          int64_t orow;
+          if (q < 2 && out_row(r0 + fr + 8 * q, orow)) {
+            const uint32_t hw = (uint32_t)(e.H * e.W), rr = (uint32_t)orow;
+            const int64_t b = rr / hw;
+            const int rem = (int)(rr - (uint32_t)b * hw), y = rem / e.W, x = rem - y * e.W;
+            const int64_t plane = (int64_t)(2 * e.H) * (2 * e.W), pix = (int64_t)(2 * y + e.py) * (2 * e.W) + 2 * x + e.px;
+            float* o = reinterpret_cast<float*>(e.out) + b * e.rgb_channels * plane + pix;
+#pragma unroll
+            for (int ch = 0; ch < 4; ++ch)
+              if (ch < e.rgb_channels) o[ch * plane] = e.rgb_b[ch] + (q ? s1[ch] : s0[ch]);
+          }
+        } else if constexpr (BN <= 128) {
+          // every other kind, 64 columns at a time: the fragments of chunk c -> the warp's box (16 rows of 256 B; 16-byte slot k of row r
+          // at k ^ (r & 7), conflict-free for both the fragment writes and the row reads) -> lane r < 16 runs row r0 + r.  The launchers
+          // give these kinds BN <= 128 only: at BN = 256 the 128 accumulators and a 64-column row would not fit the registers.
+          const uint32_t box = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;
+          int64_t orow = 0;
+          const bool own = lane < 16 && out_row(r0 + lane, orow);
+          if (own) epi.begin_row(orow);
+#pragma unroll
+          for (int c = 0; c < BN / 64; ++c) {
+            const int col0 = n_blk * BN + 64 * c;
+            if (col0 >= p.N) break;
+            __syncwarp();                                        // the lanes are done reading the previous chunk
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * c + jj;
+              const uint32_t off = (uint32_t)(((2 * jj + (q >> 1)) ^ fr) * 16 + 8 * (q & 1));
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" :: "r"(box + (uint32_t)fr * 256u + off), "f"(acc[4 * j]), "f"(acc[4 * j + 1]) : "memory");
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" :: "r"(box + (uint32_t)(fr + 8) * 256u + off), "f"(acc[4 * j + 2]), "f"(acc[4 * j + 3]) : "memory");
+            }
+            __syncwarp();
+            if (own) {
+              float v[64];
+#pragma unroll
+              for (int k = 0; k < 16; ++k)
+                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[4 * k]), "=f"(v[4 * k + 1]), "=f"(v[4 * k + 2]), "=f"(v[4 * k + 3])
+                             : "r"(box + (uint32_t)lane * 256u + (uint32_t)((k ^ (lane & 7)) * 16)) : "memory");
+              if (prefetch_resid) {
+                float r[64];
+                epi.load_resid(orow, col0, r);
+                epi.fuse_resid(col0, v, r);
+                epi.store_f32(orow, col0, v);
+              } else {
+                epi.template apply<true>(orow, col0, v, 64);
+              }
+            }
+          }
+        }
       } else {
-        // ---- register epilogues: columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread ----
-        if constexpr (FP8_CONV) dequant_acc_images<BN>(acc, p, m_blk, wg * 64 + 16 * wq, n_blk * BN, lane);
+        // ---- TC_EPI_ACT: columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread ----
         // the epilogue of one 64-column accumulator chunk held in v
         auto chunk = [&](const int c, float (&v)[64]) {
           const int col0 = n_blk * BN + c * 64;
