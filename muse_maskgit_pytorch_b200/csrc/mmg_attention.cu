@@ -2,7 +2,8 @@
 // replaces Attend.forward / flash_attn (attend.py:66-140).
 //   * mmg_attention with dtype MMG_F32  -> fp32 CUDA-core kernel (parity precision)
 //   * mmg_attention with dtype MMG_BF16 -> wgmma kernel (mmg_attention_tc.cuh): S = Q K^T and O = P V on the tensor
-//     cores, S staged through shared memory, O accumulated in registers.
+//     cores; the softmax runs on the S accumulator fragments and feeds P to the P V product as a register operand, O stays in
+//     registers through the epilogue; a producer warp keeps a ring of K / V stages loading under the math.
 #include "mmg_common.cuh"
 #include "mmg_attention_tc.cuh"
 #include "mmg_attention_split.cuh"
@@ -82,7 +83,7 @@ static int attn_launch(const AttnTcParams& p, dim3 grid, cudaStream_t st) {
   static std::once_flag once; static cudaError_t err = cudaSuccess;
   std::call_once(once, [] { err = cudaFuncSetAttribute(attention_tc_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); });
   if (err != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(attention_tc): %s", cudaGetErrorString(err));
-  MMG_CUDA(launch_pdl(attention_tc_kernel<KB>, grid, dim3(160), smem, st, p));
+  MMG_CUDA(launch_pdl(attention_tc_kernel<KB>, grid, dim3(ATTN_THREADS), smem, st, p));
   MMG_LAUNCHED();
   return MMG_OK;
 }

@@ -154,6 +154,25 @@ template <> struct Wgmma<256> {
   }
 };
 
+// D[64 x 64] (+)= A[64 x 16] * B[16 x 64] with A from registers ("RS"): thread t holds a[0..3] = bf16 pairs of A at rows 16 w + l / 4
+// (+ 8 for a[1], a[3]) and columns 2 (l % 4) (+ 8 for a[2], a[3]).  That is the accumulator layout above: the fp32 fragment d[8 s .. 8 s + 7]
+// of an m64nN product, packed pairwise, is the A operand of k16 step s of a following product.  B (V) is MN-major, as Wgmma<N>::mma<1>.
+struct WgmmaRS64 {
+  static __device__ __forceinline__ void mma(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+  }
+};
+
 // D[64 x N] (+)= A[64 x 32] * B[32 x N] with e4m3 operands: same descriptors (a 128-byte row now holds 128 elements, so a K step of 32
 // still adds 32 B), same accumulator fragment layout.  fp8 wgmma takes K-major A and B only, so there is no transpose operand.
 template <int N> struct WgmmaE4m3;
