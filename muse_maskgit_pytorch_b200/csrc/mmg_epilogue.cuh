@@ -1,5 +1,7 @@
-// Fused GEMM epilogues, shared by the wgmma kernel (mmg_gemm_tc.cuh) and the fp32 CUDA-core kernel
-// (mmg_gemm_simt.cu).  One thread owns one output row and walks it in chunks of 64 accumulator columns.
+// Fused GEMM epilogues, shared by the wgmma kernel (mmg_gemm_tc.cuh) and the fp32 CUDA-core kernel (simt_gemm_kernel in
+// mmg_gemm.cu).  One thread owns one output row and runs it one chunk of 64 accumulator columns at a time.  apply<FAST>: FAST (the
+// tensor-core kernel) takes MUFU-based erf / sigmoid, accurate far beyond bf16 output precision.  The fused RGB projection (CONVT_RGB)
+// is not here: the tensor-core kernel computes it from the accumulator fragments, and no other kernel is offered it.
 #pragma once
 #include "mmg_common.cuh"
 
@@ -8,9 +10,6 @@ namespace mmg {
 struct Epilogue {
   mmg_epilogue_args p;
   int kind;
-  int fast;                 // 1: tensor-core (bf16) path — MUFU-based erf/sigmoid are accurate far beyond bf16 output precision
-  int64_t M, N;
-  float rgb_acc[4];
   float st_a, st_b;         // LNFOLD: (mean, rstd) of the row
   int r_b, r_t;             // QKV: (batch, token) of the row; CONVT*: (batch, y * W + x)
   // the 16-byte vector accesses (Vec64, store32_bf16, float4) need a 16-byte aligned address: a row stride that is a multiple of 8 elements
@@ -49,12 +48,8 @@ struct Epilogue {
 
   __device__ __forceinline__ void begin_row(int64_t row) {
     if (kind == MMG_EPI_QKV) { const uint32_t r = (uint32_t)row, d = (uint32_t)p.tokens; r_b = (int)(r / d); r_t = (int)(r - (uint32_t)r_b * d); }
-    if (kind == MMG_EPI_CONVT || kind == MMG_EPI_CONVT_RGB) { const uint32_t r = (uint32_t)row, d = (uint32_t)(p.H * p.W); r_b = (int)(r / d); r_t = (int)(r - (uint32_t)r_b * d); }
+    if (kind == MMG_EPI_CONVT) { const uint32_t r = (uint32_t)row, d = (uint32_t)(p.H * p.W); r_b = (int)(r / d); r_t = (int)(r - (uint32_t)r_b * d); }
     if (kind == MMG_EPI_LNFOLD_RESIDUAL) ln_row_stats(row, st_a, st_b);
-    if (kind == MMG_EPI_CONVT_RGB) {
-#pragma unroll
-      for (int c = 0; c < 4; ++c) rgb_acc[c] = (c < p.rgb_channels) ? p.rgb_b[c] : 0.f;
-    }
   }
 
   // row: global output row (< M). col0: first accumulator column of this chunk (multiple of 64). nvalid: columns < N.
@@ -247,37 +242,24 @@ struct Epilogue {
         if (t == 0 && which != 0) qkv_null_row(which, b, h);
         break;
       }
-      case MMG_EPI_CONVT:
-      case MMG_EPI_CONVT_RGB: {
+      case MMG_EPI_CONVT: {
 #pragma unroll
         for (int i = 0; i < 64; ++i) v[i] = leaky01(v[i] + (p.bias && i < nvalid ? __ldg(p.bias + col0 + i) : 0.f));
-        if (kind == MMG_EPI_CONVT) {
-          const int64_t b = r_b; const int rem = r_t; const int y = rem / p.W, x = rem - y * p.W;
-          const int64_t opix = (b * 2 * p.H + 2 * y + p.py) * (int64_t)(2 * p.W) + 2 * x + p.px;
-          const bool vec_ok = (nvalid == 64) && ((p.ldo & 7) == 0);
-          if (bf) store_n(reinterpret_cast<bf16*>(p.out) + opix * p.ldo + col0, v, nvalid, vec_ok);
-          else    store_n(reinterpret_cast<float*>(p.out) + opix * p.ldo + col0, v, nvalid, vec_ok);
-        } else {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            if (c < p.rgb_channels) {
-              const float* w = p.rgb_w + (int64_t)c * N + col0;
-              float s = 0.f;
-#pragma unroll
-              for (int i = 0; i < 64; ++i) if (i < nvalid) s += v[i] * __ldg(w + i);
-              rgb_acc[c] += s;
-            }
-          }
-        }
+        const int64_t b = r_b; const int rem = r_t; const int y = rem / p.W, x = rem - y * p.W;
+        const int64_t opix = (b * 2 * p.H + 2 * y + p.py) * (int64_t)(2 * p.W) + 2 * x + p.px;
+        const bool vec_ok = (nvalid == 64) && ((p.ldo & 7) == 0);
+        if (bf) store_n(reinterpret_cast<bf16*>(p.out) + opix * p.ldo + col0, v, nvalid, vec_ok);
+        else    store_n(reinterpret_cast<float*>(p.out) + opix * p.ldo + col0, v, nvalid, vec_ok);
         break;
       }
     }
   }
 
   // ---- T5 feed-forward epilogues: GEGLU_TANH and STORE with ReLU (act == 2) ----------------------------------------------
-  // Kept out of apply() so that the kernels which never see them compile as before: the tensor-core kernel reaches this through its own
-  // TC_EPI_ACT instantiation, the CUDA-core kernel through a kind test.  gelu_new(x) = 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)));
-  // with a bf16 output the MUFU tanh (relative error ~2^-11) is used, below the bf16 rounding that follows; an fp32 output gets tanhf.
+  // Kept out of apply() so that only the instantiations that run them compile them: the tensor-core kernel's TC_EPI_ACT and the CUDA-core
+  // kernel's ACT.  Like apply(), apply_act takes one 64-column chunk of a row; a GEGLU_TANH chunk is [x(32) | gate(32)] -> 32 outputs.
+  // gelu_new(x) = 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))); with a bf16 output the MUFU tanh (relative error ~2^-11) is used,
+  // below the bf16 rounding that follows; an fp32 output gets tanhf.
   static __device__ __forceinline__ float gelu_tanh(float x, bool approx) {
     const float u = 0.7978845608028654f * fmaf(0.044715f * x, x * x, x);
     float t;
@@ -352,17 +334,6 @@ struct Epilogue {
   }
   __device__ __forceinline__ void store_f32(int64_t row, int col0, const float (&v)[64]) const {
     Vec64<float>::store(reinterpret_cast<float*>(p.out) + row * p.ldo + col0, v);
-  }
-
-  __device__ __forceinline__ void end_row(int64_t row) {
-    if (kind == MMG_EPI_CONVT_RGB) {
-      const int64_t b = r_b; const int rem = r_t; const int y = rem / p.W, x = rem - y * p.W;
-      const int oy = 2 * y + p.py, ox = 2 * x + p.px;
-      float* o = reinterpret_cast<float*>(p.out);
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        if (c < p.rgb_channels) o[((b * p.rgb_channels + c) * (int64_t)(2 * p.H) + oy) * (2 * p.W) + ox] = rgb_acc[c];
-    }
   }
 };
 

@@ -9,11 +9,10 @@ int linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* stream)
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// persistent grid of min(tiles, #SM) CTAs; every mode but TC_EPI_ACT keeps 32 KB of per-warp output boxes next to the operand ring
-// instead of TC_EPI_ACT's 66 KB staging buffer
+// persistent grid of min(tiles, #SM) CTAs
 template <int BN, int EPI_MODE, typename TA = bf16>
 static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
-  constexpr int smem = tc_staged_epilogue(EPI_MODE) ? TcCfg<BN>::SMEM_BYTES : TcCfg<BN>::SMEM_BYTES_RED;
+  constexpr int smem = TcCfg<BN>::SMEM_BYTES;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [] { attr_err = cudaFuncSetAttribute(tc_gemm_kernel<BN, EPI_MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
@@ -55,26 +54,21 @@ static int bf16_out_maps(TcGemmParams& p, int epi_mode) {
 
 static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
   const mmg_epilogue_args& e = p.epi.p;
-  if (p.epi.is_act()) {                       // T5 feed-forward epilogues: their own register-epilogue instantiation at BN = 128
-    p.num_n_tiles = (int)((N + 127) / 128);
-    p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, 128};
-    int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
-    return launch_tc<128, TC_EPI_ACT>(p, st);
-  }
   const bool in_place = (p.epi.kind == MMG_EPI_LNFOLD_RESIDUAL || (p.epi.kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
                         e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && p.mode == 0;
   const bool plain_f32 = p.epi.kind == MMG_EPI_STORE && e.out_dtype == MMG_F32 && p.mode == 0 && !e.bias && e.act == 0 && (e.ldo % 4) == 0 && aligned16(e.out);
   const bool qkv_tiles = p.epi.kind == MMG_EPI_QKV && e.out_dtype == MMG_BF16 && p.mode == 0 && e.tokens % 32 == 0 && p.M % 128 == 0 && (bn == 128 || bn == 256) &&
                          (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out))) && e.nk_heads == e.nv_heads;
   const bool geglu_tiles = p.epi.kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && bn == 256 && (e.ldo % 8) == 0 && aligned16(e.out);
-  const int epi_mode = in_place ? TC_EPI_REDUCE : (plain_f32 && (bn == 256 || bn == 128)) ? TC_EPI_TSTORE : qkv_tiles ? TC_EPI_QKV :
-                       geglu_tiles ? TC_EPI_GEGLU : TC_EPI_REGS;
+  const int epi_mode = p.epi.is_act() ? TC_EPI_ACT : in_place ? TC_EPI_REDUCE : (plain_f32 && (bn == 256 || bn == 128)) ? TC_EPI_TSTORE :
+                       qkv_tiles ? TC_EPI_QKV : geglu_tiles ? TC_EPI_GEGLU : TC_EPI_REGS;
   // 128 accumulator registers per thread at BN = 256 next to a 64-column row chunk would spill, so <256, TC_EPI_REGS> compiles only
-  // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128
+  // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128, and the T5
+  // feed-forward epilogues (their own instantiation, kept out of the VAE's) at BN = 128 only
   if (epi_mode == TC_EPI_REGS && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
+  if (epi_mode == TC_EPI_ACT) bn = 128;
   // the tile epilogues write whole 32- / 64-column boxes: pick_bn's widths divide N (N % 64 == 0 on this path)
-  MMG_CHECK_ARG(epi_mode == TC_EPI_REGS || N % bn == 0, "tile epilogue: tile width %d does not divide N = %lld", bn, (long long)N);
+  MMG_CHECK_ARG(!tc_tile_epilogue(epi_mode) || N % bn == 0, "tile epilogue: tile width %d does not divide N = %lld", bn, (long long)N);
   p.num_n_tiles = (int)((N + bn - 1) / bn);
   p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
   uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
@@ -87,6 +81,7 @@ static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_
     rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
     return launch_tc<256, TC_EPI_GEGLU>(p, st);
   }
+  if (epi_mode == TC_EPI_ACT) return launch_tc<128, TC_EPI_ACT>(p, st);
   if (epi_mode != TC_EPI_REGS) {
     uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 16};
     rc = make_tmap_f32(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
@@ -176,7 +171,6 @@ simt_gemm_kernel(const T* __restrict__ A, const T* __restrict__ Wt, int64_t M, i
       } else {
         epi.begin_row(row);
         epi.template apply<false>(row, n0, v, nvalid);
-        epi.end_row(row);
       }
     }
   }
@@ -234,7 +228,7 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   MMG_CHECK_ARG(a && a->a && a->w, "mmg_linear: NULL operand");
   MMG_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0, "mmg_linear: bad shape M=%lld N=%lld K=%lld", (long long)a->M, (long long)a->N, (long long)a->K);
   int rc = validate_epilogue(a->epilogue, a->epi, a->N); if (rc) return rc;
-  Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue; epi.fast = 0; epi.M = a->M; epi.N = a->N;
+  Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue;
   const bool tc_ok = a->dtype == MMG_BF16 && (a->K % 64 == 0) && (a->N % 64 == 0) && (a->lda % 8 == 0) && (a->ldw % 8 == 0) &&
                      aligned16(a->a) && aligned16(a->w) && (a->epi.ldo % 8 == 0 || a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_CONVT_RGB || a->epilogue == MMG_EPI_LFQ_IDS || a->epilogue == MMG_EPI_ARGMIN);
   if (!tc_ok) {
@@ -247,7 +241,7 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   p.skip_if_zero = skip_if_zero;
   p.M = a->M; p.N = a->N; p.num_kb = (int)(a->K / TC_BK); p.mode = 0;
   p.num_m_tiles = (int)((a->M + TC_BM - 1) / TC_BM);
-  p.epi = epi; p.epi.fast = 1;
+  p.epi = epi;
   uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda * 2}; uint32_t box[2] = {TC_BK, TC_BM};
   rc = make_tmap_bf16(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc;
   const int bn = pick_bn(p.num_m_tiles, a->N, a->epilogue);
@@ -285,7 +279,7 @@ extern "C" int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream) {
   p.num_m_tiles = (int)m_tiles;
   p.num_n_tiles = (int)(a->N / bn);
   p.n_fast = ((int64_t)a->N * a->K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;   // the bf16 product's tile order
-  p.epi.p = a->epi; p.epi.kind = a->epilogue; p.epi.fast = 1; p.epi.M = a->M; p.epi.N = a->N;
+  p.epi.p = a->epi; p.epi.kind = a->epilogue;
   p.a_scale = a->a_scale; p.w_scale = a->w_scale;
   { uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda}; uint32_t box[2] = {128, TC_BM};
     rc = make_tmap_u8(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc; }
@@ -306,7 +300,7 @@ extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
   const int64_t M = (int64_t)a->B * g.Ho * g.Wo, N = a->Cout, K = (int64_t)g.ntaps * a->Cin;
   MMG_CHECK_ARG(a->epilogue != MMG_EPI_GEGLU_TANH && a->epi.act != 2, "mmg_conv2d: GEGLU_TANH / ReLU epilogues are offered by mmg_linear only");
   int rc = validate_epilogue(a->epilogue, a->epi, N); if (rc) return rc;
-  Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue; epi.fast = 0; epi.M = M; epi.N = N;
+  Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue;
   TcGemmParams p{};
   const bool tc_ok = a->dtype == MMG_BF16 && a->kind != 3 && (a->Cin % 64 == 0) && (N % 64 == 0) && aligned16(a->x) && aligned16(a->w) &&
                      (a->epi.ldo % 8 == 0) && tile_geometry(g.Ho, g.Wo, &p) == 0;
@@ -317,7 +311,7 @@ extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
   p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 64; p.ntaps = g.ntaps; p.num_kb = p.ntaps * p.cchunks;
   p.Ho = g.Ho; p.Wo = g.Wo; p.B = a->B;
   p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
-  p.epi = epi; p.epi.fast = 1;
+  p.epi = epi;
   const uint64_t C = a->Cin, W = a->W, H = a->H;
   uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TB};
   if (a->kind != 2) {
@@ -400,7 +394,7 @@ extern "C" int mmg_conv2d_fp8(const mmg_conv2d_fp8_args* a, void* stream) {
   p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 128; p.ntaps = g.ntaps; p.num_kb = p.ntaps * p.cchunks;
   p.Ho = g.Ho; p.Wo = g.Wo; p.B = a->B;
   p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
-  p.epi.p = a->epi; p.epi.kind = a->epilogue; p.epi.fast = 1; p.epi.M = M; p.epi.N = N;
+  p.epi.p = a->epi; p.epi.kind = a->epilogue;
   p.a_scale = a->x_scale; p.w_scale = a->w_scale;
   rc = fp8_image_maps(p, a->x, a->B, a->H, a->W, a->Cin, a->kind == 2); if (rc) return rc;
   if (a->kind != 2) {
@@ -437,7 +431,7 @@ extern "C" int mmg_conv_transpose2d_fp8(const mmg_conv_transpose2d_fp8_args* a, 
   rc = fp8_image_maps(p, a->x, a->B, a->H, a->W, a->Cin, false); if (rc) return rc;
   for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
     TcGemmParams q = p;
-    q.epi.p = a->epi; q.epi.kind = a->epilogue; q.epi.fast = 1; q.epi.M = M; q.epi.N = N;
+    q.epi.p = a->epi; q.epi.kind = a->epilogue;
     q.epi.p.H = a->H; q.epi.p.W = a->W; q.epi.p.py = py; q.epi.p.px = px;
     q.w_scale = a->w_scale + (size_t)(py * 2 + px) * N;
     for (int t = 0; t < 4; ++t) { q.tap_map[t] = 0; q.tap_dy[t] = (int8_t)CT_D[py][t >> 1]; q.tap_dx[t] = (int8_t)CT_D[px][t & 1]; }
@@ -463,7 +457,7 @@ extern "C" int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* st
   const size_t esz = a->dtype == MMG_BF16 ? 2 : 4;
   if (!tc_ok && a->dtype == MMG_BF16) note_simt_fallback("mmg_conv_transpose2d", M, N, K);
   for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
-    Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue; epi.fast = 0; epi.M = M; epi.N = N;
+    Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue;
     epi.p.H = a->H; epi.p.W = a->W; epi.p.py = py; epi.p.px = px;
     const uint8_t* wp = reinterpret_cast<const uint8_t*>(a->w) + (size_t)(py * 2 + px) * N * K * esz;
     if (!tc_ok) {
@@ -476,7 +470,7 @@ extern "C" int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* st
     q.M = M; q.N = N; q.mode = 1; q.cchunks = a->Cin / 64; q.ntaps = 4; q.num_kb = 4 * q.cchunks;
     q.Ho = a->H; q.Wo = a->W; q.B = a->B;
     q.num_m_tiles = q.tiles_x * q.tiles_y * ((a->B + q.TB - 1) / q.TB);
-    q.epi = epi; q.epi.fast = 1;
+    q.epi = epi;
     const uint64_t C = a->Cin, W = a->W, H = a->H;
     uint64_t dims[4] = {C, W, H, (uint64_t)a->B}; uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
     uint32_t box[4] = {64, (uint32_t)q.TW, (uint32_t)q.TH, (uint32_t)q.TB};

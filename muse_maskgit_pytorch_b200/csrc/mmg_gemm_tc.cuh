@@ -5,9 +5,8 @@
 //   warps 4..11 : two consumer warpgroups.  Warpgroup g multiplies rows [64 g, 64 g + 64) of the tile (wgmma m64nBNk16, 4 per k-block,
 //                 accumulators in registers), then runs the fused Epilogue on those rows (EPI_MODE below): from the accumulator
 //                 registers into per-warp shared-memory boxes, then a TMA store / TMA reduction (tile epilogues) or one lane per row and
-//                 64-column chunk (TC_EPI_REGS); TC_EPI_ACT goes through a shared-memory staging buffer (128 columns at a time), where two
-//                 warps share a 32-row quarter and take alternate 64-column chunks.  setmaxnreg moves registers from warpgroup 0
-//                 (40/thread) to the consumers (232/thread).
+//                 64-column chunk (TC_EPI_REGS, TC_EPI_ACT).  setmaxnreg moves registers from warpgroup 0 (40/thread) to the consumers
+//                 (232/thread).
 //   persistent grid (<= #SM CTAs), static tile schedule (M- or N-fastest); the producer runs ahead into the next tile while the consumers
 //   finish the epilogue of the current one.
 //
@@ -26,7 +25,6 @@ constexpr int TC_BK = 64;
 constexpr int TC_THREADS = 384;          // warpgroup 0: warp 0 TMA (1-3 idle); warpgroups 1-2: wgmma + epilogue
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_MAX_TAPS = 16;
-constexpr int TC_STG_LD = 132;           // staging row stride (floats): 128 columns + 4, conflict-free 16-byte row reads
 constexpr int TC_SMEM_LIMIT = 227 * 1024;
 
 // How the epilogue's results leave the CTA (the EPI_MODE of tc_gemm_kernel; described above the kernel).  The launcher picks one per product.
@@ -36,12 +34,10 @@ enum TcEpiMode : int {
   TC_EPI_TSTORE = 3,    // plain fp32: per-warp tiles + TMA store
   TC_EPI_QKV = 4,       // QKV heads: per-warp tiles + TMA stores
   TC_EPI_GEGLU = 5,     // GEGLU, BN = 256: per-warp tiles + TMA store
-  TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: staging buffer, one thread per row
+  TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: TC_EPI_REGS's box, one lane per row
 };
-// the modes whose epilogue runs from the accumulator fragments through per-warp output boxes
+// the modes whose epilogue writes whole output boxes with TMA; the other two run an Epilogue kind on one row chunk per lane
 constexpr bool tc_tile_epilogue(int mode) { return mode != TC_EPI_REGS && mode != TC_EPI_ACT; }
-// the modes that keep the shared-memory staging buffer (and its shallower operand ring); every other mode uses the 32 KB of per-warp boxes
-constexpr bool tc_staged_epilogue(int mode) { return mode == TC_EPI_ACT; }
 
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
@@ -64,36 +60,30 @@ struct alignas(64) TcGemmParams {
   const float* w_scale;
 };
 
-// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][TC_EPI_ACT: staging, 2 x 64 x 132 fp32 | every other mode: per-warp
-// output boxes, 32 KB].  Without the staging buffer a kernel gets 4 operand stages at BN = 256 and 6 at BN <= 128 (TC_EPI_ACT, BN = 128:
-// 4); the 512 B static s_scale fits in what the 227 KB limit leaves over.
+// Shared memory: [<= 1 KB to align][operand ring][barriers, 1 KB][per-warp output boxes, 32 KB]: 4 operand stages at BN = 256 and 6 at
+// BN <= 128; the 512 B static s_scale fits in what the 227 KB limit leaves over.
 template <int BN> struct TcCfg {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;
   static constexpr int B_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STG_BYTES = 2 * 64 * TC_STG_LD * 4;
   static constexpr int TILE_BYTES = TC_EPI_WARPS * 4096;
-  static constexpr int stages(int extra) {
-    return (TC_SMEM_LIMIT - 1024 - 1024 - extra) / STAGE_BYTES < 6 ? (TC_SMEM_LIMIT - 1024 - 1024 - extra) / STAGE_BYTES : 6;
-  }
-  static constexpr int STAGES = stages(STG_BYTES);
-  static constexpr int STAGES_RED = stages(TILE_BYTES);
-  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 1024 + STG_BYTES;
-  static constexpr int SMEM_BYTES_RED = 1024 + STAGES_RED * STAGE_BYTES + 1024 + TILE_BYTES;
-  static_assert(STAGES >= 2 && STAGES_RED >= 2, "operand ring too shallow");
-  static_assert(SMEM_BYTES + 512 <= TC_SMEM_LIMIT && SMEM_BYTES_RED + 512 <= TC_SMEM_LIMIT, "dynamic + static shared memory over the opt-in limit");
+  static constexpr int FIT = (TC_SMEM_LIMIT - 1024 - 1024 - TILE_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = FIT < 6 ? FIT : 6;
+  static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 1024 + TILE_BYTES;
+  static_assert(STAGES >= 2, "operand ring too shallow");
+  static_assert(SMEM_BYTES + 512 <= TC_SMEM_LIMIT, "dynamic + static shared memory over the opt-in limit");
 };
 
-// The Epilogue kinds (mmg_epilogue.cuh) are written for one thread that owns a 64-column chunk of a row.  TC_EPI_ACT gets such chunks
-// through the staging buffer.  The tile epilogues need no such thing: each of their terms is elementwise, or (GEGLU) pairs column i with
-// column 32 + i, which the wgmma fragment keeps in the same thread.  They go from the accumulator registers straight into the warp's output
-// boxes, and the TMA engine writes the boxes out.  Thread t of a warpgroup (warp w, lane l) holds rows 16 w + l / 4 and + 8 at columns
-// 8 j + 2 (l % 4) and + 1, so a warp owns 16 whole rows; a box is 16 rows x 128 bytes (TMA 128-byte swizzle), and the warp's 4 KB tile
-// double-buffers two.  The launcher takes a tile epilogue only at a tile width BN that divides N, so every box lies inside the N columns.
-// TC_EPI_REGS uses the same 4 KB per warp as one fp32 box of its 16 rows x 64 columns: each 64-column chunk of the fragments goes into it,
-// and lane r < 16 reads row r back and runs the Epilogue kind on it, so every kind computes what it computes elsewhere, element for
-// element.  CONVT_RGB never forms a row: each thread projects its own fragment columns onto the (<= 4) RGB weights and two shuffles
-// finish the sum over the lane quad that shares a row.
+// The Epilogue kinds (mmg_epilogue.cuh) are written for one thread that owns a 64-column chunk of a row.  The tile epilogues need no
+// such thing: each of their terms is elementwise, or (GEGLU) pairs column i with column 32 + i, which the wgmma fragment keeps in the
+// same thread.  They go from the accumulator registers straight into the warp's output boxes, and the TMA engine writes the boxes out.
+// Thread t of a warpgroup (warp w, lane l) holds rows 16 w + l / 4 and + 8 at columns 8 j + 2 (l % 4) and + 1, so a warp owns 16 whole
+// rows; a box is 16 rows x 128 bytes (TMA 128-byte swizzle), and the warp's 4 KB tile double-buffers two.  The launcher takes a tile
+// epilogue only at a tile width BN that divides N, so every box lies inside the N columns.
+// TC_EPI_REGS and TC_EPI_ACT use the same 4 KB per warp as one fp32 box of its 16 rows x 64 columns: each 64-column chunk of the fragments
+// goes into it, and lane r < 16 reads row r back and runs the Epilogue kind on it (TC_EPI_ACT: apply_act), so every kind computes what it
+// computes elsewhere, element for element.  CONVT_RGB never forms a row: each thread projects its own fragment columns onto the (<= 4)
+// RGB weights and two shuffles finish the sum over the lane quad that shares a row.
 // TC_EPI_REDUCE: in-place residual epilogues (out == resid, fp32) push the term they add with a TMA reduction
 // (cp.reduce.async.bulk.tensor .add), 32 columns per box: the residual is never read and the adds happen in L2.
 // TC_EPI_TSTORE: plain fp32 outputs (no bias / activation; the logits GEMM) leave through the same boxes with a TMA store.
@@ -153,12 +143,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   constexpr bool ACTT = EPI_MODE == TC_EPI_ACT;
   constexpr bool TILES = tc_tile_epilogue(EPI_MODE);
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
-  constexpr int STAGES = tc_staged_epilogue(EPI_MODE) ? Cfg::STAGES : Cfg::STAGES_RED;
+  constexpr int STAGES = Cfg::STAGES;
   constexpr int STAGE_BYTES = Cfg::STAGE_BYTES;
-  constexpr int ROUNDS = (BN + 127) / 128;
-  // residual rows are fetched one chunk ahead (the first one during the main loop) only at BN <= 128: at BN = 256 the 128 accumulator
-  // registers leave no room for a 64-register residual buffer next to them, so each chunk loads its residual when it needs it
-  constexpr bool EARLY_RESID = BN <= 128;
 
   if (p.skip_if_zero) { pdl_wait(); if (*p.skip_if_zero == 0) return; }       // uniform over the grid: nothing has been set up yet
 
@@ -166,8 +152,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint8_t* tiles = smem + STAGES * STAGE_BYTES + 1024;      // tile epilogues: per-warp output tiles
-  float* staging = reinterpret_cast<float*>(tiles);         // register epilogues: staging buffer
+  uint8_t* tiles = smem + STAGES * STAGE_BYTES + 1024;      // per-warp output boxes, 4 KB each
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
@@ -220,14 +205,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     // ===================== consumer warpgroups: wgmma main loop, then the epilogue of their 64 rows =====================
     const int wg = (warp - 4) >> 2, wq = warp & 3;
-    const int quarter = 2 * wg + (wq & 1);        // this warp's 32 rows of the tile, inside its warpgroup's 64
-    const int half = wq >> 1;                     // 0: even 64-column chunks, 1: odd chunks
-    const int r_in_tile = quarter * 32 + lane;
-    float* stg = staging + wg * 64 * TC_STG_LD;
-    const float* my_row = stg + ((wq & 1) * 32 + lane) * TC_STG_LD;
     Epilogue epi = p.epi;
     if (epi.kind == MMG_EPI_QKV) { epi.p.q_scale = s_scale; epi.p.k_scale = s_scale + 64; }
-    const bool whole_row = (epi.kind == MMG_EPI_CONVT_RGB);      // needs every chunk of a row in one thread
     const bool prefetch_resid = epi.can_prefetch_resid();
     const uint32_t wtile = smem_u32(tiles) + (uint32_t)(warp - 4) * 4096u;   // tile epilogues: this warp's two 2 KB output boxes
     uint32_t nbox = 0;                                                         // boxes this warp has filled so far
@@ -237,22 +216,6 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int tile = tile0; tile < num_tiles; tile += tile_step) {
       const int m_blk = p.n_fast ? tile / p.num_n_tiles : tile % p.num_m_tiles, n_blk = p.n_fast ? tile % p.num_n_tiles : tile / p.num_m_tiles;
-      int64_t row; bool valid;
-      if (p.mode == 0) {
-        row = (int64_t)m_blk * TC_BM + r_in_tile; valid = row < p.M;
-      } else {
-        const int xt = m_blk % p.tiles_x, yt = (m_blk / p.tiles_x) % p.tiles_y, bt = m_blk / (p.tiles_x * p.tiles_y);
-        const int tx = r_in_tile % p.TW, ty = (r_in_tile / p.TW) % p.TH, tb = r_in_tile / (p.TW * p.TH);
-        const int b = bt * p.TB + tb;
-        valid = b < p.B;
-        row = ((int64_t)b * p.Ho + (yt * p.TH + ty)) * p.Wo + xt * p.TW + tx;
-      }
-      const bool mine = !whole_row || half == 0;
-      const int c_first = whole_row ? 0 : half, c_step = whole_row ? 1 : 2, c_end = BN / 64;
-      const bool pre = EARLY_RESID && ACTT && prefetch_resid && valid && mine && (n_blk * BN + c_first * 64 < p.N) && c_first < BN / 64;
-      float rbuf[64];
-      if (pre) epi.load_resid(row, n_blk * BN + c_first * 64, rbuf);      // in flight during the main loop
-      if (ACTT && valid && mine) epi.begin_row(row);                       // row geometry / folded-LayerNorm statistics: independent of the accumulator
       // tile epilogues: the warp's 16 fragment rows start at brow; LNFOLD statistics of row brow + l / 4 + 8 (l % 4) in lanes l % 4 < 2
       const int64_t brow = (int64_t)m_blk * TC_BM + wg * 64 + 16 * wq;
       float ln_a = 0.f, ln_b = 0.f;
@@ -451,8 +414,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
             }
           }
         }
-      } else if constexpr (!ACTT) {
-        // ---- TC_EPI_REGS, from the accumulator fragments (layout above the kernel) ----
+      } else {
+        // ---- TC_EPI_REGS and TC_EPI_ACT, from the accumulator fragments (layout above the kernel) ----
         const int r0 = wg * 64 + 16 * wq;                          // the warp's 16 rows of the tile
         if constexpr (FP8_CONV) dequant_acc_images<BN>(acc, p, m_blk, r0, n_blk * BN, lane);
         const int q = lane & 3, fr = lane >> 2;
@@ -464,7 +427,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
           orow = ((int64_t)b * p.Ho + (yt * p.TH + ty)) * p.Wo + xt * p.TW + tx;
           return b < p.B;
         };
-        if (epi.kind == MMG_EPI_CONVT_RGB) {
+        if (!ACTT && epi.kind == MMG_EPI_CONVT_RGB) {
           // bias + LeakyReLU per element, then the <= 4 channel dot products over this thread's BN / 4 columns of rows fr and fr + 8, and
           // over the lane quad (shfl.xor 1, 2).  The launcher gives CONVT_RGB one tile of BN = N columns, so n_blk == 0 and every column
           // is valid.  Lane q = 0 writes row fr's pixel, lane q = 1 row fr + 8's (NCHW fp32).
@@ -529,7 +492,9 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
               for (int k = 0; k < 16; ++k)
                 asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[4 * k]), "=f"(v[4 * k + 1]), "=f"(v[4 * k + 2]), "=f"(v[4 * k + 3])
                              : "r"(box + (uint32_t)lane * 256u + (uint32_t)((k ^ (lane & 7)) * 16)) : "memory");
-              if (prefetch_resid) {
+              if constexpr (ACTT) {
+                epi.apply_act(orow, col0, v, 64);
+              } else if (prefetch_resid) {
                 float r[64];
                 epi.load_resid(orow, col0, r);
                 epi.fuse_resid(col0, v, r);
@@ -540,41 +505,6 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
             }
           }
         }
-      } else {
-        // ---- TC_EPI_ACT: columns [128 rd, 128 rd + 128) of the warpgroup's 64 rows -> staging -> one row per thread ----
-        // the epilogue of one 64-column accumulator chunk held in v
-        auto chunk = [&](const int c, float (&v)[64]) {
-          const int col0 = n_blk * BN + c * 64;
-          if (ACTT) {
-            if (valid && col0 < p.N) epi.apply_act(row, col0, v, 64);
-          } else if (valid && col0 < p.N) {
-            if (prefetch_resid) {
-              if (!EARLY_RESID) epi.load_resid(row, col0, rbuf);
-              epi.fuse_resid(col0, v, rbuf);
-              const int cn = col0 + c_step * 64;
-              if (EARLY_RESID && c + c_step < BN / 64 && cn < p.N) epi.load_resid(row, cn, rbuf);   // next chunk's residual overlaps the stores
-              epi.store_f32(row, col0, v);
-            } else {
-              epi.template apply<true>(row, col0, v, 64);
-            }
-          }
-        };
-#pragma unroll
-        for (int rd = 0; rd < ROUNDS; ++rd) {
-          named_sync(1 + wg, 128);                   // the previous round's (tile's) readers are done with the staging buffer
-          stage_acc<BN / 2, TC_STG_LD>(acc, stg, 128 * rd, BN - 128 * rd < 128 ? BN - 128 * rd : 128);
-          named_sync(1 + wg, 128);
-#pragma unroll 1
-          for (int c = c_first; c < c_end; c += c_step) {
-            if (!mine) break;
-            if ((c >> 1) != rd) continue;
-            float v[64];
-            stage_ld32(my_row + (c & 1) * 64, v);
-            stage_ld32(my_row + (c & 1) * 64 + 32, v + 32);
-            chunk(c, v);
-          }
-        }
-        if (valid && mine) epi.end_row(row);
       }
     }
   }

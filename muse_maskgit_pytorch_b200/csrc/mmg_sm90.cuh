@@ -256,7 +256,8 @@ template <int R> __device__ __forceinline__ void reg_fence(float (&d)[R]) {
 }
 
 // Accumulator columns [c0, c0 + ncols) of a 64 x N wgmma tile -> rows of a row-major fp32 staging buffer `stg` (row stride LD floats):
-// the hand-over from the fragment layout to the one-thread-per-row epilogues and softmax loops.  ncols % 8 == 0, c0 % 8 == 0.
+// the hand-over from the fragment layout to the one-thread-per-row softmax and output loops of the T5 and split-precision attention
+// kernels.  ncols % 8 == 0, c0 % 8 == 0.
 template <int R, int LD> __device__ __forceinline__ void stage_acc(const float (&d)[R], float* stg, int c0, int ncols) {
   const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
   const int r0 = 16 * w + (l >> 2), cq = 2 * (l & 3);
