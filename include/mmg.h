@@ -76,6 +76,10 @@ enum mmg_epilogue {
                              all-ones by the caller, updated with atomicMin( orderkey(||e||^2 - 2 x.e) << 32 | k ): lowest k on ties */
   MMG_EPI_GEGLU_TANH = 10,/* GEGLU interleave (blocks of 32: [x(32) | gate(32)]), no bias, tanh-approximated GELU ("gelu_new" of T5 v1.1,
                              t5.py): out[r, c/2] = gelu_tanh(x) * gate; mmg_linear only                                        */
+  MMG_EPI_QKV128     = 11,/* QKV with 128-column heads: the fields of MMG_EPI_QKV, with N = (nq+nk+nv)*128, q_scale / k_scale [128],
+                             null_k / null_v [heads, 128], q_out [BH, q_rows, 128], k_out / v_out [BH, kv_rows, 128].  wgmma path only
+                             (mmg_linear with bf16 operands that it takes, mmg_linear_fp8): any call that would run on the CUDA-core
+                             kernel returns MMG_EINVAL and launches nothing                                                    */
 };
 
 typedef struct {
@@ -293,6 +297,11 @@ typedef struct {
                               (384 bf16 columns per row: q with side 0, k and v with side 1), out is fp32; exact two-pass softmax.      */
 } mmg_attention_args;
 int mmg_attention(const mmg_attention_args* a, void* stream);
+/* The same attention for 128-wide heads: q [BH, Tq, 128], k / v [BH, Tk_alloc, 128] (MMG_EPI_QKV128 outputs), out rows
+ * out[b, t, h*128 : (h+1)*128]; the same argument block, same key-mask, null-key, Tk_alloc and logit_bound conventions.
+ * MMG_BF16 with 16-byte aligned q / k / v / out, ldo % 8 == 0 and 2 <= Tk <= 4096 runs the wgmma kernel; fp32, and any other bf16
+ * call, the CUDA-core kernel.  split3 must be 0 (no split-precision kernel at this width: fp32 runs on the CUDA cores).           */
+int mmg_attention_d128(const mmg_attention_args* a, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sampler.  replaces muse_maskgit_pytorch.py:556-609 (the per-step tail of MaskGit.generate).

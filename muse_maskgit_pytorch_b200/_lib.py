@@ -8,7 +8,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MMG_LIB") or os.path.join(_HERE, "libmmg.so")     # MMG_LIB: an alternative build of the library
 
 F32, BF16, E4M3 = 0, 1, 2
-EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB, EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH = range(11)
+EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB, EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH, \
+    EPI_QKV128 = range(12)
 
 vp, i32, i64, f32, u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64
 
@@ -194,7 +195,7 @@ class RmsNormArgs(C.Structure):
 EXPORTS = {
     "mmg_linear": LinearArgs, "mmg_conv2d": Conv2dArgs, "mmg_conv_transpose2d": ConvTranspose2dArgs,
     "mmg_conv_in": ConvInArgs, "mmg_groupnorm": GroupNormArgs, "mmg_layernorm": LayerNormArgs, "mmg_embed": EmbedArgs,
-    "mmg_attention": AttentionArgs, "mmg_remask": RemaskArgs, "mmg_final_embed": FinalEmbedArgs,
+    "mmg_attention": AttentionArgs, "mmg_attention_d128": AttentionArgs, "mmg_remask": RemaskArgs, "mmg_final_embed": FinalEmbedArgs,
     "mmg_logits_sample": LogitsSampleArgs, "mmg_vq_lfq_encode": LfqEncodeArgs, "mmg_vq_l2_argmin": L2ArgminArgs,
     "mmg_vq_decode_codes": DecodeCodesArgs, "mmg_cast": CastArgs, "mmg_split3": Split3Args, "mmg_critic_score": CriticScoreArgs,
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,

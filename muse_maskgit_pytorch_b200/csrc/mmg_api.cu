@@ -16,6 +16,7 @@ extern "C" int mmg_sizeof(const char* name) {
   SZ(t5_attention); SZ(rmsnorm); SZ(remask_frozen); SZ(edit_select); SZ(logits_xent); SZ(logits_xent_rows); SZ(linear_fp8); SZ(layernorm_fp8);
   SZ(conv2d_fp8); SZ(conv_transpose2d_fp8); SZ(quantize_e4m3_images);
 #undef SZ
+  if (!strcmp(name, "mmg_attention_d128")) return (int)sizeof(mmg_attention_args);
   if (!strcmp(name, "mmg_epilogue")) return (int)sizeof(mmg_epilogue_args);
   if (!strcmp(name, "mmg_attn_weights")) return (int)sizeof(mmg_attn_weights);
   if (!strcmp(name, "mmg_layer_weights")) return (int)sizeof(mmg_layer_weights);

@@ -362,6 +362,13 @@ inline int validate_epilogue(int kind, const mmg_epilogue_args& e, int64_t N) {
       MMG_CHECK_ARG(aligned16_host(e.q_out) && aligned16_host(e.k_out) && aligned16_host(e.v_out) && aligned16_host(e.null_k) && aligned16_host(e.null_v),
                     "epilogue QKV: q / k / v outputs and null rows must be 16-byte aligned");
       break;
+    case MMG_EPI_QKV128:
+      MMG_CHECK_ARG((N % 128) == 0 && N / 128 == e.nq_heads + e.nk_heads + e.nv_heads, "epilogue QKV128: N != 128*(nq+nk+nv)");
+      MMG_CHECK_ARG(e.tokens > 0 && e.heads > 0 && e.out_dtype >= MMG_F32 && e.out_dtype <= MMG_BF16, "epilogue QKV128: tokens/heads/out_dtype");
+      MMG_CHECK_ARG((!e.nq_heads || (e.q_out && e.q_scale)) && (!e.nk_heads || (e.k_out && e.k_scale)) && (!e.nv_heads || e.v_out), "epilogue QKV128: NULL output");
+      MMG_CHECK_ARG(aligned16_host(e.q_out) && aligned16_host(e.k_out) && aligned16_host(e.v_out) && aligned16_host(e.null_k) && aligned16_host(e.null_v) &&
+                    aligned16_host(e.q_scale) && aligned16_host(e.k_scale), "epilogue QKV128: q / k / v outputs, null rows and scales must be 16-byte aligned");
+      break;
     case MMG_EPI_CONVT: MMG_CHECK_ARG(e.out && e.H > 0 && e.W > 0, "epilogue CONVT: geometry"); break;
     case MMG_EPI_CONVT_RGB: MMG_CHECK_ARG(e.out && e.rgb_w && e.rgb_b && e.rgb_channels >= 1 && e.rgb_channels <= 4, "epilogue CONVT_RGB: args"); break;
     default: return fail(MMG_EINVAL, "unknown epilogue %d", kind);

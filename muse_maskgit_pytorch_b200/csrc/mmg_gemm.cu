@@ -36,12 +36,12 @@ static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
 static int bf16_out_maps(TcGemmParams& p, int epi_mode) {
   const mmg_epilogue_args& e = p.epi.p;
   int rc = MMG_OK;
-  if (epi_mode == TC_EPI_QKV) {
-    const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads;
-    uint64_t str[1] = {128}; uint32_t box[2] = {64, 16};
-    if (e.nq_heads) { uint64_t d[2] = {64, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
+  if (epi_mode == TC_EPI_QKV || epi_mode == TC_EPI_QKV128) {
+    const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads, hd = epi_mode == TC_EPI_QKV ? 64 : 128;
+    uint64_t str[1] = {hd * 2}; uint32_t box[2] = {64, 16};
+    if (e.nq_heads) { uint64_t d[2] = {hd, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
     if (e.nk_heads) {
-      uint64_t d[2] = {64, seqs * (uint64_t)e.kv_rows};
+      uint64_t d[2] = {hd, seqs * (uint64_t)e.kv_rows};
       rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
       rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
     }
@@ -52,8 +52,28 @@ static int bf16_out_maps(TcGemmParams& p, int epi_mode) {
   return rc;
 }
 
+// QKV128 on the tile epilogue: bf16 heads, whole 16-token boxes of one sequence (the conditions of TC_EPI_QKV)
+static bool qkv128_tiles(const TcGemmParams& p) {
+  const mmg_epilogue_args& e = p.epi.p;
+  return e.out_dtype == MMG_BF16 && p.mode == 0 && e.tokens % 32 == 0 && p.M % 128 == 0 && e.nk_heads == e.nv_heads &&
+         (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out)));
+}
+
 static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
   const mmg_epilogue_args& e = p.epi.p;
+  if (p.epi.kind == MMG_EPI_QKV128) {
+    // whole heads per tile: BN = 256 or 128 on the tile epilogue, 128 (64 accumulators per thread) on the fragment stores
+    MMG_CHECK_ARG(p.mode == 0, "QKV128: dense products only");
+    const bool tiles = qkv128_tiles(p);
+    bn = tiles && bn == 256 ? 256 : 128;
+    p.num_n_tiles = (int)(N / bn);
+    p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
+    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
+    int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
+    if (!tiles) return launch_tc<128, TC_EPI_QKV128_REGS>(p, st);
+    rc = bf16_out_maps(p, TC_EPI_QKV128); if (rc) return rc;
+    return bn == 256 ? launch_tc<256, TC_EPI_QKV128>(p, st) : launch_tc<128, TC_EPI_QKV128>(p, st);
+  }
   const bool in_place = (p.epi.kind == MMG_EPI_LNFOLD_RESIDUAL || (p.epi.kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
                         e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && p.mode == 0;
   const bool plain_f32 = p.epi.kind == MMG_EPI_STORE && e.out_dtype == MMG_F32 && p.mode == 0 && !e.bias && e.act == 0 && (e.ldo % 4) == 0 && aligned16(e.out);
@@ -180,6 +200,7 @@ template <bool CONV>
 static int launch_simt(int dtype, const void* a, const void* w, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldw,
                        const ConvGeom& g, const Epilogue& epi, cudaStream_t st) {
   MMG_CHECK_ARG(epi.kind != MMG_EPI_CONVT_RGB, "CONVT_RGB epilogue requires the bf16 tensor-core path");
+  MMG_CHECK_ARG(epi.kind != MMG_EPI_QKV128, "QKV128 epilogue requires the wgmma path of mmg_linear");
   MMG_CHECK_ARG(M > 0 && N > 0 && K > 0, "empty GEMM");
   dim3 grid((unsigned)((M + 63) / 64), (unsigned)((N + 63) / 64));
   MMG_CHECK_ARG(grid.y < 65536, "N too large for the fp32 path");
@@ -230,7 +251,10 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   int rc = validate_epilogue(a->epilogue, a->epi, a->N); if (rc) return rc;
   Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue;
   const bool tc_ok = a->dtype == MMG_BF16 && (a->K % 64 == 0) && (a->N % 64 == 0) && (a->lda % 8 == 0) && (a->ldw % 8 == 0) &&
-                     aligned16(a->a) && aligned16(a->w) && (a->epi.ldo % 8 == 0 || a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_CONVT_RGB || a->epilogue == MMG_EPI_LFQ_IDS || a->epilogue == MMG_EPI_ARGMIN);
+                     aligned16(a->a) && aligned16(a->w) && (a->epi.ldo % 8 == 0 || a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_QKV128 ||
+                                                             a->epilogue == MMG_EPI_CONVT_RGB || a->epilogue == MMG_EPI_LFQ_IDS || a->epilogue == MMG_EPI_ARGMIN);
+  // QKV128 has no CUDA-core epilogue: bf16 operands with K % 64 == 0, 8-element rows and 16-byte aligned a / w, or nothing
+  MMG_CHECK_ARG(tc_ok || a->epilogue != MMG_EPI_QKV128, "mmg_linear: QKV128 needs the wgmma path (bf16, K %% 64 == 0, lda / ldw %% 8 == 0, aligned a / w)");
   if (!tc_ok) {
     MMG_CHECK_ARG(!skip_if_zero, "skippable GEMM requires the bf16 tensor-core path");
     if (a->dtype == MMG_BF16) note_simt_fallback("mmg_linear", a->M, a->N, a->K);
@@ -258,18 +282,18 @@ extern "C" int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream) {
                 (long long)a->M, (long long)a->N, (long long)a->K);
   MMG_CHECK_ARG(a->lda >= a->K && a->ldw >= a->K && a->lda % 16 == 0 && a->ldw % 16 == 0 && aligned16(a->a) && aligned16(a->w) &&
                 (reinterpret_cast<uintptr_t>(a->w_scale) & 7) == 0, "mmg_linear_fp8: operands need 16-byte rows, w_scale 8-byte alignment");
-  MMG_CHECK_ARG(a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_GEGLU, "mmg_linear_fp8: epilogue %d (QKV or GEGLU only)", a->epilogue);
+  MMG_CHECK_ARG(a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_QKV128 || a->epilogue == MMG_EPI_GEGLU, "mmg_linear_fp8: epilogue %d (QKV or GEGLU only, or QKV128)", a->epilogue);
   int rc = validate_epilogue(a->epilogue, a->epi, a->N); if (rc) return rc;
   const mmg_epilogue_args& e = a->epi;
   const int64_t m_tiles = (a->M + TC_BM - 1) / TC_BM;
   int bn = 256, epi_mode = TC_EPI_GEGLU;
-  if (a->epilogue == MMG_EPI_QKV) {
+  if (a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_QKV128) {
     MMG_CHECK_ARG(e.out_dtype == MMG_BF16 && e.tokens > 0 && e.tokens % 32 == 0 && a->M % 128 == 0 && a->N % 128 == 0 && e.nk_heads == e.nv_heads &&
                   (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out))),
                   "mmg_linear_fp8: QKV needs bf16 outputs, tokens %% 32 == 0, M %% 128 == 0, N %% 128 == 0 (M=%lld N=%lld tokens=%d)",
                   (long long)a->M, (long long)a->N, e.tokens);
     bn = pick_bn(m_tiles, a->N, a->epilogue) == 256 ? 256 : 128;
-    epi_mode = TC_EPI_QKV;
+    epi_mode = a->epilogue == MMG_EPI_QKV ? TC_EPI_QKV : TC_EPI_QKV128;
   } else {
     MMG_CHECK_ARG(e.out_dtype == MMG_BF16 && a->N % 256 == 0 && e.ldo % 8 == 0 && aligned16(e.out),
                   "mmg_linear_fp8: GEGLU needs bf16 out, N %% 256 == 0, ldo %% 8 == 0 (N=%lld)", (long long)a->N);
@@ -287,6 +311,7 @@ extern "C" int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream) {
     rc = make_tmap_u8(&p.tma_b, a->w, 2, dims, str, box); if (rc) return rc; }
   rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
   if (epi_mode == TC_EPI_GEGLU) return launch_tc<256, TC_EPI_GEGLU, fp8e4>(p, st);
+  if (epi_mode == TC_EPI_QKV128) return bn == 256 ? launch_tc<256, TC_EPI_QKV128, fp8e4>(p, st) : launch_tc<128, TC_EPI_QKV128, fp8e4>(p, st);
   return bn == 256 ? launch_tc<256, TC_EPI_QKV, fp8e4>(p, st) : launch_tc<128, TC_EPI_QKV, fp8e4>(p, st);
 }
 

@@ -35,15 +35,19 @@ enum TcEpiMode : int {
   TC_EPI_QKV = 4,       // QKV heads: per-warp tiles + TMA stores
   TC_EPI_GEGLU = 5,     // GEGLU, BN = 256: per-warp tiles + TMA store
   TC_EPI_ACT = 6,       // T5 feed-forward epilogues (GEGLU_TANH, STORE + ReLU), BN = 128: TC_EPI_REGS's box, one lane per row
+  TC_EPI_QKV128 = 7,    // QKV with 128-column heads (bf16, TC_EPI_QKV's conditions): per-warp tiles + TMA stores, two boxes per head
+  TC_EPI_QKV128_REGS = 8,   // QKV with 128-column heads, any other call (fp32 out, tokens % 32 != 0, M % 128 != 0), BN = 128: stores
+                            // straight from the fragments
 };
-// the modes whose epilogue writes whole output boxes with TMA; the other two run an Epilogue kind on one row chunk per lane
-constexpr bool tc_tile_epilogue(int mode) { return mode != TC_EPI_REGS && mode != TC_EPI_ACT; }
+// the modes whose epilogue writes whole output boxes with TMA; the others run an Epilogue kind on one row chunk per lane, or (QKV128_REGS)
+// store from the fragments
+constexpr bool tc_tile_epilogue(int mode) { return mode != TC_EPI_REGS && mode != TC_EPI_ACT && mode != TC_EPI_QKV128_REGS; }
 
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
   CUtensorMap tma_b;
   CUtensorMap tma_out;      // REDUCE / TSTORE: the fp32 output [M, N] in boxes of 16 rows x 32 columns (128 B), SWIZZLE_128B; GEGLU: bf16 [M, N/2], 16 x 64
-  CUtensorMap tma_qkv[3];   // QKV: q / k / v as [rows, 64] bf16 matrices in boxes of 16 rows x 64 columns (128 B)
+  CUtensorMap tma_qkv[3];   // QKV: q / k / v as [rows, 64] bf16 matrices in boxes of 16 rows x 64 columns (128 B); QKV128: [rows, 128], same boxes
   int64_t M, N;
   int num_kb, num_m_tiles, num_n_tiles;
   int mode;                 // 0 dense, 1 conv (4-D A maps)
@@ -125,6 +129,50 @@ __device__ __forceinline__ void dequant_acc_images(float (&acc)[BN / 2], const T
   }
 }
 
+// QKV128: F.normalize * scale of the 128-column head at fragment groups j0 .. j0 + 15 (columns 8 jj + 2 q + e of rows fr and fr + 8), in
+// place.  The quad of lanes that shares a row holds the whole row: four fma chains per row over the thread's 32 values, then shfl.xor 1
+// and 2 (every lane of the quad ends with the same sum).  scale: q_scale / k_scale [128] in global memory (read through the L1).
+template <int BN>
+__device__ __forceinline__ void qkv128_normalise(float (&acc)[BN / 2], int j0, const float* __restrict__ scale, int q) {
+  float sa[4] = {0.f, 0.f, 0.f, 0.f}, sb[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const float x = acc[4 * (j0 + jj) + e], y = acc[4 * (j0 + jj) + 2 + e];
+      sa[2 * (jj & 1) + e] = fmaf(x, x, sa[2 * (jj & 1) + e]);
+      sb[2 * (jj & 1) + e] = fmaf(y, y, sb[2 * (jj & 1) + e]);
+    }
+  float ssa = (sa[0] + sa[1]) + (sa[2] + sa[3]), ssb = (sb[0] + sb[1]) + (sb[2] + sb[3]);
+  ssa += __shfl_xor_sync(0xffffffffu, ssa, 1); ssb += __shfl_xor_sync(0xffffffffu, ssb, 1);
+  ssa += __shfl_xor_sync(0xffffffffu, ssa, 2); ssb += __shfl_xor_sync(0xffffffffu, ssb, 2);
+  const float ia = rsqrtf(fmaxf(ssa, 1e-24f)), ib = rsqrtf(fmaxf(ssb, 1e-24f));
+#pragma unroll
+  for (int jj = 0; jj < 16; ++jj) {
+    const float2 sv = __ldg(reinterpret_cast<const float2*>(scale + 8 * jj + 2 * q));
+    acc[4 * (j0 + jj)] *= ia * sv.x; acc[4 * (j0 + jj) + 1] *= ia * sv.y;
+    acc[4 * (j0 + jj) + 2] *= ib * sv.x; acc[4 * (j0 + jj) + 3] *= ib * sv.y;
+  }
+}
+
+// QKV128: which output the 128-column head chunk at accumulator column col0 belongs to (0 q, 1 k, 2 v) and its head
+__device__ __forceinline__ int qkv128_head(const mmg_epilogue_args& e, int col0, int& h) {
+  const int hc = col0 >> 7;
+  const int which = hc < e.nq_heads ? 0 : (hc < e.nq_heads + e.nk_heads ? 1 : 2);
+  h = which == 0 ? hc : (which == 1 ? hc - e.nq_heads : hc - e.nq_heads - e.nk_heads);
+  return which;
+}
+
+// QKV128: the learned null key / value [heads, 128] -> key row 0 of (b, h) (muse_maskgit_pytorch.py:145-149)
+__device__ __forceinline__ void qkv128_null_row(const mmg_epilogue_args& e, int which, int64_t b, int h) {
+  const void* nsrc = which == 1 ? e.null_k : e.null_v;
+  if (!nsrc) return;
+  const size_t esz = e.out_dtype == MMG_BF16 ? 2 : 4;
+  const uint4* sp = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(nsrc) + (size_t)h * 128 * esz);
+  uint4* dp = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(which == 1 ? e.k_out : e.v_out) + (size_t)(b * e.heads + h) * e.kv_rows * 128 * esz);
+  for (int i = 0; i < (int)(128 * esz / 16); ++i) dp[i] = sp[i];
+}
+
 template <int BN, int EPI_MODE, typename TA = bf16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
@@ -132,7 +180,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   using Cfg = TcCfg<BN>;
   constexpr bool FP8 = sizeof(TA) == 1;
   constexpr int BK = 128 / (int)sizeof(TA);           // elements per k-block: one 128-byte row
-  static_assert(!FP8 || EPI_MODE == TC_EPI_QKV || EPI_MODE == TC_EPI_GEGLU || EPI_MODE == TC_EPI_REGS,
+  static_assert(!FP8 || EPI_MODE == TC_EPI_QKV || EPI_MODE == TC_EPI_QKV128 || EPI_MODE == TC_EPI_GEGLU || EPI_MODE == TC_EPI_REGS,
                 "e4m3 operands are dequantised by the QKV / GEGLU tile epilogues (dense) or the register epilogues (convolutions) only");
   // e4m3 convolutions: a k-block is one tap x 128 channels.  The dense e4m3 instantiations never run mode 1 and keep the bf16 channel step.
   constexpr bool FP8_CONV = FP8 && EPI_MODE == TC_EPI_REGS;
@@ -141,6 +189,7 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
   constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
   constexpr bool ACTT = EPI_MODE == TC_EPI_ACT;
+  static_assert((EPI_MODE != TC_EPI_QKV128 || BN >= 128) && (EPI_MODE != TC_EPI_QKV128_REGS || BN == 128), "QKV128: whole heads per tile");
   constexpr bool TILES = tc_tile_epilogue(EPI_MODE);
   static_assert(!GEGLUT || BN == 256, "the GEGLU tile epilogue pairs adjacent 64-column chunks of a 256-column tile");
   constexpr int STAGES = Cfg::STAGES;
@@ -412,6 +461,57 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
               bulk_commit();
               if (which != 0 && t0 == 0) epi.qkv_null_row(which, bq, h);
             }
+          }
+        } else if constexpr (EPI_MODE == TC_EPI_QKV128) {
+          const uint32_t rw = (uint32_t)brow, tok = (uint32_t)epi.p.tokens;
+          const uint32_t bq = rw / tok, t0 = rw - bq * tok;   // warp-uniform: the 16 rows are tokens t0 .. t0+15 of sequence bq
+#pragma unroll
+          for (int c = 0; c < BN / 128; ++c) {                // one head = two boxes of 64 columns
+            int h;
+            const int which = qkv128_head(epi.p, n_blk * BN + 128 * c, h);
+            if (which != 2) qkv128_normalise<BN>(acc, 16 * c, which == 0 ? epi.p.q_scale : epi.p.k_scale, q);
+            const int64_t drow = which == 0 ? ((int64_t)bq * epi.p.heads + h) * epi.p.q_rows + t0
+                                            : ((int64_t)bq * epi.p.heads + h) * epi.p.kv_rows + epi.p.key_off + t0;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const uint32_t box = box_begin();
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int j = 16 * c + 8 * hh + jj;
+                const uint32_t off = (uint32_t)((jj ^ fr) * 16 + 4 * q);
+                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowa + off), "r"(pack_bf16(acc[4 * j], acc[4 * j + 1])) : "memory");
+                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowb + off), "r"(pack_bf16(acc[4 * j + 2], acc[4 * j + 3])) : "memory");
+              }
+              box_ready();
+              if (lane == 0) { tma_store_2d(&p.tma_qkv[which], box, 64 * hh, (int)drow); bulk_commit(); }
+            }
+            if (lane == 0 && which != 0 && t0 == 0) qkv128_null_row(epi.p, which, bq, h);
+          }
+        }
+      } else if constexpr (EPI_MODE == TC_EPI_QKV128_REGS) {
+        // ---- QKV128 off the tile path: normalise on the fragments, then each thread stores its own column pairs of rows fr and fr + 8
+        // (rows past M are never stored); the thread of quad lane 0 that holds token 0 of a sequence writes the null row ----
+        const int q = lane & 3, fr = lane >> 2;
+        const mmg_epilogue_args& e = epi.p;
+        const int64_t row0 = (int64_t)m_blk * TC_BM + wg * 64 + 16 * wq + fr;
+        int h;
+        const int which = qkv128_head(e, n_blk * BN, h);
+        if (which != 2) qkv128_normalise<BN>(acc, 0, which == 0 ? e.q_scale : e.k_scale, q);
+        void* dst = which == 0 ? e.q_out : (which == 1 ? e.k_out : e.v_out);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int64_t row = row0 + 8 * rr;
+          if (row < p.M) {
+            const int64_t b = row / e.tokens, t = row - b * e.tokens;
+            const int64_t off = (which == 0 ? ((b * e.heads + h) * (int64_t)e.q_rows + t) : ((b * e.heads + h) * (int64_t)e.kv_rows + e.key_off + t)) * 128;
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj) {
+              const int col = 8 * jj + 2 * q;
+              const float v0 = acc[4 * jj + 2 * rr], v1 = acc[4 * jj + 2 * rr + 1];
+              if (e.out_dtype == MMG_BF16) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(dst) + off + col) = pack_bf16(v0, v1);
+              else *reinterpret_cast<float2*>(reinterpret_cast<float*>(dst) + off + col) = make_float2(v0, v1);
+            }
+            if (q == 0 && t == 0 && which != 0) qkv128_null_row(e, which, b, h);
           }
         }
       } else {

@@ -86,9 +86,12 @@ class Attention(nn.Module):
 class TransformerBlocks(nn.Module):
     def __init__(self, *, dim, depth, dim_head=64, heads=8, ff_mult=4, flash=True):
         super().__init__()
-        assert dim_head == 64, ("dim_head must be 64 here: the wgmma attention kernel (one 128-byte swizzled row per head "
-                                "vector) and the QKV epilogue are specialised for the head size every Muse config uses; the reference accepts "
-                                "any value (muse_maskgit_pytorch.py:95-110, 164-172)")
+        if dim_head not in (64, 128):
+            raise ValueError(f"dim_head must be 64 or 128 here (got {dim_head}): the QKV epilogues and the attention kernels are written for "
+                             "those two head sizes; the reference accepts any value (muse_maskgit_pytorch.py:95-110, 164-172)")
+        if dim_head == 128 and dim % 64 != 0:
+            raise ValueError(f"dim_head=128 needs dim % 64 == 0 (got dim = {dim}): the 128-wide QKV epilogue runs on the wgmma product only, "
+                             "whose k-blocks are 64 wide")
         self.dim, self.depth, self.heads, self.dim_head, self.ff_mult = dim, depth, heads, dim_head, ff_mult
         self.layers = nn.ModuleList([nn.ModuleList([Attention(dim, dim_head, heads), Attention(dim, dim_head, heads, True),
                                                     _ff_params(dim, ff_mult)]) for _ in range(depth)])
@@ -248,10 +251,10 @@ class Transformer(nn.Module):
         kvs = []
         for lay in P["layers"]:
             ca = lay["ca"]
-            k = torch.zeros((b * heads, tk_alloc, 64), device=dev, dtype=adt)
-            v = torch.zeros((b * heads, tk_alloc, 64), device=dev, dtype=adt)
+            k = torch.zeros((b * heads, tk_alloc, tb.dim_head), device=dev, dtype=adt)
+            v = torch.zeros((b * heads, tk_alloc, tb.dim_head), device=dev, dtype=adt)
             epi = ops.qkv_epilogue(adt, heads, m, k=k, v=v, k_scale=ca["ks"], key_off=1, null_k=ca["nk"], null_v=ca["nv"])
-            ops.linear(ctx, ca["wkv"], None, epilogue=ops.EPI_QKV, epi=epi)
+            ops.linear(ctx, ca["wkv"], None, epilogue=ops.qkv_kind(k), epi=epi)
             if len(branches) > 1:
                 k, v = k.repeat(len(branches), 1, 1), v.repeat(len(branches), 1, 1)
             kvs.append((k, v))
@@ -265,16 +268,17 @@ class Transformer(nn.Module):
             return cache[key]
         P = self._packed()
         adt, tb = P["adt"], self.transformer_blocks
-        heads, dim, inner = tb.heads, self.dim, tb.heads * 64
+        heads, dim, dh = tb.heads, self.dim, tb.dim_head
+        inner = heads * dh
         R = nb * b * n
         Fp = max([l["ff"]["Fp"] for l in P["layers"]] + ([P["sc"]["Fp"]] if P["sc"] is not None else []))
         tk_alloc = _round_up(n + 1, 8)
         ws = dict(key=key,
                   x=torch.empty((R, dim), device=dev, dtype=torch.float32),
                   xn=torch.empty((R, dim), device=dev, dtype=adt),
-                  q=torch.empty((nb * b * heads, n, 64), device=dev, dtype=adt),
-                  k=torch.zeros((nb * b * heads, tk_alloc, 64), device=dev, dtype=adt),
-                  v=torch.zeros((nb * b * heads, tk_alloc, 64), device=dev, dtype=adt),
+                  q=torch.empty((nb * b * heads, n, dh), device=dev, dtype=adt),
+                  k=torch.zeros((nb * b * heads, tk_alloc, dh), device=dev, dtype=adt),
+                  v=torch.zeros((nb * b * heads, tk_alloc, dh), device=dev, dtype=adt),
                   ao=torch.empty((R, inner), device=dev, dtype=adt),
                   h=torch.empty((R, Fp), device=dev, dtype=adt),
                   hn=torch.empty((R, Fp), device=dev, dtype=adt),
@@ -298,6 +302,7 @@ class Transformer(nn.Module):
         dev = ids.device
         ws = self._workspace(nb, b, n, dev)
         x, xn, q, k, v, ao = ws["x"], ws["xn"], ws["q"], ws["k"], ws["v"], ws["ao"]
+        qkv = ops.qkv_kind(q)
         R, bn = nb * b * n, b * n
         if self.self_cond and self_cond_embed is not None:
             # x += self_cond_to_init_embed(embed of the previous step), identical for every CFG branch (muse_maskgit_pytorch.py:325-328);
@@ -325,9 +330,9 @@ class Transformer(nn.Module):
             epi = ops.qkv_epilogue(adt, heads, n, q=q, k=k, v=v, q_scale=sa["qs"], k_scale=sa["ks"], key_off=1,
                                    null_k=sa["nk"], null_v=sa["nv"])
             if "wqkv_8" in sa:
-                ops.linear_fp8(ws["xq"], ws["xs"], sa["wqkv_8"], sa["s_qkv"], None, epilogue=ops.EPI_QKV, epi=epi)
+                ops.linear_fp8(ws["xq"], ws["xs"], sa["wqkv_8"], sa["s_qkv"], None, epilogue=qkv, epi=epi)
             else:
-                ops.linear(xn, sa["wqkv"], None, epilogue=ops.EPI_QKV, epi=epi)
+                ops.linear(xn, sa["wqkv"], None, epilogue=qkv, epi=epi)
             ops.attention(q, k, v, ao, nb * b, heads, n + 1, logit_bound=sa["bound"])
             ops.linear(ao, sa["wo"], x, epilogue=ops.EPI_RESIDUAL, resid=x)
             # --- cross attention ---
@@ -336,9 +341,9 @@ class Transformer(nn.Module):
                 norm(slice(0, Rl), ca["g"], "wq_8" in ca)
                 epi = ops.qkv_epilogue(adt, heads, n, q=q[:ql], q_scale=ca["qs"])
                 if "wq_8" in ca:
-                    ops.linear_fp8(ws["xq"][:Rl], ws["xs"][:Rl], ca["wq_8"], ca["s_q"], None, epilogue=ops.EPI_QKV, epi=epi)
+                    ops.linear_fp8(ws["xq"][:Rl], ws["xs"][:Rl], ca["wq_8"], ca["s_q"], None, epilogue=qkv, epi=epi)
                 else:
-                    ops.linear(xn[:Rl], ca["wq"], None, epilogue=ops.EPI_QKV, epi=epi)
+                    ops.linear(xn[:Rl], ca["wq"], None, epilogue=qkv, epi=epi)
                 ops.attention(q[:ql], kc[:ql], vc[:ql], ao[:Rl], live * b, heads, ctx["m"] + 1, key_mask=ctx["key_mask"][:live * b],
                               logit_bound=ca["bound"])
                 ops.linear(ao[:Rl], ca["wo"], x[:Rl], epilogue=ops.EPI_RESIDUAL, resid=x[:Rl])
@@ -699,6 +704,9 @@ class MaskGit(nn.Module):
         if self.use_native_step and self.transformer.precision == "fp8":
             raise ValueError('use_native_step=True runs mmg_decode_step, whose weights carry no fp8 scales: it cannot run precision="fp8"; '
                              "set use_native_step = False")
+        if self.use_native_step and self.transformer.transformer_blocks.dim_head != 64:
+            raise ValueError("use_native_step=True runs mmg_decode_step, which is written for 64-wide heads: it cannot run dim_head="
+                             f"{self.transformer.transformer_blocks.dim_head}; set use_native_step = False")
         if negative_texts is not None:
             raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
         return self._decode(self._request(texts, cond_images=cond_images, fmap_size=fmap_size, temperature=temperature, timesteps=timesteps,

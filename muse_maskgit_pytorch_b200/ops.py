@@ -6,7 +6,7 @@ import torch
 
 from . import _lib as L
 from ._lib import (F32, BF16, EPI_STORE, EPI_RESIDUAL, EPI_GEGLU, EPI_GLU, EPI_QKV, EPI_CONVT, EPI_CONVT_RGB,  # noqa: F401
-                   EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH)
+                   EPI_LNFOLD_RESIDUAL, EPI_LFQ_IDS, EPI_ARGMIN, EPI_GEGLU_TANH, EPI_QKV128)
 
 
 def _chk(t, name="tensor"):
@@ -92,7 +92,7 @@ def linear(a, w, out, epilogue=EPI_STORE, bias=None, act=0, resid=None, M=None, 
 
 def linear_fp8(a, a_scale, w, w_scale, out, epilogue=EPI_GEGLU, epi=None, row_stats=None):
     """e4m3 product with per-row scales: out = epilogue((a @ w.T) * a_scale[:, None] * w_scale[None, :]).  a [M, K], w [N, K] float8_e4m3fn,
-    a_scale [M], w_scale [N] fp32; epilogue EPI_QKV (pass `epi` from qkv_epilogue) or EPI_GEGLU (bf16 `out`, optional row_stats)."""
+    a_scale [M], w_scale [N] fp32; epilogue EPI_QKV / EPI_QKV128 (pass `epi` from qkv_epilogue) or EPI_GEGLU (bf16 `out`, optional row_stats)."""
     _chk(a, "a"); _chk(w, "w"); _chk(a_scale, "a_scale"); _chk(w_scale, "w_scale")
     assert a.dtype == torch.float8_e4m3fn and w.dtype == torch.float8_e4m3fn and w.shape[1] == a.shape[1]
     assert a_scale.dtype == torch.float32 and w_scale.dtype == torch.float32
@@ -123,8 +123,18 @@ def layernorm_fp8(x, gamma, y, row_scale, add=None, x_out=None, add_from=0):
     return y
 
 
+def qkv_kind(t):
+    """The QKV epilogue for head tensors t [BH, rows, dh]: EPI_QKV for dh = 64, EPI_QKV128 for dh = 128."""
+    dh = t.shape[-1]
+    if dh not in (64, 128):
+        raise ValueError(f"QKV epilogue: head width {dh} (64 or 128 only)")
+    return EPI_QKV if dh == 64 else EPI_QKV128
+
+
 def qkv_epilogue(dtype_t, heads, tokens, q=None, k=None, v=None, q_scale=None, k_scale=None, key_off=0, null_k=None, null_v=None):
-    """Epilogue block for MMG_EPI_QKV.  q [BH, q_rows, 64]; k, v [BH, kv_rows, 64]."""
+    """Epilogue block for MMG_EPI_QKV (q [BH, q_rows, 64]; k, v [BH, kv_rows, 64]) or MMG_EPI_QKV128 (the same with 128-wide heads):
+    pass it with epilogue=qkv_kind(q or k)."""
+    assert len({t.shape[-1] for t in (q, k, v) if t is not None}) == 1, "q / k / v: one head width"
     e = L.EpilogueArgs()
     e.out_dtype = L.F32 if dtype_t == torch.float32 else L.BF16
     e.heads = heads; e.tokens = tokens; e.key_off = key_off
@@ -267,11 +277,14 @@ def embed(ids, token_emb, pos_emb, x, n, copies=1, use_pos=True):
 
 
 def attention(q, k, v, out, B, heads, Tk, key_mask=None, kv_shared=False, scale=8.0, logit_bound=0.0):
-    """q [B*heads, Tq, 64]; k, v [(B or 1)*heads, Tk_alloc, 64]; out [B*Tq, heads*64]."""
+    """q [B*heads, Tq, dh]; k, v [(B or 1)*heads, Tk_alloc, dh]; out [B*Tq, heads*dh]; dh = 64 (mmg_attention) or 128 (mmg_attention_d128,
+    whose fp32 path runs on the CUDA cores)."""
     a = L.AttentionArgs()
     _chk(q); _chk(k); _chk(v)
-    Tq, Tk_alloc, dtype = q.shape[1], k.shape[1], L.dt(q)
-    if q.dtype == torch.float32 and _FP32_TC[0] and 2 <= Tk <= 4096 and out.dtype == torch.float32 and out.stride(0) % 8 == 0:
+    Tq, Tk_alloc, dtype, dh = q.shape[1], k.shape[1], L.dt(q), q.shape[-1]
+    assert dh in (64, 128) and k.shape[-1] == v.shape[-1] == dh, "attention: q / k / v heads of one width, 64 or 128"
+    entry = "mmg_attention" if dh == 64 else "mmg_attention_d128"
+    if dh == 64 and q.dtype == torch.float32 and _FP32_TC[0] and 2 <= Tk <= 4096 and out.dtype == torch.float32 and out.stride(0) % 8 == 0:
         # fp32 parity on the tensor cores: three bf16 terms per operand, six cross terms per product (mmg_attention_split.cuh)
         q, k, v = split3(q.view(-1, 64), 0), split3(k.view(-1, 64), 1), split3(v.view(-1, 64), 1)
         dtype = L.BF16; a.split3 = 1
@@ -279,7 +292,7 @@ def attention(q, k, v, out, B, heads, Tk, key_mask=None, kv_shared=False, scale=
     a.key_mask = L.ptr(key_mask)
     a.B = B; a.heads = heads; a.Tq = Tq; a.Tk = Tk; a.Tk_alloc = Tk_alloc; a.dtype = dtype
     a.ldo = out.stride(0); a.kv_batch_stride_zero = int(kv_shared); a.scale = scale; a.logit_bound = logit_bound
-    L.call("mmg_attention", a)
+    L.call(entry, a)
     return out
 
 
