@@ -1,4 +1,5 @@
-// mmg_linear / mmg_conv2d / mmg_conv_transpose2d: launchers for the wgmma GEMM (bf16) and the fp32 CUDA-core GEMM.
+// mmg_linear / mmg_conv2d / mmg_conv_transpose2d and their e4m3 forms: launchers for the wgmma GEMM (bf16 / e4m3) and the fp32
+// CUDA-core GEMM.
 #include "mmg_gemm_tc.cuh"
 #include "mmg_tmap.cuh"
 #include <mutex>
@@ -8,6 +9,7 @@ namespace mmg {
 int linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* stream);
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
 
 // persistent grid of min(tiles, #SM) CTAs
 template <int BN, int EPI_MODE, typename TA = bf16>
@@ -24,6 +26,39 @@ static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
   return MMG_OK;
 }
 
+// every instantiation of tc_gemm_kernel: 15 with bf16 operands, 8 with e4m3 ones
+static constexpr int tc_key(bool fp8, int bn, int mode) { return (fp8 ? 1 << 16 : 0) | bn << 4 | mode; }
+
+static int launch_instantiation(bool fp8, int bn, int mode, const TcGemmParams& p, cudaStream_t st) {
+  if (bn != 64 && bn != 128 && bn != 256) return fail(MMG_EINVAL, "unsupported tile width %d", bn);
+  switch (tc_key(fp8, bn, mode)) {
+    case tc_key(false, 64, TC_EPI_REGS): return launch_tc<64, TC_EPI_REGS>(p, st);
+    case tc_key(false, 128, TC_EPI_REGS): return launch_tc<128, TC_EPI_REGS>(p, st);
+    case tc_key(false, 256, TC_EPI_REGS): return launch_tc<256, TC_EPI_REGS>(p, st);          // CONVT_RGB only
+    case tc_key(false, 64, TC_EPI_REDUCE): return launch_tc<64, TC_EPI_REDUCE>(p, st);
+    case tc_key(false, 128, TC_EPI_REDUCE): return launch_tc<128, TC_EPI_REDUCE>(p, st);
+    case tc_key(false, 256, TC_EPI_REDUCE): return launch_tc<256, TC_EPI_REDUCE>(p, st);
+    case tc_key(false, 128, TC_EPI_TSTORE): return launch_tc<128, TC_EPI_TSTORE>(p, st);      // the sample GEMM of the fused tail at small batch
+    case tc_key(false, 256, TC_EPI_TSTORE): return launch_tc<256, TC_EPI_TSTORE>(p, st);
+    case tc_key(false, 128, TC_EPI_QKV): return launch_tc<128, TC_EPI_QKV>(p, st);
+    case tc_key(false, 256, TC_EPI_QKV): return launch_tc<256, TC_EPI_QKV>(p, st);
+    case tc_key(false, 256, TC_EPI_GEGLU): return launch_tc<256, TC_EPI_GEGLU>(p, st);
+    case tc_key(false, 128, TC_EPI_ACT): return launch_tc<128, TC_EPI_ACT>(p, st);
+    case tc_key(false, 128, TC_EPI_QKV128): return launch_tc<128, TC_EPI_QKV128>(p, st);
+    case tc_key(false, 256, TC_EPI_QKV128): return launch_tc<256, TC_EPI_QKV128>(p, st);
+    case tc_key(false, 128, TC_EPI_QKV128_REGS): return launch_tc<128, TC_EPI_QKV128_REGS>(p, st);
+    case tc_key(true, 64, TC_EPI_REGS): return launch_tc<64, TC_EPI_REGS, fp8e4>(p, st);
+    case tc_key(true, 128, TC_EPI_REGS): return launch_tc<128, TC_EPI_REGS, fp8e4>(p, st);
+    case tc_key(true, 256, TC_EPI_REGS): return launch_tc<256, TC_EPI_REGS, fp8e4>(p, st);  // CONVT_RGB only
+    case tc_key(true, 128, TC_EPI_QKV): return launch_tc<128, TC_EPI_QKV, fp8e4>(p, st);
+    case tc_key(true, 256, TC_EPI_QKV): return launch_tc<256, TC_EPI_QKV, fp8e4>(p, st);
+    case tc_key(true, 256, TC_EPI_GEGLU): return launch_tc<256, TC_EPI_GEGLU, fp8e4>(p, st);
+    case tc_key(true, 128, TC_EPI_QKV128): return launch_tc<128, TC_EPI_QKV128, fp8e4>(p, st);
+    case tc_key(true, 256, TC_EPI_QKV128): return launch_tc<256, TC_EPI_QKV128, fp8e4>(p, st);
+  }
+  return fail(MMG_EINVAL, "no tc_gemm_kernel<%d, %d> instantiation for %s operands", bn, mode, fp8 ? "e4m3" : "bf16");
+}
+
 static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
   if (epilogue == MMG_EPI_CONVT_RGB) return (int)N;             // whole row in one tile
   if (N % 256 == 0 && M_tiles * (N / 256) >= 2 * num_sms()) return 256;
@@ -32,12 +67,54 @@ static int pick_bn(int64_t M_tiles, int64_t N, int epilogue) {
   return (N % 64 == 0 && N % 128 != 0) ? 64 : ((M_tiles * ((N + 127) / 128) >= 96) ? 128 : 64);
 }
 
-// the output tensor maps of the QKV (q / k / v heads) and GEGLU (bf16 [M, N / 2]) tile epilogues
-static int bf16_out_maps(TcGemmParams& p, int epi_mode) {
+// The tile plan of every wgmma GEMM launch: (BN, EPI_MODE) from the operand type and p's geometry (mode, M, num_m_tiles) and epilogue.
+static int plan_tc(const TcGemmParams& p, bool fp8, int* bn_out, int* mode_out) {
+  const mmg_epilogue_args& e = p.epi.p;
+  const int kind = p.epi.kind;
+  MMG_CHECK_ARG(kind != MMG_EPI_QKV128 || p.mode == 0, "QKV128: dense products only");
+  int bn = pick_bn(p.num_m_tiles, p.N, kind), mode;
+  const bool in_place = (kind == MMG_EPI_LNFOLD_RESIDUAL || (kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
+                        e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && p.mode == 0;
+  const bool plain_f32 = kind == MMG_EPI_STORE && e.out_dtype == MMG_F32 && p.mode == 0 && !e.bias && e.act == 0 && (e.ldo % 4) == 0 && aligned16(e.out);
+  // QKV / QKV128 tile epilogue: bf16 heads, whole 16-token boxes of one sequence
+  const bool qkv_tiles = (kind == MMG_EPI_QKV || kind == MMG_EPI_QKV128) && e.out_dtype == MMG_BF16 && p.mode == 0 && e.tokens % 32 == 0 &&
+                         p.M % 128 == 0 && e.nk_heads == e.nv_heads && (!e.nq_heads || aligned16(e.q_out)) &&
+                         (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out)));
+  const bool geglu_tiles = kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && (e.ldo % 8) == 0 && aligned16(e.out);
+  // A dense e4m3 product has no register-epilogue instantiation: its argument checks leave it only the shapes its tile epilogue takes, and
+  // it runs that epilogue at every M: QKV at 128 where pick_bn gives 64 (where the bf16 product takes <64, REGS>), GEGLU at 256 whatever
+  // pick_bn gives.  QKV128 (whole 128-column heads) runs its tile epilogue at 128 or 256 for either operand type.
+  const bool tile_at_any_bn = fp8 && p.mode == 0;
+  if (p.epi.is_act()) {
+    mode = TC_EPI_ACT; bn = 128;              // the T5 feed-forward epilogues: an instantiation of their own, kept out of the VAE's
+  } else if (in_place) {
+    mode = TC_EPI_REDUCE;
+  } else if (plain_f32 && bn >= 128) {
+    mode = TC_EPI_TSTORE;
+  } else if (qkv_tiles && (bn != 64 || tile_at_any_bn || kind == MMG_EPI_QKV128)) {
+    mode = kind == MMG_EPI_QKV ? TC_EPI_QKV : TC_EPI_QKV128; bn = bn == 256 ? 256 : 128;
+  } else if (kind == MMG_EPI_QKV128) {
+    mode = TC_EPI_QKV128_REGS; bn = 128;      // 64 accumulators per thread, stored from the fragments
+  } else if (geglu_tiles && (bn == 256 || tile_at_any_bn)) {
+    mode = TC_EPI_GEGLU; bn = 256;
+  } else {
+    // 128 accumulator registers per thread at BN = 256 next to a 64-column row chunk would spill, so <256, TC_EPI_REGS> compiles only
+    // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128
+    mode = TC_EPI_REGS;
+    if (bn == 256 && kind != MMG_EPI_CONVT_RGB) bn = 128;
+  }
+  // the tile epilogues write whole 32- / 64-column boxes: pick_bn's widths divide N (N % 64 == 0 on this path)
+  MMG_CHECK_ARG(!tc_tile_epilogue(mode) || p.N % bn == 0, "tile epilogue: tile width %d does not divide N = %lld", bn, (long long)p.N);
+  *bn_out = bn; *mode_out = mode;
+  return MMG_OK;
+}
+
+// the output tensor maps of the tile epilogues: q / k / v heads (QKV, QKV128), bf16 [M, N / 2] (GEGLU), fp32 [M, N] (REDUCE, TSTORE)
+static int tile_out_maps(TcGemmParams& p, int mode) {
   const mmg_epilogue_args& e = p.epi.p;
   int rc = MMG_OK;
-  if (epi_mode == TC_EPI_QKV || epi_mode == TC_EPI_QKV128) {
-    const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads, hd = epi_mode == TC_EPI_QKV ? 64 : 128;
+  if (mode == TC_EPI_QKV || mode == TC_EPI_QKV128) {
+    const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads, hd = mode == TC_EPI_QKV ? 64 : 128;
     uint64_t str[1] = {hd * 2}; uint32_t box[2] = {64, 16};
     if (e.nq_heads) { uint64_t d[2] = {hd, seqs * (uint64_t)e.q_rows}; rc = make_tmap_bf16(&p.tma_qkv[0], e.q_out, 2, d, str, box); if (rc) return rc; }
     if (e.nk_heads) {
@@ -45,77 +122,34 @@ static int bf16_out_maps(TcGemmParams& p, int epi_mode) {
       rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
       rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
     }
-  } else if (epi_mode == TC_EPI_GEGLU) {
+  } else if (mode == TC_EPI_GEGLU) {
     uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 16};
     rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob);
+  } else if (mode == TC_EPI_REDUCE || mode == TC_EPI_TSTORE) {
+    uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 16};
+    rc = make_tmap_f32(&p.tma_out, e.out, 2, od, os, ob);
   }
   return rc;
 }
 
-// QKV128 on the tile epilogue: bf16 heads, whole 16-token boxes of one sequence (the conditions of TC_EPI_QKV)
-static bool qkv128_tiles(const TcGemmParams& p) {
-  const mmg_epilogue_args& e = p.epi.p;
-  return e.out_dtype == MMG_BF16 && p.mode == 0 && e.tokens % 32 == 0 && p.M % 128 == 0 && e.nk_heads == e.nv_heads &&
-         (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out)));
+// an operand tensor map of the wgmma GEMM: bf16, or e4m3 moved as bytes
+static int operand_map(CUtensorMap* m, bool fp8, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box) {
+  return fp8 ? make_tmap_u8(m, base, rank, dims, strides, box) : make_tmap_bf16(m, base, rank, dims, strides, box);
 }
 
-static int dispatch_tc(TcGemmParams& p, int bn, const void* w, int64_t N, int64_t K, int64_t ldw, cudaStream_t st) {
-  const mmg_epilogue_args& e = p.epi.p;
-  if (p.epi.kind == MMG_EPI_QKV128) {
-    // whole heads per tile: BN = 256 or 128 on the tile epilogue, 128 (64 accumulators per thread) on the fragment stores
-    MMG_CHECK_ARG(p.mode == 0, "QKV128: dense products only");
-    const bool tiles = qkv128_tiles(p);
-    bn = tiles && bn == 256 ? 256 : 128;
-    p.num_n_tiles = (int)(N / bn);
-    p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
-    int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
-    if (!tiles) return launch_tc<128, TC_EPI_QKV128_REGS>(p, st);
-    rc = bf16_out_maps(p, TC_EPI_QKV128); if (rc) return rc;
-    return bn == 256 ? launch_tc<256, TC_EPI_QKV128>(p, st) : launch_tc<128, TC_EPI_QKV128>(p, st);
-  }
-  const bool in_place = (p.epi.kind == MMG_EPI_LNFOLD_RESIDUAL || (p.epi.kind == MMG_EPI_RESIDUAL && e.act == 0)) && e.out_dtype == MMG_F32 &&
-                        e.out == e.resid && e.ldo == e.ldr && (e.ldo % 4) == 0 && aligned16(e.out) && p.mode == 0;
-  const bool plain_f32 = p.epi.kind == MMG_EPI_STORE && e.out_dtype == MMG_F32 && p.mode == 0 && !e.bias && e.act == 0 && (e.ldo % 4) == 0 && aligned16(e.out);
-  const bool qkv_tiles = p.epi.kind == MMG_EPI_QKV && e.out_dtype == MMG_BF16 && p.mode == 0 && e.tokens % 32 == 0 && p.M % 128 == 0 && (bn == 128 || bn == 256) &&
-                         (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out))) && e.nk_heads == e.nv_heads;
-  const bool geglu_tiles = p.epi.kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && bn == 256 && (e.ldo % 8) == 0 && aligned16(e.out);
-  const int epi_mode = p.epi.is_act() ? TC_EPI_ACT : in_place ? TC_EPI_REDUCE : (plain_f32 && (bn == 256 || bn == 128)) ? TC_EPI_TSTORE :
-                       qkv_tiles ? TC_EPI_QKV : geglu_tiles ? TC_EPI_GEGLU : TC_EPI_REGS;
-  // 128 accumulator registers per thread at BN = 256 next to a 64-column row chunk would spill, so <256, TC_EPI_REGS> compiles only
-  // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128, and the T5
-  // feed-forward epilogues (their own instantiation, kept out of the VAE's) at BN = 128 only
-  if (epi_mode == TC_EPI_REGS && bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;
-  if (epi_mode == TC_EPI_ACT) bn = 128;
-  // the tile epilogues write whole 32- / 64-column boxes: pick_bn's widths divide N (N % 64 == 0 on this path)
-  MMG_CHECK_ARG(!tc_tile_epilogue(epi_mode) || N % bn == 0, "tile epilogue: tile width %d does not divide N = %lld", bn, (long long)N);
-  p.num_n_tiles = (int)((N + bn - 1) / bn);
-  p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
-  uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)ldw * 2}; uint32_t box[2] = {TC_BK, (uint32_t)bn};
-  int rc = make_tmap_bf16(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
-  if (epi_mode == TC_EPI_QKV) {
-    rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
-    return bn == 256 ? launch_tc<256, TC_EPI_QKV>(p, st) : launch_tc<128, TC_EPI_QKV>(p, st);
-  }
-  if (epi_mode == TC_EPI_GEGLU) {
-    rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
-    return launch_tc<256, TC_EPI_GEGLU>(p, st);
-  }
-  if (epi_mode == TC_EPI_ACT) return launch_tc<128, TC_EPI_ACT>(p, st);
-  if (epi_mode != TC_EPI_REGS) {
-    uint64_t od[2] = {(uint64_t)p.N, (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {32, 16};
-    rc = make_tmap_f32(&p.tma_out, e.out, 2, od, os, ob); if (rc) return rc;
-  }
-  if (epi_mode == TC_EPI_TSTORE) return bn == 256 ? launch_tc<256, TC_EPI_TSTORE>(p, st) : launch_tc<128, TC_EPI_TSTORE>(p, st);   // 128: the sample GEMM of the fused tail at small batch
-  if (epi_mode == TC_EPI_REDUCE) {
-    switch (bn) { case 64: return launch_tc<64, TC_EPI_REDUCE>(p, st); case 128: return launch_tc<128, TC_EPI_REDUCE>(p, st); case 256: return launch_tc<256, TC_EPI_REDUCE>(p, st); }
-  }
-  switch (bn) {
-    case 64: return launch_tc<64, TC_EPI_REGS>(p, st);
-    case 128: return launch_tc<128, TC_EPI_REGS>(p, st);
-    case 256: return launch_tc<256, TC_EPI_REGS>(p, st);       // CONVT_RGB: the whole 256-column row in one tile
-  }
-  return fail(MMG_EINVAL, "unsupported tile width %d", bn);
+// Plans and launches one wgmma GEMM whose A operand map(s), geometry and epilogue p already holds.  w: the [N, K] weights, rows ldw
+// elements apart; a k-block is 128 bytes of them.
+static int dispatch_tc(TcGemmParams& p, bool fp8, const void* w, int64_t K, int64_t ldw, cudaStream_t st) {
+  int bn, mode;
+  int rc = plan_tc(p, fp8, &bn, &mode); if (rc) return rc;
+  const uint64_t esz = fp8 ? 1 : 2;
+  p.num_n_tiles = (int)((p.N + bn - 1) / bn);
+  // N-fastest while the weights (counted at 2 bytes an element for either operand type) fit 8 MiB in 2..16 column tiles
+  p.n_fast = ((int64_t)p.N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;
+  uint64_t dims[2] = {(uint64_t)K, (uint64_t)p.N}; uint64_t str[1] = {(uint64_t)ldw * esz}; uint32_t box[2] = {(uint32_t)(128 / esz), (uint32_t)bn};
+  rc = operand_map(&p.tma_b, fp8, w, 2, dims, str, box); if (rc) return rc;
+  rc = tile_out_maps(p, mode); if (rc) return rc;
+  return launch_instantiation(fp8, bn, mode, p, st);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -216,16 +250,25 @@ static int launch_simt(int dtype, const void* a, const void* w, int64_t M, int64
 
 
 // conv tap tables.  kind 0: 1x1; 1: 3x3 s1 p1; 2: 4x4 s2 p1; 3: 5x5 s1 p2.  Tap index t = r*kw + s (weights packed tap-major).
+// CONVT_PARITY + py * 2 + px: conv-transpose (k4 s2 p1) parity class (py, px) over the input grid: 2x2 taps, tap t = a*2+b at input
+// offset (CT_D[py][a], CT_D[px][b]).
+constexpr int CONVT_PARITY = 4;
+static const int CT_D[2][2] = {{0, -1}, {1, 0}};
+
 static void conv_geom(int kind, int B, int H, int W, int Cin, ConvGeom* g) {
+  g->B = B; g->H = H; g->W = W; g->Cin = Cin;
+  if (kind >= CONVT_PARITY) {
+    const int py = (kind - CONVT_PARITY) >> 1, px = (kind - CONVT_PARITY) & 1;
+    g->stride = 1; g->Ho = H; g->Wo = W; g->ntaps = 4;
+    for (int t = 0; t < 4; ++t) { g->tdy[t] = (int8_t)CT_D[py][t >> 1]; g->tdx[t] = (int8_t)CT_D[px][t & 1]; }
+    return;
+  }
   const int k = kind == 0 ? 1 : kind == 1 ? 3 : kind == 2 ? 4 : 5;
   const int pad = kind == 0 ? 0 : kind == 1 ? 1 : kind == 2 ? 1 : 2;
-  g->B = B; g->H = H; g->W = W; g->Cin = Cin; g->stride = (kind == 2) ? 2 : 1;
+  g->stride = (kind == 2) ? 2 : 1;
   g->Ho = H / g->stride; g->Wo = W / g->stride; g->ntaps = k * k;
   for (int r = 0; r < k; ++r) for (int s = 0; s < k; ++s) { g->tdy[r * k + s] = (int8_t)(r - pad); g->tdx[r * k + s] = (int8_t)(s - pad); }
 }
-
-// conv-transpose (k4 s2 p1) parity class (py,px): 2x2 taps, tap t = a*2+b, input offset dy = DY[py][a], kernel row r = R[py][a].
-static const int CT_D[2][2] = {{0, -1}, {1, 0}};
 
 static int tile_geometry(int Ho, int Wo, TcGemmParams* p) {
   int TW = Wo < 128 ? Wo : 128;
@@ -235,6 +278,39 @@ static int tile_geometry(int Ho, int Wo, TcGemmParams* p) {
   p->TW = TW; p->TH = TH; p->TB = 128 / (TW * TH);
   p->tiles_x = Wo / TW; p->tiles_y = Ho / TH;
   return 0;
+}
+
+// the tap table of tc_gemm_kernel's conv mode: tap t reads A map tap_map[t] at the output pixel + (tap_dy[t], tap_dx[t]).  Stride 2:
+// input row 2y + dy = 2(y + (dy - py) / 2) + py, so the tap reads the map of input parity (py, px) at the half-resolution offset.
+static void conv_taps(TcGemmParams& p, const ConvGeom& g) {
+  for (int t = 0; t < g.ntaps; ++t) {
+    if (g.stride == 1) { p.tap_map[t] = 0; p.tap_dy[t] = g.tdy[t]; p.tap_dx[t] = g.tdx[t]; continue; }
+    const int oy = g.tdy[t], ox = g.tdx[t];
+    const int py = ((oy % 2) + 2) % 2, px = ((ox % 2) + 2) % 2;
+    p.tap_map[t] = (int8_t)(py * 2 + px); p.tap_dy[t] = (int8_t)((oy - py) / 2); p.tap_dx[t] = (int8_t)((ox - px) / 2);
+  }
+}
+
+// The implicit-GEMM operand of tc_gemm_kernel's conv mode over the NHWC image x (bf16, or e4m3 bytes) of geometry g: the problem shape,
+// the tap table and the A tensor map(s), one 4-D map or, at stride 2, one per input parity (py, px) over the (H/2, W/2) grid.  A k-block
+// is one tap x 128 bytes of channels.  tile_geometry() has filled p's tile fields.
+static int conv_operand(TcGemmParams& p, const ConvGeom& g, const void* x, bool fp8, int64_t N) {
+  const uint64_t esz = fp8 ? 1 : 2, C = g.Cin, W = g.W, H = g.H;
+  p.M = (int64_t)g.B * g.Ho * g.Wo; p.N = N; p.mode = 1; p.cchunks = (int)(C * esz / 128); p.ntaps = g.ntaps; p.num_kb = p.ntaps * p.cchunks;
+  p.Ho = g.Ho; p.Wo = g.Wo; p.B = g.B;
+  p.num_m_tiles = p.tiles_x * p.tiles_y * ((g.B + p.TB - 1) / p.TB);
+  conv_taps(p, g);
+  uint32_t box[4] = {(uint32_t)(128 / esz), (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TB};
+  if (g.stride == 1) {
+    uint64_t dims[4] = {C, W, H, (uint64_t)g.B}; uint64_t str[3] = {C * esz, W * C * esz, H * W * C * esz};
+    return operand_map(&p.tma_a[0], fp8, x, 4, dims, str, box);
+  }
+  for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
+    const uint8_t* base = reinterpret_cast<const uint8_t*>(x) + ((uint64_t)py * W + px) * C * esz;
+    uint64_t dims[4] = {C, W / 2, H / 2, (uint64_t)g.B}; uint64_t str[3] = {2 * C * esz, 2 * W * C * esz, H * W * C * esz};
+    const int rc = operand_map(&p.tma_a[py * 2 + px], fp8, base, 4, dims, str, box); if (rc) return rc;
+  }
+  return MMG_OK;
 }
 
 }  // namespace mmg
@@ -268,12 +344,13 @@ int mmg::linear_impl(const mmg_linear_args* a, const int* skip_if_zero, void* st
   p.epi = epi;
   uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda * 2}; uint32_t box[2] = {TC_BK, TC_BM};
   rc = make_tmap_bf16(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc;
-  const int bn = pick_bn(p.num_m_tiles, a->N, a->epilogue);
-  MMG_CHECK_ARG(bn == 64 || bn == 128 || bn == 256, "mmg_linear: unsupported N=%lld for this epilogue", (long long)a->N);
-  return dispatch_tc(p, bn, a->w, a->N, a->K, a->ldw, st);
+  // CONVT_RGB takes the whole row in one tile
+  MMG_CHECK_ARG(a->epilogue != MMG_EPI_CONVT_RGB || a->N == 64 || a->N == 128 || a->N == 256, "mmg_linear: unsupported N=%lld for this epilogue", (long long)a->N);
+  return dispatch_tc(p, false, a->w, a->K, a->ldw, st);
 }
 
-// e4m3 operands: the QKV and GEGLU tile epilogues only, at the tile widths and tile order the bf16 product of the same shape takes
+// e4m3 operands: the QKV and GEGLU tile epilogues only (plan_tc states the tile widths), in the tile order the bf16 product of the same
+// shape takes
 extern "C" int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->a && a->w && a->a_scale && a->w_scale, "mmg_linear_fp8: NULL operand or scale");
@@ -281,38 +358,27 @@ extern "C" int mmg_linear_fp8(const mmg_linear_fp8_args* a, void* stream) {
   MMG_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0 && a->K % 128 == 0, "mmg_linear_fp8: bad shape M=%lld N=%lld K=%lld (K %% 128 == 0)",
                 (long long)a->M, (long long)a->N, (long long)a->K);
   MMG_CHECK_ARG(a->lda >= a->K && a->ldw >= a->K && a->lda % 16 == 0 && a->ldw % 16 == 0 && aligned16(a->a) && aligned16(a->w) &&
-                (reinterpret_cast<uintptr_t>(a->w_scale) & 7) == 0, "mmg_linear_fp8: operands need 16-byte rows, w_scale 8-byte alignment");
+                aligned8(a->w_scale), "mmg_linear_fp8: operands need 16-byte rows, w_scale 8-byte alignment");
   MMG_CHECK_ARG(a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_QKV128 || a->epilogue == MMG_EPI_GEGLU, "mmg_linear_fp8: epilogue %d (QKV or GEGLU only, or QKV128)", a->epilogue);
   int rc = validate_epilogue(a->epilogue, a->epi, a->N); if (rc) return rc;
   const mmg_epilogue_args& e = a->epi;
-  const int64_t m_tiles = (a->M + TC_BM - 1) / TC_BM;
-  int bn = 256, epi_mode = TC_EPI_GEGLU;
   if (a->epilogue == MMG_EPI_QKV || a->epilogue == MMG_EPI_QKV128) {
     MMG_CHECK_ARG(e.out_dtype == MMG_BF16 && e.tokens > 0 && e.tokens % 32 == 0 && a->M % 128 == 0 && a->N % 128 == 0 && e.nk_heads == e.nv_heads &&
                   (!e.nq_heads || aligned16(e.q_out)) && (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out))),
                   "mmg_linear_fp8: QKV needs bf16 outputs, tokens %% 32 == 0, M %% 128 == 0, N %% 128 == 0 (M=%lld N=%lld tokens=%d)",
                   (long long)a->M, (long long)a->N, e.tokens);
-    bn = pick_bn(m_tiles, a->N, a->epilogue) == 256 ? 256 : 128;
-    epi_mode = a->epilogue == MMG_EPI_QKV ? TC_EPI_QKV : TC_EPI_QKV128;
   } else {
     MMG_CHECK_ARG(e.out_dtype == MMG_BF16 && a->N % 256 == 0 && e.ldo % 8 == 0 && aligned16(e.out),
                   "mmg_linear_fp8: GEGLU needs bf16 out, N %% 256 == 0, ldo %% 8 == 0 (N=%lld)", (long long)a->N);
   }
   TcGemmParams p{};
   p.M = a->M; p.N = a->N; p.num_kb = (int)(a->K / 128); p.mode = 0;
-  p.num_m_tiles = (int)m_tiles;
-  p.num_n_tiles = (int)(a->N / bn);
-  p.n_fast = ((int64_t)a->N * a->K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;   // the bf16 product's tile order
+  p.num_m_tiles = (int)((a->M + TC_BM - 1) / TC_BM);
   p.epi.p = a->epi; p.epi.kind = a->epilogue;
   p.a_scale = a->a_scale; p.w_scale = a->w_scale;
-  { uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda}; uint32_t box[2] = {128, TC_BM};
-    rc = make_tmap_u8(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc; }
-  { uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->N}; uint64_t str[1] = {(uint64_t)a->ldw}; uint32_t box[2] = {128, (uint32_t)bn};
-    rc = make_tmap_u8(&p.tma_b, a->w, 2, dims, str, box); if (rc) return rc; }
-  rc = bf16_out_maps(p, epi_mode); if (rc) return rc;
-  if (epi_mode == TC_EPI_GEGLU) return launch_tc<256, TC_EPI_GEGLU, fp8e4>(p, st);
-  if (epi_mode == TC_EPI_QKV128) return bn == 256 ? launch_tc<256, TC_EPI_QKV128, fp8e4>(p, st) : launch_tc<128, TC_EPI_QKV128, fp8e4>(p, st);
-  return bn == 256 ? launch_tc<256, TC_EPI_QKV, fp8e4>(p, st) : launch_tc<128, TC_EPI_QKV, fp8e4>(p, st);
+  uint64_t dims[2] = {(uint64_t)a->K, (uint64_t)a->M}; uint64_t str[1] = {(uint64_t)a->lda}; uint32_t box[2] = {128, TC_BM};
+  rc = make_tmap_u8(&p.tma_a[0], a->a, 2, dims, str, box); if (rc) return rc;
+  return dispatch_tc(p, true, a->w, a->K, a->ldw, st);
 }
 
 extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
@@ -333,71 +399,14 @@ extern "C" int mmg_conv2d(const mmg_conv2d_args* a, void* stream) {
     if (a->dtype == MMG_BF16) note_simt_fallback("mmg_conv2d", M, N, K);
     return launch_simt<true>(a->dtype, a->x, a->w, M, N, K, 0, K, g, epi, st);
   }
-  p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 64; p.ntaps = g.ntaps; p.num_kb = p.ntaps * p.cchunks;
-  p.Ho = g.Ho; p.Wo = g.Wo; p.B = a->B;
-  p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
   p.epi = epi;
-  const uint64_t C = a->Cin, W = a->W, H = a->H;
-  uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TB};
-  if (a->kind != 2) {
-    uint64_t dims[4] = {C, W, H, (uint64_t)a->B}; uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
-    rc = make_tmap_bf16(&p.tma_a[0], a->x, 4, dims, str, box); if (rc) return rc;
-    for (int t = 0; t < g.ntaps; ++t) { p.tap_map[t] = 0; p.tap_dy[t] = g.tdy[t]; p.tap_dx[t] = g.tdx[t]; }
-  } else {
-    // stride 2: input row 2y + (r-1) = 2(y+dy) + py.  One tensor map per input parity (py,px) over the (H/2, W/2) grid.
-    for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
-      const uint8_t* base = reinterpret_cast<const uint8_t*>(a->x) + ((uint64_t)py * W + px) * C * 2;
-      uint64_t dims[4] = {C, W / 2, H / 2, (uint64_t)a->B}; uint64_t str[3] = {2 * C * 2, 2 * W * C * 2, H * W * C * 2};
-      rc = make_tmap_bf16(&p.tma_a[py * 2 + px], base, 4, dims, str, box); if (rc) return rc;
-    }
-    for (int r = 0; r < 4; ++r) for (int s = 0; s < 4; ++s) {
-      const int oy = r - 1, ox = s - 1;
-      const int py = ((oy % 2) + 2) % 2, px = ((ox % 2) + 2) % 2;
-      p.tap_map[r * 4 + s] = (int8_t)(py * 2 + px); p.tap_dy[r * 4 + s] = (int8_t)((oy - py) / 2); p.tap_dx[r * 4 + s] = (int8_t)((ox - px) / 2);
-    }
-  }
-  const int bn = pick_bn(p.num_m_tiles, N, a->epilogue);
-  return dispatch_tc(p, bn, a->w, N, K, K, st);
+  rc = conv_operand(p, g, a->x, false, N); if (rc) return rc;
+  return dispatch_tc(p, false, a->w, K, K, st);
 }
 
-// ------------------------------------------------------------------------------------------------------------------
 // e4m3 convolutions: the conv mode of tc_gemm_kernel<BN, TC_EPI_REGS, fp8e4> at the tile geometry, tile width and tile order the bf16
-// convolution of the same shape takes.  A k-block is one tap x 128 channels (Cin % 128 == 0); the register epilogue first dequantises
-// with x_scale[image] * w_scale[col].  Shapes the kernel does not take are argument errors: there is no other e4m3 convolution kernel.
-// ------------------------------------------------------------------------------------------------------------------
-static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
-
-static int launch_conv_fp8(TcGemmParams& p, const void* w, int64_t N, int64_t K, cudaStream_t st) {
-  int bn = pick_bn(p.num_m_tiles, N, p.epi.kind);
-  if (bn == 256 && p.epi.kind != MMG_EPI_CONVT_RGB) bn = 128;        // dispatch_tc's register-epilogue width (<256, REGS>: RGB only)
-  p.num_n_tiles = (int)((N + bn - 1) / bn);
-  p.n_fast = ((int64_t)N * K * 2 <= (8 << 20) && p.num_n_tiles > 1 && p.num_n_tiles <= 16) ? 1 : 0;   // the bf16 product's tile order
-  uint64_t dims[2] = {(uint64_t)K, (uint64_t)N}; uint64_t str[1] = {(uint64_t)K}; uint32_t box[2] = {128, (uint32_t)bn};
-  int rc = make_tmap_u8(&p.tma_b, w, 2, dims, str, box); if (rc) return rc;
-  switch (bn) {
-    case 64: return launch_tc<64, TC_EPI_REGS, fp8e4>(p, st);
-    case 128: return launch_tc<128, TC_EPI_REGS, fp8e4>(p, st);
-    case 256: return launch_tc<256, TC_EPI_REGS, fp8e4>(p, st);      // CONVT_RGB: the whole 256-column row in one tile
-  }
-  return fail(MMG_EINVAL, "e4m3 convolution: unsupported tile width %d", bn);
-}
-
-// the A tensor map(s) of an e4m3 NHWC map: one 4-D map (stride 1), or one per input parity over the (H/2, W/2) grid (stride 2)
-static int fp8_image_maps(TcGemmParams& p, const void* x, int B, int H, int W, int Cin, bool stride2) {
-  const uint64_t C = Cin, Wd = W, Hd = H;
-  uint32_t box[4] = {128, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TB};
-  if (!stride2) {
-    uint64_t dims[4] = {C, Wd, Hd, (uint64_t)B}; uint64_t str[3] = {C, Wd * C, Hd * Wd * C};
-    return make_tmap_u8(&p.tma_a[0], x, 4, dims, str, box);
-  }
-  for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
-    const uint8_t* base = reinterpret_cast<const uint8_t*>(x) + ((uint64_t)py * Wd + px) * C;
-    uint64_t dims[4] = {C, Wd / 2, Hd / 2, (uint64_t)B}; uint64_t str[3] = {2 * C, 2 * Wd * C, Hd * Wd * C};
-    const int rc = make_tmap_u8(&p.tma_a[py * 2 + px], base, 4, dims, str, box); if (rc) return rc;
-  }
-  return MMG_OK;
-}
-
+// convolution of the same shape takes; the register epilogue first dequantises with x_scale[image] * w_scale[col].  Shapes the kernel
+// does not take are argument errors: there is no other e4m3 convolution kernel.
 extern "C" int mmg_conv2d_fp8(const mmg_conv2d_fp8_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->x && a->w && a->x_scale && a->w_scale, "mmg_conv2d_fp8: NULL operand or scale");
@@ -412,26 +421,14 @@ extern "C" int mmg_conv2d_fp8(const mmg_conv2d_fp8_args* a, void* stream) {
                 "mmg_conv2d_fp8: epilogue %d (STORE, RESIDUAL or GLU)", a->epilogue);
   MMG_CHECK_ARG(a->epi.act != 2, "mmg_conv2d_fp8: ReLU epilogues are offered by mmg_linear only");
   ConvGeom g; conv_geom(a->kind, a->B, a->H, a->W, a->Cin, &g);
-  const int64_t M = (int64_t)a->B * g.Ho * g.Wo, N = a->Cout, K = (int64_t)g.ntaps * a->Cin;
+  const int64_t N = a->Cout, K = (int64_t)g.ntaps * a->Cin;
   int rc = validate_epilogue(a->epilogue, a->epi, N); if (rc) return rc;
   TcGemmParams p{};
   MMG_CHECK_ARG(tile_geometry(g.Ho, g.Wo, &p) == 0, "mmg_conv2d_fp8: no conv tile geometry for a %d x %d output", g.Ho, g.Wo);
-  p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 128; p.ntaps = g.ntaps; p.num_kb = p.ntaps * p.cchunks;
-  p.Ho = g.Ho; p.Wo = g.Wo; p.B = a->B;
-  p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
   p.epi.p = a->epi; p.epi.kind = a->epilogue;
   p.a_scale = a->x_scale; p.w_scale = a->w_scale;
-  rc = fp8_image_maps(p, a->x, a->B, a->H, a->W, a->Cin, a->kind == 2); if (rc) return rc;
-  if (a->kind != 2) {
-    for (int t = 0; t < g.ntaps; ++t) { p.tap_map[t] = 0; p.tap_dy[t] = g.tdy[t]; p.tap_dx[t] = g.tdx[t]; }
-  } else {
-    for (int r = 0; r < 4; ++r) for (int s = 0; s < 4; ++s) {
-      const int oy = r - 1, ox = s - 1;
-      const int py = ((oy % 2) + 2) % 2, px = ((ox % 2) + 2) % 2;
-      p.tap_map[r * 4 + s] = (int8_t)(py * 2 + px); p.tap_dy[r * 4 + s] = (int8_t)((oy - py) / 2); p.tap_dx[r * 4 + s] = (int8_t)((ox - px) / 2);
-    }
-  }
-  return launch_conv_fp8(p, a->w, N, K, st);
+  rc = conv_operand(p, g, a->x, true, N); if (rc) return rc;
+  return dispatch_tc(p, true, a->w, K, K, st);
 }
 
 extern "C" int mmg_conv_transpose2d_fp8(const mmg_conv_transpose2d_fp8_args* a, void* stream) {
@@ -444,24 +441,22 @@ extern "C" int mmg_conv_transpose2d_fp8(const mmg_conv_transpose2d_fp8_args* a, 
   MMG_CHECK_ARG(aligned16(a->x) && aligned16(a->w) && aligned8(a->w_scale), "mmg_conv_transpose2d_fp8: x and w need 16-byte alignment, w_scale 8-byte alignment");
   MMG_CHECK_ARG(a->epilogue == MMG_EPI_CONVT_RGB ? (a->Cout == 64 || a->Cout == 128 || a->Cout == 256) : (a->epi.ldo % 8 == 0),
                 "mmg_conv_transpose2d_fp8: CONVT_RGB needs Cout in {64, 128, 256}, CONVT epi.ldo %% 8 == 0");
-  const int64_t M = (int64_t)a->B * a->H * a->W, N = a->Cout, K = 4 * (int64_t)a->Cin;
+  const int64_t N = a->Cout, K = 4 * (int64_t)a->Cin;
   int rc;
   { mmg_epilogue_args e = a->epi; e.H = a->H; e.W = a->W; rc = validate_epilogue(a->epilogue, e, N); if (rc) return rc; }
   TcGemmParams p{};
   MMG_CHECK_ARG(tile_geometry(a->H, a->W, &p) == 0, "mmg_conv_transpose2d_fp8: no conv tile geometry for a %d x %d input", a->H, a->W);
-  p.M = M; p.N = N; p.mode = 1; p.cchunks = a->Cin / 128; p.ntaps = 4; p.num_kb = 4 * p.cchunks;
-  p.Ho = a->H; p.Wo = a->W; p.B = a->B;
-  p.num_m_tiles = p.tiles_x * p.tiles_y * ((a->B + p.TB - 1) / p.TB);
   p.a_scale = a->x_scale;
-  rc = fp8_image_maps(p, a->x, a->B, a->H, a->W, a->Cin, false); if (rc) return rc;
+  ConvGeom g; conv_geom(CONVT_PARITY, a->B, a->H, a->W, a->Cin, &g);
+  rc = conv_operand(p, g, a->x, true, N); if (rc) return rc;            // one A map: every parity class reads the same input grid
   for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px) {
     TcGemmParams q = p;
     q.epi.p = a->epi; q.epi.kind = a->epilogue;
     q.epi.p.H = a->H; q.epi.p.W = a->W; q.epi.p.py = py; q.epi.p.px = px;
     q.w_scale = a->w_scale + (size_t)(py * 2 + px) * N;
-    for (int t = 0; t < 4; ++t) { q.tap_map[t] = 0; q.tap_dy[t] = (int8_t)CT_D[py][t >> 1]; q.tap_dx[t] = (int8_t)CT_D[px][t & 1]; }
+    conv_geom(CONVT_PARITY + py * 2 + px, a->B, a->H, a->W, a->Cin, &g); conv_taps(q, g);
     const uint8_t* wp = reinterpret_cast<const uint8_t*>(a->w) + (size_t)(py * 2 + px) * N * K;
-    rc = launch_conv_fp8(q, wp, N, K, st); if (rc) return rc;
+    rc = dispatch_tc(q, true, wp, K, K, st); if (rc) return rc;
   }
   return MMG_OK;
 }
@@ -485,25 +480,15 @@ extern "C" int mmg_conv_transpose2d(const mmg_conv_transpose2d_args* a, void* st
     Epilogue epi; epi.p = a->epi; epi.kind = a->epilogue;
     epi.p.H = a->H; epi.p.W = a->W; epi.p.py = py; epi.p.px = px;
     const uint8_t* wp = reinterpret_cast<const uint8_t*>(a->w) + (size_t)(py * 2 + px) * N * K * esz;
+    ConvGeom g{}; conv_geom(CONVT_PARITY + py * 2 + px, a->B, a->H, a->W, a->Cin, &g);
     if (!tc_ok) {
-      ConvGeom g{}; g.B = a->B; g.H = a->H; g.W = a->W; g.Cin = a->Cin; g.Ho = a->H; g.Wo = a->W; g.stride = 1; g.ntaps = 4;
-      for (int t = 0; t < 4; ++t) { g.tdy[t] = (int8_t)CT_D[py][t >> 1]; g.tdx[t] = (int8_t)CT_D[px][t & 1]; }
       rc = launch_simt<true>(a->dtype, a->x, wp, M, N, K, 0, K, g, epi, st); if (rc) return rc;
       continue;
     }
     TcGemmParams q = p;
-    q.M = M; q.N = N; q.mode = 1; q.cchunks = a->Cin / 64; q.ntaps = 4; q.num_kb = 4 * q.cchunks;
-    q.Ho = a->H; q.Wo = a->W; q.B = a->B;
-    q.num_m_tiles = q.tiles_x * q.tiles_y * ((a->B + q.TB - 1) / q.TB);
     q.epi = epi;
-    const uint64_t C = a->Cin, W = a->W, H = a->H;
-    uint64_t dims[4] = {C, W, H, (uint64_t)a->B}; uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
-    uint32_t box[4] = {64, (uint32_t)q.TW, (uint32_t)q.TH, (uint32_t)q.TB};
-    rc = make_tmap_bf16(&q.tma_a[0], a->x, 4, dims, str, box); if (rc) return rc;
-    for (int t = 0; t < 4; ++t) { q.tap_map[t] = 0; q.tap_dy[t] = (int8_t)CT_D[py][t >> 1]; q.tap_dx[t] = (int8_t)CT_D[px][t & 1]; }
-    const int bn = pick_bn(q.num_m_tiles, N, a->epilogue);
-    rc = dispatch_tc(q, bn, wp, N, K, K, st); if (rc) return rc;
+    rc = conv_operand(q, g, a->x, false, N); if (rc) return rc;
+    rc = dispatch_tc(q, false, wp, K, K, st); if (rc) return rc;
   }
   return MMG_OK;
 }
-

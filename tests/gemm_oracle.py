@@ -48,14 +48,15 @@ GELU_ABS = 6e-7
 TANH_APPROX = 2.0 ** -12
 
 # epilogue kinds (include/mmg.h)
-STORE, RESIDUAL, GEGLU, GLU, QKV, CONVT, CONVT_RGB, LNFOLD, LFQ_IDS, ARGMIN, GEGLU_TANH = range(11)
+STORE, RESIDUAL, GEGLU, GLU, QKV, CONVT, CONVT_RGB, LNFOLD, LFQ_IDS, ARGMIN, GEGLU_TANH, QKV128 = range(12)
 # tc_gemm_kernel EPI_MODE values (mmg_gemm_tc.cuh)
-M_REGS, M_REDUCE, M_TSTORE, M_QKV, M_GEGLU, M_ACT = 0, 2, 3, 4, 5, 6
+M_REGS, M_REDUCE, M_TSTORE, M_QKV, M_GEGLU, M_ACT, M_QKV128 = 0, 2, 3, 4, 5, 6, 7
 SPLIT3 = "split3_kernel"
+E4M3 = "__nv_fp8_e4m3"
 
 
-def TC(bn, mode):
-    return f"tc_gemm_kernel<{bn}, {mode}, __nv_bfloat16>"
+def TC(bn, mode, ta="__nv_bfloat16"):
+    return f"tc_gemm_kernel<{bn}, {mode}, {ta}>"
 
 
 def SIMT(dtype, conv, act):
@@ -114,8 +115,8 @@ def is_act(kind, e):
 
 
 def tc_plan(kind, e, M, N, K, m_tiles, sms, conv):
-    """(tile width, EPI_MODE, n_fast) of dispatch_tc.  e: out ('f32' | 'bf16'), act, bias, in_place (out is resid with ldr == ldo), ldo,
-    out_aligned (16 bytes), tokens, nq / nk / nv heads, qkv_aligned."""
+    """(tile width, EPI_MODE, n_fast) of plan_tc for bf16 operands.  e: out ('f32' | 'bf16'), act, bias, in_place (out is resid with
+    ldr == ldo), ldo, out_aligned (16 bytes), tokens, nq / nk / nv heads, qkv_aligned."""
     bn = pick_bn(m_tiles, N, kind, sms)
     if is_act(kind, e):
         return 128, M_ACT, n_fast(N, K, (N + 127) // 128)
@@ -131,6 +132,18 @@ def tc_plan(kind, e, M, N, K, m_tiles, sms, conv):
     if mode != M_REGS and N % bn:
         raise ValueError("tile epilogue: tile width does not divide N")
     return bn, mode, n_fast(N, K, (N + bn - 1) // bn)
+
+
+def fp8_plan(kind, M, N, K, sms):
+    """(tile width, EPI_MODE, n_fast) of mmg_linear_fp8 (QKV, QKV128 or GEGLU; its argument checks refuse the shapes the tile epilogues
+    do not take).  An e4m3 dense product has no register-epilogue instantiation, so it always takes its tile epilogue: QKV and QKV128 at
+    256 where pick_bn gives 256 and at 128 otherwise, GEGLU at 256.  This differs from tc_plan at small M: a 256-row cross-attention q
+    product with N = 128 runs <128, QKV, e4m3> where the bf16 product of that shape runs <64, REGS>."""
+    if kind == GEGLU:
+        bn, mode = 256, M_GEGLU
+    else:
+        bn, mode = 256 if pick_bn((M + 127) // 128, N, kind, sms) == 256 else 128, M_QKV if kind == QKV else M_QKV128
+    return bn, mode, n_fast(N, K, N // bn)
 
 
 def linear_kernels(M, N, K, kind, e, *, dtype="bf16", sms=132, lda=None, ldw=None, a_aligned=True, w_aligned=True, split=False, order=False):

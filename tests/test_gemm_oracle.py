@@ -92,6 +92,13 @@ def test_dispatch_table():
     assert G.linear_kernels(58 * 128, 1024, 64, G.STORE, F32, sms=132) == [TC(128, G.M_TSTORE)]
     assert G.linear_kernels(58 * 128, 1024, 64, G.GEGLU, {"out": "bf16"}, sms=114) == [TC(256, G.M_GEGLU)]
     assert G.linear_kernels(58 * 128, 1024, 64, G.GEGLU, {"out": "bf16"}, sms=132) == [TC(128, G.M_REGS)]
+    # e4m3 (mmg_linear_fp8) always takes its tile epilogue: the small-M cross-attention q product runs <128, QKV> where bf16 runs <64, REGS>
+    assert G.fp8_plan(G.QKV, 256, 128, 128, 132) == (128, G.M_QKV, 0)
+    assert G.linear_kernels(256, 128, 128, G.QKV, {"out": "bf16", "tokens": 64, "nk": 0, "nv": 0}, sms=132) == [TC(64, G.M_REGS)]
+    assert G.fp8_plan(G.QKV, 32768, 1536, 512, 132) == (256, G.M_QKV, 1)
+    assert G.fp8_plan(G.QKV128, 384, 768, 256, 132) == (128, G.M_QKV128, 1)
+    assert G.fp8_plan(G.GEGLU, 129, 2816, 256, 132) == (256, G.M_GEGLU, 1)
+    assert G.fp8_plan(G.GEGLU, 1000, 4352, 512, 132) == (256, G.M_GEGLU, 0)                  # 17 column tiles
 
 
 def test_tile_geometry():

@@ -3,21 +3,29 @@
   mmg_layernorm_fp8: bytes and row scales equal the CPU oracle (tests/fp8_oracle.py) applied to mmg_layernorm's fp32 output, bit for bit,
   with and without the add / x_out / add_from fold;
   mmg_linear_fp8: <256, QKV> (self QKV), <128, QKV> (cross q), <256, GEGLU> (FF1) against fp64 on the dequantised operands, through the
-  epilogue's math, at C3 shapes and smaller / ragged M; unsupported shapes raise;
+  epilogue's math, at C3 shapes and smaller / ragged M, in both tile orders; unsupported shapes raise.  Which instantiation each case
+  reached (tests/gemm_oracle.py's fp8_plan) is asserted from torch.profiler captures taken in a child process
+  (test_linear_fp8_cases_reached_their_kernels runs those cases again with MMG_FP8_PROFILE=1), as in tests/test_gpu_gemm.py;
   C3 full-config teacher-forced flip rate against the fp32 oracle; generate() determinism, eager vs CUDA graph; inpaint; MaskGit.forward
   against the fp32 loss; the precision="fp8" rejections.
 """
 import math
+import os
+import subprocess
+import sys
 
 import numpy as np
 import pytest
 import torch
 
 from tests import fp8_oracle as Q
+from tests import gemm_oracle as G
+from tests.test_gpu_row_kernels import kernels_of, assert_ran
 
 pytestmark = pytest.mark.gpu
 torch.set_grad_enabled(False)
 E4 = torch.float8_e4m3fn
+PROFILE = os.environ.get("MMG_FP8_PROFILE") == "1"
 
 
 def M():
@@ -76,6 +84,24 @@ def test_layernorm_fp8_pads_columns_past_width():
 
 
 # ------------------------------------------------------------------------------------------------ e4m3 GEMM
+@pytest.fixture(scope="module", autouse=True)
+def _warm_up():
+    if PROFILE and torch.cuda.is_available():
+        kernels_of(lambda: torch.ones(8, device="cuda").sum())
+
+
+def run_planned(fn, kind, M, N, K, bn, order):
+    """fn(), one mmg_linear_fp8 call the case builds for tile width bn and tile order order ('n' or 'm' fastest), both checked against
+    gemm_oracle.fp8_plan; in the profiling process also that exactly the planned instantiation ran"""
+    pbn, mode, nf = G.fp8_plan(kind, M, N, K, torch.cuda.get_device_properties(0).multi_processor_count)
+    assert (pbn, nf) == (bn, int(order == "n")), f"built for <{bn}> {order}-fast, the plan gives <{pbn}> n_fast = {nf}"
+    if PROFILE:
+        _, names = kernels_of(fn)
+        assert_ran(names, G.TC(bn, mode, G.E4M3))
+    else:
+        fn()
+
+
 def fp8_operands(Mr, N, K, seed):
     g = torch.Generator(device="cuda").manual_seed(seed)
     a = (torch.randn((Mr, K), device="cuda", generator=g) * 120).clamp(-448, 448).to(E4)
@@ -90,10 +116,12 @@ def gelu64(x):
     return 0.5 * x * (1 + torch.erf(x / math.sqrt(2)))
 
 
-@pytest.mark.parametrize("Mr,K,tokens,heads,cross", [(32768, 512, 256, 8, False), (384, 256, 32, 4, False),
-                                                       (16384, 512, 256, 8, True), (256, 128, 64, 2, True)],
-                         ids=["self-C3", "self-small", "cross-C3", "cross-small"])
-def test_linear_fp8_qkv_vs_fp64(Mr, K, tokens, heads, cross):
+# (256, 'n'): 6 column tiles; (256, 'm'): 18 column tiles; cross-small: 256 rows, one 128-column tile (the bf16 product runs <64, REGS>)
+@pytest.mark.parametrize("Mr,K,tokens,heads,cross,bn,order", [(32768, 512, 256, 8, False, 256, "n"), (384, 256, 32, 4, False, 128, "n"),
+                                                              (16384, 512, 256, 8, True, 128, "n"), (256, 128, 64, 2, True, 128, "m"),
+                                                              (2048, 256, 64, 24, False, 256, "m")],
+                         ids=["self-C3", "self-small", "cross-C3", "cross-small", "self-mfast"])
+def test_linear_fp8_qkv_vs_fp64(Mr, K, tokens, heads, cross, bn, order):
     o = ops()
     inner = heads * 64
     N = inner if cross else 3 * inner
@@ -111,7 +139,7 @@ def test_linear_fp8_qkv_vs_fp64(Mr, K, tokens, heads, cross):
         nk = torch.randn((heads, 64), device="cuda", generator=g).bfloat16()
         nv = torch.randn((heads, 64), device="cuda", generator=g).bfloat16()
         epi = o.qkv_epilogue(torch.bfloat16, heads, tokens, q=q, k=k, v=v, q_scale=qs, k_scale=ks, key_off=1, null_k=nk, null_v=nv)
-    o.linear_fp8(a, sa, w, sw, None, epilogue=o.EPI_QKV, epi=epi)
+    run_planned(lambda: o.linear_fp8(a, sa, w, sw, None, epilogue=o.EPI_QKV, epi=epi), G.QKV, Mr, N, K, bn, order)
     # [bsz, tokens, part, heads, 64] fp64 reference, heads laid out [q heads | k heads | v heads] along N
     R = ref.view(bsz, tokens, -1, heads, 64)
     Sm = S.view(bsz, tokens, -1, heads, 64)
@@ -133,14 +161,14 @@ def test_linear_fp8_qkv_vs_fp64(Mr, K, tokens, heads, cross):
     print(f"QKV fp8 M={Mr} N={N} K={K}: largest |err| / sum|a w| = {worst:.2e}")
 
 
-@pytest.mark.parametrize("Mr,K", [(32768, 512), (1000, 512), (129, 256)], ids=["C3", "ragged-1000", "ragged-129"])
-def test_linear_fp8_geglu_vs_fp64(Mr, K):
+@pytest.mark.parametrize("Mr,N,K,order", [(32768, 2816, 512, "n"), (1000, 2816, 512, "n"), (129, 2816, 256, "n"), (1000, 4352, 512, "m")],
+                         ids=["C3", "ragged-1000", "ragged-129", "mfast-17-tiles"])
+def test_linear_fp8_geglu_vs_fp64(Mr, N, K, order):
     o = ops()
-    N = 2816
     a, w, sa, sw, ref, S = fp8_operands(Mr, N, K, Mr)
     h = torch.empty((Mr, N // 2), device="cuda", dtype=torch.bfloat16)
     stats = torch.full((Mr, N // 64, 2), float("nan"), device="cuda")
-    o.linear_fp8(a, sa, w, sw, h, epilogue=o.EPI_GEGLU, row_stats=stats)
+    run_planned(lambda: o.linear_fp8(a, sa, w, sw, h, epilogue=o.EPI_GEGLU, row_stats=stats), G.GEGLU, Mr, N, K, 256, order)
     R, Sv = ref.view(Mr, N // 64, 2, 32), S.view(Mr, N // 64, 2, 32)
     xr, gr, sx, sg = R[:, :, 0], R[:, :, 1], Sv[:, :, 0], Sv[:, :, 1]
     ref_o = (gr * gelu64(xr)).reshape(Mr, N // 2)
@@ -174,6 +202,19 @@ def test_linear_fp8_rejects_unsupported_shapes():
     a, w, sa, sw, _, _ = fp8_operands(256, 256, 128, 4)           # epilogues other than QKV / GEGLU
     with pytest.raises(_lib.MMGError, match="QKV or GEGLU"):
         o.linear_fp8(a, sa, w, sw, torch.empty((256, 256), device="cuda", dtype=torch.bfloat16), epilogue=o.EPI_STORE)
+
+
+def test_linear_fp8_cases_reached_their_kernels():
+    """the e4m3 product cases of this file again, in a fresh process, each under torch.profiler: profiler sessions early in a whole-suite
+    process make later captures come back empty"""
+    if PROFILE:
+        pytest.skip("this is the profiling process")
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-q", "-rP", "-m", "gpu", "-k", "linear_fp8 and vs_fp64",
+                        "--no-header", "-p", "no:cacheprovider"], cwd=root, env=dict(os.environ, MMG_FP8_PROFILE="1"), capture_output=True,
+                       text=True, timeout=600)
+    print(r.stdout[-6000:])
+    assert r.returncode == 0, r.stdout[-6000:] + r.stderr[-2000:]
 
 
 # ------------------------------------------------------------------------------------------------ end to end

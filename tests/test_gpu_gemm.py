@@ -221,7 +221,7 @@ def test_plain_fp32_tile_store(M, N, K, order):
 @pytest.mark.parametrize("route", ["oop-bn64", "oop-bn128", "oop-lowered-256", "bf16", "act", "inplace-ldo4", "inplace-misaligned"])
 def test_residual_register_routes(route):
     """out != resid (the prefetch route, with the next chunk's residual fetched early: every register-epilogue RESIDUAL runs at BN <= 128,
-    since dispatch_tc lowers BN = 256 to 128 for all but CONVT_RGB), bf16 RESIDUAL, RESIDUAL with act, and in place where the TMA reduction
+    since plan_tc lowers BN = 256 to 128 for all but CONVT_RGB), bf16 RESIDUAL, RESIDUAL with act, and in place where the TMA reduction
     does not take it: ldo % 8 != 0 (which also takes bf16 operands to the CUDA cores) and an `out` 8 bytes off a 16-byte boundary, which
     reaches the register epilogue in place with its residual read and its output written element by element"""
     M, N = {"oop-bn128": (300, 1024), "oop-lowered-256": (8400, 1024)}.get(route, (300, 192))
