@@ -1261,8 +1261,13 @@ class Muse(nn.Module):
         lowres = self.base_maskgit.generate(texts=texts, cond_scale=cond_scale, temperature=temperature, timesteps=timesteps)
         superres = self.superres_maskgit.generate(texts=texts, cond_scale=cond_scale, cond_images=lowres, temperature=temperature,
                                                   timesteps=superres_timesteps if superres_timesteps is not None else timesteps)
-        if return_pil_images:
-            import torchvision.transforms as T
-            lowres = list(map(T.ToPILImage(), lowres))
-            superres = list(map(T.ToPILImage(), superres))
-        return (superres, lowres) if return_lowres else superres
+        return _muse_result(superres, lowres, return_lowres, return_pil_images)
+
+
+def _muse_result(superres, lowres, return_lowres, return_pil_images):
+    """What Muse.forward returns for the cascade's image tensors (parallel.muse_sharded converts after its all-gather)."""
+    if return_pil_images:
+        import torchvision.transforms as T
+        lowres = None if lowres is None else list(map(T.ToPILImage(), lowres))
+        superres = list(map(T.ToPILImage(), superres))
+    return (superres, lowres) if return_lowres else superres

@@ -1,13 +1,16 @@
-"""Batch-sharded generation over the GPUs of one node (SURVEY.md 8e): every sequence is independent through the whole
-of generate(), so rank r generates a contiguous slice of the batch with replicated weights and the decoded images are
-assembled with ONE all-gather at the end.  No collective runs inside the decode loop.  The sampler's Philox counters are
+"""Batch-sharded generation and editing over the GPUs of one node (SURVEY.md 8e): every sequence is independent through the whole
+of generate(), inpaint(), edit() and the Muse cascade, so rank r runs a contiguous slice of the batch with replicated weights and the
+results are assembled with all-gathers at the end.  No collective runs inside the decode loop.  The sampler's Philox counters are
 keyed on the global sequence index (MaskGit.row_offset), so token ids do not depend on the number of ranks."""
 import numbers
 
 import torch
 import torch.distributed as dist
 
+from .muse_maskgit import _muse_result
+
 PER_IMAGE_SETTINGS = ("temperature", "cond_scale", "critic_noise_scale")
+ROW_INPUTS = ("images", "mask", "cond_images")      # call inputs indexed by global row, sliced like `texts`
 
 
 def shard_bounds(total, rank, world):
@@ -39,51 +42,145 @@ def gather_batch(local, total, group=None):
     return torch.cat(pieces, 0)
 
 
-def generate_sharded(maskgit, texts, text_embeds=None, cond_images=None, group=None, *, text_embeds_shard=None, cond_images_shard=None,
-                     seed=None, **generate_kwargs):
-    """maskgit.generate over this rank's slice of `texts`, then one all-gather.  Returns the full batch on every rank.
+def _gather(local, total, group):
+    """gather_batch of a call's result: one tensor, or each tensor of an (images, ids) tuple."""
+    if isinstance(local, tuple):
+        return tuple(gather_batch(t, total, group) for t in local)
+    return gather_batch(local, total, group)
 
-    Inputs indexed by GLOBAL row (`text_embeds` [B, L, D], `cond_images` [B, ...]) are sliced here; a caller whose loader already
-    holds only its own rows passes `text_embeds_shard` / `cond_images_shard` (rows [lo, hi) of shard_bounds) instead.
 
-    The sampler noise is keyed on the global sequence index, so the token ids do not depend on the number of ranks:
-    "mmg" mode uses ONE seed for all ranks — `seed` when the caller passes the same value on every rank (no communication), else rank
-    0's `sampler_seed` or its draw from torch's generator, broadcast; "aten" mode is told the size of the whole batch the reference would
-    have drawn noise for (`global_batch`)."""
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
-    rank = dist.get_rank(group) if dist.is_initialized() else 0
-    total = len(texts)
-    lo, hi = shard_bounds(total, rank, world)
+def _empty_result(maskgit, return_ids=False, fmap_size=None):
+    """What a rank without rows contributes: (0, C, S, S) fp32 images and, with return_ids, (0, f, f) int64 ids, on the model's device."""
+    device = next(maskgit.parameters()).device
+    size = maskgit.image_size
+    images = torch.empty((0, maskgit.vae.channels, size, size), dtype=torch.float32, device=device)
+    if not return_ids:
+        return images
+    f = fmap_size if fmap_size is not None else maskgit.vae.get_encoded_fmap_size(size)
+    return images, torch.empty((0, f, f), dtype=torch.int64, device=device)
+
+
+def _run_shard(method, maskgits, texts, lo, hi, total, empty, *, group=None, seeds=None, text_embeds=None, text_embeds_shard=None,
+               cond_images_shard=None, **kwargs):
+    """method(texts[lo:hi], **kwargs) as the holder of rows [lo, hi) of a batch of `total` images; returns this rank's result, or
+    empty() when lo == hi.  Every rank of `group` must call it, with its own (lo, hi): the seeds are one broadcast.
+
+    maskgits: the MaskGits `method` samples with, in the order one process draws their seeds.  Each gets row_offset = lo, global_batch =
+    total and one seed shared by every rank: seeds[i] when given (no communication), else its sampler_seed or a draw from torch's
+    generator, as rank 0 of `group` has them.  text_embeds (rows of the whole batch) or text_embeds_shard (rows [lo, hi)) replace every
+    maskgit transformer's encode_text.  kwargs named in ROW_INPUTS and per-image settings given per image are indexed by global row and
+    sliced here; cond_images_shard replaces the slice of cond_images.  The attributes are restored on return, also when the call raises."""
     for name in PER_IMAGE_SETTINGS:       # per-image settings (a sequence or 1-D tensor of `total` values) are sliced like text_embeds
-        value = generate_kwargs.get(name)
+        value = kwargs.get(name)
         if value is None or isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
             continue
         if len(value) != total:
             raise ValueError(f"{name} has {len(value)} values for {total} texts")
-        generate_kwargs[name] = value[lo:hi]
-    tr = maskgit.transformer
-    saved = (tr.encode_text, maskgit.row_offset, maskgit.global_batch, maskgit.sampler_seed)
+        kwargs[name] = value[lo:hi]
+    for name in ROW_INPUTS:
+        value = kwargs.get(name)
+        if value is None:
+            continue
+        if len(value) != total:
+            raise ValueError(f"{name} has {len(value)} rows for {total} texts")
+        kwargs[name] = value[lo:hi]
+    if cond_images_shard is not None:
+        kwargs["cond_images"] = cond_images_shard
+    if seeds is None:
+        seeds = [m.sampler_seed if m.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item()) for m in maskgits]
+        if dist.is_initialized() and dist.get_world_size(group) > 1:
+            box = [seeds]
+            dist.broadcast_object_list(box, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+            seeds = box[0]
+    if text_embeds_shard is None and text_embeds is not None:
+        text_embeds_shard = text_embeds[lo:hi]
+    if text_embeds_shard is not None:
+        assert text_embeds_shard.shape[0] == hi - lo, "text_embeds_shard must hold exactly this rank's rows"
+    saved = [(m.transformer.encode_text, m.row_offset, m.global_batch, m.sampler_seed) for m in maskgits]
     try:
-        if seed is None:
-            seed = maskgit.sampler_seed if maskgit.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
-            if world > 1:
-                box = [seed]
-                dist.broadcast_object_list(box, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
-                seed = box[0]
-        maskgit.sampler_seed, maskgit.row_offset, maskgit.global_batch = seed, lo, total
-        if text_embeds_shard is None and text_embeds is not None:
-            text_embeds_shard = text_embeds[lo:hi]
-        if text_embeds_shard is not None:
-            assert text_embeds_shard.shape[0] == hi - lo, "text_embeds_shard must hold exactly this rank's rows"
-            shard = text_embeds_shard
-            tr.encode_text = lambda t: shard
-        if cond_images_shard is None and cond_images is not None:
-            cond_images_shard = cond_images[lo:hi]
+        for m, seed in zip(maskgits, seeds):
+            m.sampler_seed, m.row_offset, m.global_batch = seed, lo, total
+            if text_embeds_shard is not None:
+                m.transformer.encode_text = lambda t, shard=text_embeds_shard: shard
         if hi > lo:
-            local = maskgit.generate(texts[lo:hi], cond_images=cond_images_shard, **generate_kwargs)
-        else:       # more ranks than sequences: this rank contributes an empty shard of the right shape / dtype / device
-            size = maskgit.image_size
-            local = torch.empty((0, maskgit.vae.channels, size, size), dtype=torch.float32, device=next(maskgit.parameters()).device)
+            return method(texts[lo:hi], **kwargs)
+        return empty()            # more ranks than sequences: an empty shard of the right shape / dtype / device
     finally:
-        tr.encode_text, maskgit.row_offset, maskgit.global_batch, maskgit.sampler_seed = saved
-    return gather_batch(local, total, group)
+        for m, (encode_text, row_offset, global_batch, sampler_seed) in reversed(list(zip(maskgits, saved))):
+            m.transformer.encode_text, m.row_offset, m.global_batch, m.sampler_seed = encode_text, row_offset, global_batch, sampler_seed
+
+
+def _sharded_call(maskgit, method, texts, group, seed, kwargs):
+    """A MaskGit call over this rank's rows, then the all-gather of its result."""
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    total = len(texts)
+    lo, hi = shard_bounds(total, rank, world)
+    empty = lambda: _empty_result(maskgit, kwargs.get("return_ids", False), kwargs.get("fmap_size"))
+    local = _run_shard(method, (maskgit,), texts, lo, hi, total, empty, group=group, seeds=None if seed is None else (seed,), **kwargs)
+    return _gather(local, total, group)
+
+
+def generate_sharded(maskgit, texts, text_embeds=None, cond_images=None, group=None, *, text_embeds_shard=None, cond_images_shard=None,
+                     seed=None, **generate_kwargs):
+    """maskgit.generate over this rank's slice of `texts`, then one all-gather.  Returns the full batch on every rank (with
+    return_ids=True, the (images, ids) of the whole batch).
+
+    Inputs indexed by GLOBAL row (`text_embeds` [B, L, D], `cond_images` [B, ...], per-image settings) are sliced here; a caller whose
+    loader already holds only its own rows passes `text_embeds_shard` / `cond_images_shard` (rows [lo, hi) of shard_bounds) instead.
+
+    The sampler noise is keyed on the global sequence index, so the token ids do not depend on the number of ranks:
+    "mmg" mode uses ONE seed for all ranks — `seed` when the caller passes the same value on every rank (no communication), else rank
+    0's `sampler_seed` or its draw from torch's generator, broadcast; "aten" mode is told the size of the whole batch the reference would
+    have drawn noise for (`global_batch`).  Not with `sampler_noise_fn`: the callable sees only this rank's shape."""
+    return _sharded_call(maskgit, maskgit.generate, texts, group, seed,
+                         dict(generate_kwargs, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard, cond_images=cond_images,
+                              cond_images_shard=cond_images_shard))
+
+
+def inpaint_sharded(maskgit, texts, images, mask, text_embeds=None, cond_images=None, group=None, *, text_embeds_shard=None,
+                    cond_images_shard=None, seed=None, **inpaint_kwargs):
+    """maskgit.inpaint over this rank's rows, then the all-gather of the images (and ids with return_ids=True).  `images` and `mask`
+    (every form inpaint takes) are indexed by global row and sliced here, as are text_embeds, cond_images and per-image settings.  Each
+    rank counts the regenerated tokens of its own rows only, and samples mask_schedule(its largest count) rows per image and step.
+
+    Seeds and the rank-count invariance of the token ids are generate_sharded's: one seed for every rank in "mmg" mode, `global_batch`
+    in "aten" mode; not with `sampler_noise_fn`."""
+    return _sharded_call(maskgit, maskgit.inpaint, texts, group, seed,
+                         dict(inpaint_kwargs, images=images, mask=mask, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard,
+                              cond_images=cond_images, cond_images_shard=cond_images_shard))
+
+
+def edit_sharded(maskgit, texts, images, mask=None, text_embeds=None, cond_images=None, group=None, *, text_embeds_shard=None,
+                 cond_images_shard=None, seed=None, **edit_kwargs):
+    """maskgit.edit over this rank's rows, then the all-gather, sliced as inpaint_sharded (`mask` may be None: every token editable).
+    The selection keys are keyed on the global position too, so with one seed for every rank ("mmg" mode) the token ids do not depend
+    on the number of ranks.  sampler_rng = "aten" raises ValueError on every rank, as edit() does; `sampler_noise_fn` is not covered."""
+    if maskgit.sampler_rng == "aten":          # raised here, before any collective, so that ranks without rows raise it too
+        raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
+    return _sharded_call(maskgit, maskgit.edit, texts, group, seed,
+                         dict(edit_kwargs, images=images, mask=mask, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard,
+                              cond_images=cond_images, cond_images_shard=cond_images_shard))
+
+
+def muse_sharded(muse, texts, text_embeds=None, group=None, *, text_embeds_shard=None, **forward_kwargs):
+    """Muse.forward over this rank's texts: the base stage makes this rank's low-res images and the super-resolution stage, on the same
+    rank, is conditioned on them, so nothing is exchanged between the stages.  One all-gather of the super-resolution images (and one of
+    the low-res images with return_lowres) at the end; PIL conversion follows the gather, so every rank returns what Muse.forward returns.
+
+    Seeds: each stage's own `sampler_seed`, else a draw from torch's generator, base first, as one process draws them; rank 0's pair
+    reaches every rank in one broadcast.  text_embeds / text_embeds_shard are handed to both stages' transformers.  Per-image
+    cond_scale / temperature are sliced by global row.  Token ids do not depend on the number of ranks, as for generate_sharded."""
+    return_lowres = forward_kwargs.pop("return_lowres", False)
+    return_pil_images = forward_kwargs.pop("return_pil_images", True)
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    total = len(texts)
+    lo, hi = shard_bounds(total, rank, world)
+    base, superres = muse.base_maskgit, muse.superres_maskgit
+    empty = lambda: (_empty_result(superres), _empty_result(base))
+    hi_res, low_res = _run_shard(muse.forward, (base, superres), texts, lo, hi, total, empty, group=group, text_embeds=text_embeds,
+                                 text_embeds_shard=text_embeds_shard, return_lowres=True, return_pil_images=False, **forward_kwargs)
+    hi_res = gather_batch(hi_res, total, group)
+    low_res = gather_batch(low_res, total, group) if return_lowres else None
+    return _muse_result(hi_res, low_res, return_lowres, return_pil_images)
