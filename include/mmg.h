@@ -346,6 +346,20 @@ typedef struct {
 } mmg_edit_select_args;
 int mmg_edit_select(const mmg_edit_select_args* a, void* stream);
 
+/* one window of image extrapolation (MaskGit.extrapolate): moves the f x f block of the token canvas whose top-left token is
+ * (row0, col0) between the canvas and the decode buffers.  The window's strip is its `stride` columns (direction 0 "right": the last
+ * ones, 1 "left": the first ones) or rows (2 "down": the last ones, 3 "up": the first ones).  store == 0 (load): ids[b, i*f + j] =
+ * canvas[b, row0 + i, col0 + j], mask_id on the strip, and every score 0.  store == 1: the strip of ids is written into the canvas,
+ * nothing else changes.  The window must lie inside the canvas; 1 <= stride <= f <= 128.  No host synchronisation, no allocation. */
+typedef struct {
+  int64_t* canvas;                                    /* [B, canvas_h, canvas_w]                                    */
+  int64_t* ids; float* scores;                        /* [B, f*f], [B, f*f]                                         */
+  int32_t B, f, canvas_h, canvas_w;
+  int32_t row0, col0, direction, stride;
+  int32_t store, _pad; int64_t mask_id;
+} mmg_extrapolate_window_args;
+int mmg_extrapolate_window(const mmg_extrapolate_window_args* a, void* stream);
+
 /* Final LayerNorm + classifier-free-guidance combine on the masked rows only, in embedding space:
  *   e[j] = LN(x_null[r]) + (LN(x_cond[r]) - LN(x_null[r])) * cond_scale,  r = b*n + masked_pos[b, j]
  * (to_logits is linear and bias-free, so W e == null + (cond - null) * scale of muse_maskgit_pytorch.py:254).

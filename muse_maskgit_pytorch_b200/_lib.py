@@ -104,6 +104,11 @@ class EditSelectArgs(C.Structure):
                 ("row_offset", i64), ("B", i32), ("n", i32), ("iteration", i32), ("_pad", i32), ("mask_id", i64)]
 
 
+class ExtrapolateWindowArgs(C.Structure):
+    _fields_ = [("canvas", vp), ("ids", vp), ("scores", vp), ("B", i32), ("f", i32), ("canvas_h", i32), ("canvas_w", i32), ("row0", i32),
+                ("col0", i32), ("direction", i32), ("stride", i32), ("store", i32), ("_pad", i32), ("mask_id", i64)]
+
+
 class FinalEmbedArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("masked_pos", vp), ("e", vp), ("e_dtype", i32),
                 ("B", i32), ("n", i32), ("num_masked", i32), ("dim", i32), ("cond_scale", f32), ("cond_scale_dev", vp)]
@@ -200,7 +205,7 @@ EXPORTS = {
     "mmg_vq_decode_codes": DecodeCodesArgs, "mmg_cast": CastArgs, "mmg_split3": Split3Args, "mmg_critic_score": CriticScoreArgs,
     "mmg_ff_geglu": FfGegluArgs, "mmg_decode_step": DecodeStepArgs, "mmg_logits_fused": LogitsFusedArgs,
     "mmg_t5_attention": T5AttentionArgs, "mmg_rmsnorm": RmsNormArgs, "mmg_remask_frozen": RemaskFrozenArgs, "mmg_edit_select": EditSelectArgs,
-    "mmg_logits_xent": LogitsXentArgs, "mmg_logits_xent_rows": LogitsXentRowsArgs,
+    "mmg_extrapolate_window": ExtrapolateWindowArgs, "mmg_logits_xent": LogitsXentArgs, "mmg_logits_xent_rows": LogitsXentRowsArgs,
     "mmg_linear_fp8": LinearFp8Args, "mmg_layernorm_fp8": LayerNormFp8Args,
     "mmg_conv2d_fp8": Conv2dFp8Args, "mmg_conv_transpose2d_fp8": ConvTranspose2dFp8Args, "mmg_quantize_e4m3_images": QuantizeE4m3ImagesArgs,
 }

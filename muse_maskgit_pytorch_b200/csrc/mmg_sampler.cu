@@ -488,6 +488,30 @@ edit_select_kernel(const mmg_edit_select_args a) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// image extrapolation (MaskGit.extrapolate): one thread per window token.  Load copies the canvas block into ids with
+// mask_id on the strip and zeroes the scores; store writes the strip of ids back into the canvas.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+extrapolate_window_kernel(const mmg_extrapolate_window_args a) {
+  pdl_wait(); pdl_trigger();
+  const int nn = a.f * a.f;
+  const int64_t total = (int64_t)a.B * nn;
+  for (int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x; t < total; t += (int64_t)gridDim.x * 256) {
+    const int64_t b = t / nn;
+    const int p = (int)(t - b * nn), i = p / a.f, j = p - i * a.f;
+    const int k = a.direction < 2 ? j : i;                                   // position across the strip's axis
+    const bool strip = (a.direction & 1) ? k < a.stride : k >= a.f - a.stride;
+    const int64_t c = (b * a.canvas_h + a.row0 + i) * a.canvas_w + a.col0 + j;
+    if (a.store) {
+      if (strip) a.canvas[c] = a.ids[t];
+    } else {
+      a.ids[t] = strip ? a.mask_id : a.canvas[c];
+      a.scores[t] = 0.f;
+    }
+  }
+}
+
 
 // ---------------------------------------------------------------------------------------------------------------
 // token-critic scores (muse_maskgit_pytorch.py:590-600): per sequence position, the dim_out = 1 head applied to the
@@ -599,6 +623,22 @@ extern "C" int mmg_edit_select(const mmg_edit_select_args* a, void* stream) {
   static const cudaError_t attr = cudaFuncSetAttribute(edit_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 9);
   if (attr != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(edit_select): %s", cudaGetErrorString(attr));
   MMG_CUDA(launch_pdl(edit_select_kernel, dim3(a->B), dim3(256), smem, st, *a));
+  MMG_LAUNCHED();
+  return MMG_OK;
+}
+
+extern "C" int mmg_extrapolate_window(const mmg_extrapolate_window_args* a, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MMG_CHECK_ARG(a && a->canvas && a->ids && a->scores, "mmg_extrapolate_window: NULL pointer");
+  MMG_CHECK_ARG(a->B >= 0 && a->f > 0 && a->f <= 128 && a->stride >= 1 && a->stride <= a->f && a->direction >= 0 && a->direction <= 3 &&
+                (a->store == 0 || a->store == 1), "mmg_extrapolate_window: B=%d f=%d stride=%d direction=%d store=%d", a->B, a->f, a->stride,
+                a->direction, a->store);
+  MMG_CHECK_ARG(a->row0 >= 0 && a->col0 >= 0 && (int64_t)a->row0 + a->f <= a->canvas_h && (int64_t)a->col0 + a->f <= a->canvas_w,
+                "mmg_extrapolate_window: window at (%d, %d) of size %d outside the %d x %d canvas", a->row0, a->col0, a->f, a->canvas_h,
+                a->canvas_w);
+  if (a->B == 0) return MMG_OK;
+  const int64_t blocks = ((int64_t)a->B * a->f * a->f + 255) / 256;
+  MMG_CUDA(launch_pdl(extrapolate_window_kernel, dim3((unsigned)(blocks < 65535 ? blocks : 65535)), dim3(256), 0, st, *a));
   MMG_LAUNCHED();
   return MMG_OK;
 }

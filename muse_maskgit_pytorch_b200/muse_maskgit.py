@@ -540,13 +540,31 @@ def regen_tokens(mask, b, image_size, fmap_size):
 
 
 @dataclasses.dataclass(frozen=True)
+class _Window:
+    """extrapolate()'s window plan, in tokens: the canvas (canvas_h, canvas_w), where the encoded input sits in it (row, col), and the
+    top-left token (row0, col0) of each f x f window in order.  Every window regenerates the `stride` columns (rows) at its far side."""
+    direction: str
+    stride: int
+    canvas: tuple
+    input_at: tuple
+    corners: tuple
+
+    @property
+    def key(self):
+        return ("extrapolate", self.direction, len(self.corners), self.stride, self.canvas)
+
+
+@dataclasses.dataclass(frozen=True)
 class _Region:
-    """The tokens inpaint() regenerates or edit() resamples.  n_max: the most an image regenerates per round (its schedule gives the rows
-    sampled per step); iterations: None for inpaint(), else edit()'s rounds, each opened by an mmg_edit_select that writes its frozen map;
-    tensors: images, counts int32 [timesteps, b], and frozen uint8 [b, n] or keep uint8 [b, n] (1 = not editable) + num_select int32 [b]."""
+    """The tokens inpaint() regenerates, edit() resamples or extrapolate() generates.  n_max: the most an image regenerates per round (its
+    schedule gives the rows sampled per step); iterations: None for inpaint(), else the rounds of edit() (each opened by an mmg_edit_select
+    that writes its frozen map) or of extrapolate() (one per window); tensors: images, counts int32 [timesteps, b], and frozen uint8 [b, n]
+    or keep uint8 [b, n] (1 = not editable) + num_select int32 [b]; window: extrapolate()'s plan, whose rounds load their window from the
+    token canvas and store its new strip back (frozen is then the map of every window: 1 outside the strip)."""
     n_max: int
     iterations: Optional[int]
     tensors: dict
+    window: Optional[_Window] = None
 
 
 def _per_image(name, value, b):
@@ -585,7 +603,7 @@ def _fill_on_device(t, device):
 
 @dataclasses.dataclass(frozen=True)
 class _DecodeRequest:
-    """One validated generate() / inpaint() / edit() call.  temperature, cond_scale, critic_noise_scale: one float per image.
+    """One validated generate() / inpaint() / edit() / extrapolate() call.  temperature, cond_scale, critic_noise_scale: one float per image.
     seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs)."""
     texts: List[str]
     cond_images: Optional[torch.Tensor]
@@ -782,17 +800,107 @@ class MaskGit(nn.Module):
                                           topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
                                           force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
 
+    @torch.no_grad()
+    def extrapolate(self, texts: List[str], images: torch.Tensor, direction="right", amount=256, stride=None, timesteps=18, cond_scale=3,
+                    temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False, force_not_use_token_critic=False, critic_noise_scale=1,
+                    return_ids=False):
+        """Grows `images` past their frame by `amount` pixels on one side (an extension, as inpaint() is; MaskGIT's image extrapolation),
+        window by window, on a token canvas that stays on the device.
+
+        images: fp32 NCHW (b, C, H, W).  direction "right" / "left": H = image_size and W >= image_size a multiple of the patch p = 2**layers
+        (an already widened image may be extended again); "down" / "up": the same with the axes swapped.  f = fmap_size; stride (tokens each
+        window generates, default f // 2) lies in [1, f]; amount is a positive multiple of stride * p, and K = amount / (stride * p) windows run.
+          1. The canvas is vae.encode_ids(images) at the kept side and mask_id everywhere else (H'/p x W'/p tokens).
+          2. Window w (0 <= w < K) is the f x f block whose far edge lies stride * (w + 1) tokens past the input's edge ("right": canvas
+             columns [W/p + stride (w + 1) - f, W/p + stride (w + 1))).  Its `stride` columns (rows) at the far side are generated, the rest
+             is frozen context read from the canvas.
+          3. The window runs exactly inpaint()'s token loop with that strip as the regenerated region: `timesteps` steps on the schedule
+             max(int(noise_schedule(t) * f * stride), 1), the temperature annealed over the window's steps, scores and the self-conditioning
+             embedding reset at its start.  Step s has the global step index w * timesteps + s, which keys the sampler's Philox streams
+             (global row (row_offset + b) * f * f + p with p window-local) and is the step passed to `sampler_noise_fn`.
+          4. The strip is then written into the canvas; after the last window one vae.decode_from_ids(canvas) gives the pixels.
+        Input tokens keep their encoded ids bit for bit and every new token is generated by exactly one window.  The defaults (stride f // 2,
+        18 steps per window) are this project's provisional choice.  Returns fp32 images (b, C, H', W') grown by `amount`, and with
+        return_ids the int64 canvas (b, H'/p, W'/p).  temperature, cond_scale and critic_noise_scale are per image or scalar, as for generate().
+        Raises ValueError before any launch on a wrong direction, amount, stride, timesteps or image shape, for sampler_rng = "aten" (no
+        reference stream), for a MaskGit conditioned on a low-resolution image, and for an fp8 VAE without conv tiles for the canvas.
+        `use_native_step` does not apply here, as for inpaint()."""
+        if isinstance(timesteps, bool) or not isinstance(timesteps, int) or timesteps < 1:
+            raise ValueError(f"timesteps must be an int >= 1, got {timesteps!r}")
+        b = len(texts)
+        window = self._extrapolate_plan(images, b, direction, amount, stride)
+        f = self.vae.get_encoded_fmap_size(self.image_size)
+        frozen = (~self._window_strip(direction, f, window.stride)).reshape(1, -1).to(torch.uint8).repeat(b, 1)
+        region = self._region(images, [f * window.stride] * b, timesteps, len(window.corners), window, frozen=frozen)
+        return self._decode(self._request(texts, temperature=temperature, timesteps=timesteps, region=region, cond_images=None,
+                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
+
     def _check_images(self, images, b):
         if not isinstance(images, torch.Tensor) or tuple(images.shape) != (b, self.vae.channels, self.image_size, self.image_size):
             raise ValueError(f"images must be a (b, {self.vae.channels}, {self.image_size}, {self.image_size}) tensor for b = {b} texts, got "
                              f"{tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__}")
 
-    def _region(self, images, counts, timesteps, iterations=None, **tensors):
+    def _region(self, images, counts, timesteps, iterations=None, window=None, **tensors):
         """The _Region of a call whose image b regenerates counts[b] tokens per round, on the schedule of that count (none: 0 throughout)."""
         table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in counts]
         tensors.update(images=images.to(torch.float32), counts=torch.tensor(table, dtype=torch.int32).t())        # counts: [timesteps, b]
         device = next(self.parameters()).device
-        return _Region(max(counts, default=0), iterations, {k: v.to(device).contiguous() for k, v in tensors.items()})
+        return _Region(max(counts, default=0), iterations, {k: v.to(device).contiguous() for k, v in tensors.items()}, window)
+
+    def _extrapolate_plan(self, images, b, direction, amount, stride):
+        """Validates extrapolate()'s arguments for b images (ValueError naming the constraint) and returns its _Window."""
+        if direction not in ops.EXTRAPOLATE_DIRECTIONS:
+            raise ValueError(f"direction must be one of {ops.EXTRAPOLATE_DIRECTIONS}, got {direction!r}")
+        if self.sampler_rng == "aten":
+            raise ValueError('extrapolate() has no "aten" noise stream (the reference has no extrapolation): use sampler_rng = "mmg" or '
+                             "sampler_noise_fn")
+        if self.resize_image_for_cond_image:
+            raise ValueError("extrapolate() does not run a MaskGit conditioned on a low-resolution image (cond_image_size / cond_vae): the "
+                             "conditioning image would have to grow with the canvas")
+        f = self.vae.get_encoded_fmap_size(self.image_size)
+        p = self.vae.dim_divisor
+        stride = f // 2 if stride is None else stride
+        if isinstance(stride, bool) or not isinstance(stride, int) or not 1 <= stride <= f:
+            raise ValueError(f"stride must be an int in [1, fmap_size = {f}], got {stride!r}")
+        if isinstance(amount, bool) or not isinstance(amount, int) or amount <= 0 or amount % (stride * p):
+            raise ValueError(f"amount must be a positive multiple of stride * patch = {stride} * {p} = {stride * p} pixels, got {amount!r}")
+        vertical = direction in ("down", "up")
+        C = self.vae.channels
+        shape = tuple(images.shape) if isinstance(images, torch.Tensor) else None
+        long_side = None if shape is None or len(shape) != 4 else shape[2 if vertical else 3]
+        ok = (long_side is not None and shape[:2] == (b, C) and shape[3 if vertical else 2] == self.image_size and long_side >= self.image_size
+              and long_side % p == 0)
+        if not ok:
+            want = (f"(b, {C}, H, {self.image_size}), H >= {self.image_size} a multiple of {p}" if vertical else
+                    f"(b, {C}, {self.image_size}, W), W >= {self.image_size} a multiple of {p}")
+            raise ValueError(f'images must be {want} for direction "{direction}" and b = {b} texts, got '
+                             f"{shape if shape is not None else type(images).__name__}")
+        K, grow, n_in = amount // (stride * p), amount // p, long_side // p
+        if vertical:
+            canvas, input_at = (n_in + grow, f), ((grow, 0) if direction == "up" else (0, 0))
+        else:
+            canvas, input_at = (f, n_in + grow), ((0, grow) if direction == "left" else (0, 0))
+        # first row / column of window w, whose far edge lies stride * (w + 1) tokens past the input's edge on the grown side
+        start = [n_in + stride * (w + 1) - f if direction in ("right", "down") else grow - stride * (w + 1) for w in range(K)]
+        corners = tuple((e, 0) if vertical else (0, e) for e in start)
+        if self.vae.precision == "fp8":
+            # the e4m3 convolutions have no CUDA-core fallback: every grid the input's encode and the canvas decode run at needs a tile
+            for what, (h, w) in (("input", shape[2:]), ("canvas", (canvas[0] * p, canvas[1] * p))):
+                for k in range(1, self.vae.enc_dec.layers + 1):
+                    if not VQGanVAE._tc_tile_ok(h >> k, w >> k):
+                        raise ValueError(f'VQGanVAE precision="fp8" has no conv tile geometry for the {h >> k} x {w >> k} feature map of the '
+                                         f'{h} x {w} {what}; use a VAE with precision="bf16" for this size')
+        return _Window(direction, stride, canvas, input_at, corners)
+
+    @staticmethod
+    def _window_strip(direction, f, stride):
+        """(f, f) bool: the tokens of a window that extrapolate() generates (its `stride` columns or rows at the far side)."""
+        strip = torch.zeros((f, f), dtype=torch.bool)
+        far = {"right": (slice(None), slice(f - stride, f)), "left": (slice(None), slice(0, stride)),
+               "down": (slice(f - stride, f), slice(None)), "up": (slice(0, stride), slice(None))}[direction]
+        strip[far] = True
+        return strip
 
     def _request(self, texts, *, force_not_use_token_critic, fmap_size=None, **settings):
         use_critic = self.token_critic is not None and not force_not_use_token_critic
@@ -832,7 +940,7 @@ class MaskGit(nn.Module):
         return net, nb, ctx, whead, bhead, net._packed()["gf"]
 
     def _decode(self, req):
-        """Runs a generate() / inpaint() / edit() request in eval mode.  A call whose fused tail overflowed is repeated on the materialised
+        """Runs a generate() / inpaint() / edit() / extrapolate() request in eval mode.  A call whose fused tail overflowed is repeated on the materialised
         path with the same noise: the same libmmg seed, or the ATen generator position the failed attempt started from."""
         was_training, saved = self.training, self.use_fused_tail
         self.eval()
@@ -886,7 +994,9 @@ class MaskGit(nn.Module):
                float(req.topk_filter_thres), int(req.timesteps), req.branches, int(self.row_offset),
                tr.precision, self.vae.precision, req.use_critic, bool(req.can_remask_prev_masked),
                None if aten is None else aten["key"], bool(self.use_native_step), id(self.noise_schedule), bool(self.use_fused_tail))
-        if req.region is not None:
+        if req.region is not None and req.region.window is not None:
+            key += (req.region.window.key,)
+        elif req.region is not None:
             key += (("inpaint", req.region.n_max) if req.region.iterations is None else ("edit", req.region.iterations, req.region.n_max),)
         critic_net = self.token_critic if isinstance(self.token_critic, Transformer) and req.use_critic else None
         pack_ids = lambda: (id(tr._pack), id(self.vae._pack), id(self.cond_vae._pack), id(critic_net._pack) if critic_net is not None else 0,
@@ -1031,9 +1141,17 @@ class MaskGit(nn.Module):
         ctx = tr._prepare_context(text_embeds, cond_ids, [False, True][:nb])
         P = tr._packed()
         adt = P["adt"]
-        edit = req.region is not None and req.region.iterations is not None
+        window = None if req.region is None else req.region.window
+        edit = req.region is not None and req.region.iterations is not None and window is None
         if req.region is None:
             ids = torch.full((b, n), self.mask_id, dtype=torch.long, device=device)
+        elif window is not None:      # the token canvas: the encoded input at the kept side, mask_id elsewhere; each round loads its window
+            canvas = torch.full((b,) + window.canvas, self.mask_id, dtype=torch.long, device=device)
+            known = self.vae.encode_ids(region["images"])
+            r, c = window.input_at
+            canvas[:, r:r + known.shape[1], c:c + known.shape[2]] = known
+            ids = torch.empty((b, n), dtype=torch.long, device=device)
+            frozen = region["frozen"]
         elif edit:
             ids = self.vae.encode_ids(region["images"]).reshape(b, n)
             frozen = torch.empty((b, n), dtype=torch.uint8, device=device)          # written by each round's mmg_edit_select
@@ -1064,13 +1182,16 @@ class MaskGit(nn.Module):
                                               aten["stride_c" if critic else "stride_g"])
 
         nvtx = os.environ.get("MMG_NVTX", "0") == "1"            # host-side NVTX ranges per decode step / stage (visible in nsys / ncu --nvtx)
-        iterations = req.region.iterations if edit else 1
-        # edit(): `iterations` rounds of the token loop, step = the global step index (iteration * timesteps + s); one round otherwise
+        iterations = req.region.iterations if req.region is not None and req.region.iterations is not None else 1
+        # edit() / extrapolate(): `iterations` rounds of the token loop (edit's iterations, extrapolate's windows), step = the global step
+        # index (round * timesteps + s); one round otherwise
         for step, (num_masked, steps_until_x0) in enumerate(zip(sched * iterations, list(reversed(range(timesteps))) * iterations)):
             s = step % timesteps
             if edit and s == 0:
                 ops.edit_select(ids, scores, frozen, region["keep"], region["num_select"], self.mask_id, step // timesteps,
                                 u=self._injected_noise(step, (b, n), device), seed_dev=self._seed_dev, row_offset=self.row_offset * n)
+            if window is not None and s == 0:
+                ops.extrapolate_window(canvas, ids, scores, window.corners[step // timesteps], window.direction, window.stride, self.mask_id)
             if nvtx:
                 if step:
                     torch.cuda.nvtx.range_pop()
@@ -1105,7 +1226,10 @@ class MaskGit(nn.Module):
                                  float(lead(req.critic_noise_scale) * (steps_until_x0 / timesteps)), scores, u=self._injected_noise(step, (b, n), device),
                                  seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, aten=aten_draw(step, critic=True),
                                  cond_scale_dev=settings["crit_cond_scale"], noise_mul_dev=settings["crit_noise"][s])
-        ids = ids.view(b, req.fmap_size, req.fmap_size)
+            if window is not None and s == timesteps - 1:
+                ops.extrapolate_window(canvas, ids, scores, window.corners[step // timesteps], window.direction, window.stride, self.mask_id,
+                                       store=True)
+        ids = canvas if window is not None else ids.view(b, req.fmap_size, req.fmap_size)
         if nvtx:
             torch.cuda.nvtx.range_pop()
             torch.cuda.nvtx.range_push("mmg.vae_decode")

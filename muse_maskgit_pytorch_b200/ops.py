@@ -1,5 +1,6 @@
 """Thin tensor-level wrappers over the C-ABI (one Python function per mmg_* entry point).  PyTorch supplies device
 memory and the stream; every number is computed by libmmg.so."""
+import math
 import os
 
 import torch
@@ -358,6 +359,24 @@ def edit_select(ids, scores, frozen_out, keep, num_select, mask_id, iteration, u
     a.num_select = num_select.data_ptr(); a.u = L.ptr(u); a.seed = seed; a.seed_dev = L.ptr(seed_dev); a.row_offset = row_offset
     a.B, a.n = ids.shape; a.iteration = iteration; a.mask_id = mask_id
     L.call("mmg_edit_select", a)
+
+
+EXTRAPOLATE_DIRECTIONS = ("right", "left", "down", "up")       # the direction codes of mmg_extrapolate_window
+
+
+def extrapolate_window(canvas, ids, scores, corner, direction, stride, mask_id, store=False):
+    """Moves one f x f window of an extrapolation between the token canvas (int64 [B, H, W]) and the decode buffers ids (int64 [B, f*f]) /
+    scores (fp32 [B, f*f]); corner = the window's top-left (row, col) in the canvas, the strip = its `stride` columns (rows) at the far side of
+    `direction`.  Load (store=False): ids = the canvas block with mask_id on the strip, scores = 0.  Store: the strip of ids into the canvas."""
+    _chk(canvas, "canvas"); _chk(ids, "ids"); _chk(scores, "scores")
+    B, H, W = canvas.shape
+    f = math.isqrt(ids.shape[1])
+    assert canvas.dtype == ids.dtype == torch.int64 and scores.dtype == torch.float32 and ids.shape == scores.shape == (B, f * f)
+    a = L.ExtrapolateWindowArgs()
+    a.canvas = canvas.data_ptr(); a.ids = ids.data_ptr(); a.scores = scores.data_ptr()
+    a.B = B; a.f = f; a.canvas_h = H; a.canvas_w = W; a.row0, a.col0 = corner
+    a.direction = EXTRAPOLATE_DIRECTIONS.index(direction); a.stride = stride; a.store = int(store); a.mask_id = mask_id
+    L.call("mmg_extrapolate_window", a)
 
 
 def _per_row_table(t, rows, name):

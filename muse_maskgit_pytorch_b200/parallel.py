@@ -1,5 +1,5 @@
 """Batch-sharded generation and editing over the GPUs of one node (SURVEY.md 8e): every sequence is independent through the whole
-of generate(), inpaint(), edit() and the Muse cascade, so rank r runs a contiguous slice of the batch with replicated weights and the
+of generate(), inpaint(), edit(), extrapolate() and the Muse cascade, so rank r runs a contiguous slice of the batch with replicated weights and the
 results are assembled with all-gathers at the end.  No collective runs inside the decode loop.  The sampler's Philox counters are
 keyed on the global sequence index (MaskGit.row_offset), so token ids do not depend on the number of ranks."""
 import numbers
@@ -49,15 +49,21 @@ def _gather(local, total, group):
     return gather_batch(local, total, group)
 
 
-def _empty_result(maskgit, return_ids=False, fmap_size=None):
-    """What a rank without rows contributes: (0, C, S, S) fp32 images and, with return_ids, (0, f, f) int64 ids, on the model's device."""
+def _empty_result(maskgit, return_ids=False, fmap_size=None, image_hw=None):
+    """What a rank without rows contributes: (0, C, S, S) fp32 images and, with return_ids, (0, f, f) int64 ids, on the model's device.
+    image_hw: the (H, W) of a call whose images are not S x S (extrapolate); its ids are then (0, H / p, W / p)."""
     device = next(maskgit.parameters()).device
     size = maskgit.image_size
-    images = torch.empty((0, maskgit.vae.channels, size, size), dtype=torch.float32, device=device)
+    H, W = image_hw if image_hw is not None else (size, size)
+    images = torch.empty((0, maskgit.vae.channels, H, W), dtype=torch.float32, device=device)
     if not return_ids:
         return images
-    f = fmap_size if fmap_size is not None else maskgit.vae.get_encoded_fmap_size(size)
-    return images, torch.empty((0, f, f), dtype=torch.int64, device=device)
+    if image_hw is not None:
+        shape = (H // maskgit.vae.dim_divisor, W // maskgit.vae.dim_divisor)
+    else:
+        f = fmap_size if fmap_size is not None else maskgit.vae.get_encoded_fmap_size(size)
+        shape = (f, f)
+    return images, torch.empty((0,) + shape, dtype=torch.int64, device=device)
 
 
 def _run_shard(method, maskgits, texts, lo, hi, total, empty, *, group=None, seeds=None, text_embeds=None, text_embeds_shard=None,
@@ -110,13 +116,13 @@ def _run_shard(method, maskgits, texts, lo, hi, total, empty, *, group=None, see
             m.transformer.encode_text, m.row_offset, m.global_batch, m.sampler_seed = encode_text, row_offset, global_batch, sampler_seed
 
 
-def _sharded_call(maskgit, method, texts, group, seed, kwargs):
-    """A MaskGit call over this rank's rows, then the all-gather of its result."""
+def _sharded_call(maskgit, method, texts, group, seed, kwargs, image_hw=None):
+    """A MaskGit call over this rank's rows, then the all-gather of its result (image_hw: as _empty_result's)."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     total = len(texts)
     lo, hi = shard_bounds(total, rank, world)
-    empty = lambda: _empty_result(maskgit, kwargs.get("return_ids", False), kwargs.get("fmap_size"))
+    empty = lambda: _empty_result(maskgit, kwargs.get("return_ids", False), kwargs.get("fmap_size"), image_hw)
     local = _run_shard(method, (maskgit,), texts, lo, hi, total, empty, group=group, seeds=None if seed is None else (seed,), **kwargs)
     return _gather(local, total, group)
 
@@ -161,6 +167,22 @@ def edit_sharded(maskgit, texts, images, mask=None, text_embeds=None, cond_image
     return _sharded_call(maskgit, maskgit.edit, texts, group, seed,
                          dict(edit_kwargs, images=images, mask=mask, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard,
                               cond_images=cond_images, cond_images_shard=cond_images_shard))
+
+
+def extrapolate_sharded(maskgit, texts, images, direction="right", amount=256, text_embeds=None, group=None, *, text_embeds_shard=None,
+                        seed=None, **extrapolate_kwargs):
+    """maskgit.extrapolate over this rank's rows, then the all-gather of the grown images (and canvases with return_ids=True).  `images`
+    is indexed by global row and sliced here, as are text_embeds and per-image settings; a rank without rows contributes the grown
+    (0, C, H', W') / (0, H'/p, W'/p) shapes.  The arguments are checked on the whole batch before any collective, so every rank raises the
+    same ValueError.  The sampler noise is keyed on the global row and the window-local position, so with one seed for every rank ("mmg"
+    mode) the token ids do not depend on the number of ranks; sampler_rng = "aten" raises ValueError, as extrapolate() does, and
+    `sampler_noise_fn` is not covered."""
+    window = maskgit._extrapolate_plan(images, len(texts), direction, amount, extrapolate_kwargs.get("stride"))
+    p = maskgit.vae.dim_divisor
+    return _sharded_call(maskgit, maskgit.extrapolate, texts, group, seed,
+                         dict(extrapolate_kwargs, images=images, direction=direction, amount=amount, text_embeds=text_embeds,
+                              text_embeds_shard=text_embeds_shard),
+                         image_hw=(window.canvas[0] * p, window.canvas[1] * p))
 
 
 def muse_sharded(muse, texts, text_embeds=None, group=None, *, text_embeds_shard=None, **forward_kwargs):
