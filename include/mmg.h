@@ -331,7 +331,8 @@ int mmg_remask_frozen(const mmg_remask_frozen_args* a, void* stream);
 
 /* selection of one mask-free editing iteration (MaskGit.edit).  Row b takes one uniform key per position: u[b, p] when u != NULL,
  * else Philox4x32-10(counter = (0xFFFFFFFE, iteration, row_offset + b*n + p), key = seed + *seed_dev) >> 8 * 2^-24 (disjoint from
- * the gumbel stream, c0 = vocabulary index, and the critic stream, c0 = 0xFFFFFFFF).  Among its editable positions (keep == 0)
+ * the gumbel stream, c0 = vocabulary index, and the critic stream, c0 = 0xFFFFFFFF); with image_seed != NULL the key is image_seed[b]
+ * and the row counter the image-local position p, so row b's keys do not depend on the batch around it.  Among its editable positions (keep == 0)
  * it selects the num_select[b] largest keys (ties: lowest position first), writes frozen_out[b, p] = 1 at every other position
  * and 0 at the selected ones, mask_id at the selected ids and 0 into every score of the row.  A following mmg_remask_frozen
  * with frozen = frozen_out and count num_select[b] re-masks exactly the selected positions.  num_select is read on the device. */
@@ -343,6 +344,7 @@ typedef struct {
   uint64_t seed; const uint64_t* seed_dev;            /* seed_dev optional, as in mmg_logits_sample_args          */
   int64_t row_offset;                                 /* global position of this call's first token                */
   int32_t B, n, iteration, _pad; int64_t mask_id;
+  const uint64_t* image_seed;                         /* [B] per-image Philox keys or NULL (u == NULL only)        */
 } mmg_edit_select_args;
 int mmg_edit_select(const mmg_edit_select_args* a, void* stream);
 
@@ -379,7 +381,8 @@ int mmg_final_embed(const mmg_final_embed_args* a, void* stream);
  *   pred = argmax_v( logit_v / max(T, 1e-10) - log(-log(u_v)) ),   u clamped at 1e-20 as the reference's log();
  *   score = 1 - softmax(logits)[pred];  ids[b, pos] = pred;  scores[b, pos] = score.
  * Noise: `u` != NULL -> injected uniforms, u[(b*n + pos) * V + v] (parity mode: the tensor the reference would
- * draw); else Philox4x32-10(seed, counter = (global row, v)) so results do not depend on the GPU count.          */
+ * draw); else Philox4x32-10(seed, counter = (global row, v)) so results do not depend on the GPU count; with
+ * image_seed != NULL, Philox4x32-10(image_seed[b], counter = (pos, v)) so they do not depend on the batch either.  */
 typedef struct {
   const float* logits;     /* [R, V] fp32, R = B*num_masked, row j of batch b at b*num_masked + j                  */
   const int32_t* masked_pos;
@@ -404,6 +407,9 @@ typedef struct {
   const int32_t* row_index; const int32_t* row_count_dev; int32_t row_index_cap, _pad2;
   const float* temperature_dev;  /* [B] per-image temperatures or NULL (use `temperature`): sampled row j of image b = j / num_masked
                                     divides by max(temperature_dev[b], 1e-10)                                                       */
+  const uint64_t* image_seed;    /* [B] per-image Philox keys or NULL (rng_mode 0, u == NULL only): image b (found as for temperature_dev)
+                                    draws with counter (v, step, pos, 0) and key image_seed[b] in place of (v, step, global row) and
+                                    seed + *seed_dev; seed, seed_dev and row_offset are then not read                              */
 } mmg_logits_sample_args;
 int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream);
 
@@ -460,7 +466,9 @@ int mmg_logits_xent_rows(const mmg_logits_xent_rows_args* a, void* stream);
  *   s[r] = dot(LayerNorm(x_cond[r]) * gamma, w) + bias;   x_null != NULL: s = s_null + (s - s_null) * cond_scale  (CFG, :257)
  *   scores[r] = s + (u[r] - 0.5) * noise_mul       noise_mul = critic_noise_scale * steps_until_x0 / timesteps
  * x_* are the residual streams after the critic's last block (the final LayerNorm and the 1-wide head are applied here).
- * u == NULL: u = Philox4x32-10(counter = (0xFFFFFFFF, step, row_offset + r), key = seed + *seed_dev) >> 8 * 2^-24.
+ * u == NULL: u = Philox4x32-10(counter = (0xFFFFFFFF, step, row_offset + r), key = seed + *seed_dev) >> 8 * 2^-24; with row_key != NULL
+ * (rng_mode 0), counter = (0xFFFFFFFF, step, row_key[r][1]) and key = row_key[r][0] (a host gives each row its image's seed and its
+ * image-local position, as it expands per-image settings over the rows).
  * cond_scale_dev / noise_mul_dev != NULL: row r reads its scale / noise multiplier from them instead of the scalars (a host expands
  * per-image settings over the image's rows); a row whose scale is exactly 1 keeps s from x_cond alone, as the x_null == NULL launch. */
 typedef struct {
@@ -473,6 +481,7 @@ typedef struct {
   int32_t rng_mode;                           /* 1: ATen's `uniform(scores.shape)` stream (:598), see mmg_logits_sample_args */
   uint64_t aten_offset; const uint64_t* aten_offset_dev; uint32_t aten_stride, _pad;
   const float* cond_scale_dev; const float* noise_mul_dev;   /* [rows] per-row values or NULL (use cond_scale / noise_mul)      */
+  const uint64_t* row_key;                    /* [rows, 2] per-row (Philox key, row counter) or NULL                  */
 } mmg_critic_score_args;
 int mmg_critic_score(const mmg_critic_score_args* a, void* stream);
 
@@ -552,6 +561,7 @@ typedef struct {
                                                      the caller (the padding rows of the self-attention K/V stay zero)        */
   const float* cond_scale_dev; const float* temperature_dev;   /* [b] per-image settings or NULL (use cond_scale / temperature): passed
                                                      to mmg_final_embed_args.cond_scale_dev / mmg_logits_sample_args.temperature_dev */
+  const uint64_t* image_seed;                     /* [b] per-image Philox keys or NULL: passed to mmg_logits_sample_args.image_seed */
 } mmg_decode_step_args;
 uint64_t mmg_decode_step_workspace_bytes(int32_t b, int32_t branches, int32_t n, int32_t dim, int32_t heads, int32_t Fp, int32_t V, int32_t max_masked);
 int mmg_decode_step(const mmg_decode_step_args* a, void* stream);

@@ -101,7 +101,8 @@ class RemaskFrozenArgs(C.Structure):
 
 class EditSelectArgs(C.Structure):
     _fields_ = [("ids", vp), ("scores", vp), ("frozen_out", vp), ("keep", vp), ("num_select", vp), ("u", vp), ("seed", u64), ("seed_dev", vp),
-                ("row_offset", i64), ("B", i32), ("n", i32), ("iteration", i32), ("_pad", i32), ("mask_id", i64)]
+                ("row_offset", i64), ("B", i32), ("n", i32), ("iteration", i32), ("_pad", i32), ("mask_id", i64),
+                ("image_seed", vp)]
 
 
 class ExtrapolateWindowArgs(C.Structure):
@@ -119,7 +120,7 @@ class LogitsSampleArgs(C.Structure):
                 ("B", i32), ("n", i32), ("num_masked", i32), ("V", i32), ("k", i32), ("temperature", f32),
                 ("seed", u64), ("step", u64), ("row_offset", i64), ("seed_dev", vp), ("mask_id", i64), ("only_masked", i32), ("rng_mode", i32),
                 ("aten_offset", u64), ("aten_offset_dev", vp), ("aten_stride", C.c_uint32), ("_pad", i32),
-                ("row_index", vp), ("row_count_dev", vp), ("row_index_cap", i32), ("_pad2", i32), ("temperature_dev", vp)]
+                ("row_index", vp), ("row_count_dev", vp), ("row_index_cap", i32), ("_pad2", i32), ("temperature_dev", vp), ("image_seed", vp)]
 
 
 class LogitsFusedArgs(C.Structure):
@@ -140,7 +141,7 @@ class CriticScoreArgs(C.Structure):
     _fields_ = [("x_cond", vp), ("x_null", vp), ("gamma", vp), ("w", vp), ("bias", f32), ("cond_scale", f32), ("noise_mul", f32),
                 ("dim", i32), ("u", vp), ("scores", vp), ("rows", i64), ("row_offset", i64), ("seed", u64), ("seed_dev", vp),
                 ("step", i32), ("rng_mode", i32), ("aten_offset", u64), ("aten_offset_dev", vp), ("aten_stride", C.c_uint32), ("_pad", i32),
-                ("cond_scale_dev", vp), ("noise_mul_dev", vp)]
+                ("cond_scale_dev", vp), ("noise_mul_dev", vp), ("row_key", vp)]
 
 
 class FfGegluArgs(C.Structure):
@@ -164,7 +165,7 @@ class DecodeStepArgs(C.Structure):
                 ("ctx_key_mask", vp), ("ctx_keys", i32), ("ctx_alloc", i32), ("ids", vp), ("scores", vp), ("masked_pos", vp), ("mask_id", i64),
                 ("num_masked", i32), ("k_keep", i32), ("step", i32), ("temperature", f32), ("cond_scale", f32), ("_pad", i32),
                 ("u", vp), ("seed", u64), ("seed_dev", vp), ("row_offset", i64), ("workspace", vp), ("workspace_bytes", u64),
-                ("cond_scale_dev", vp), ("temperature_dev", vp)]
+                ("cond_scale_dev", vp), ("temperature_dev", vp), ("image_seed", vp)]
 
 
 class LfqEncodeArgs(C.Structure):

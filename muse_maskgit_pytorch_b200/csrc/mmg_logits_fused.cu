@@ -467,8 +467,8 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
   bool fallback = s_bad || n < k;
   if (!fallback) {
     const uint2* row_lists = f.lists + r * (int64_t)nseg * f.cap;
-    const int64_t grow = a.row_offset + (int64_t)b * a.n + pos;
-    const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+    uint64_t seed; int64_t grow;
+    row_noise_key<MODE>(a, b, pos, seed, grow);
     tdiv = image_tdiv(a, b, tdiv);
     const float inv_t = 1.0f / tdiv;
     uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
@@ -740,6 +740,7 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
   MMG_CHECK_ARG(lf_supported(s.V, a->K, s.k), "mmg_logits_fused: unsupported V=%d K=%d k=%d (use mmg_linear + mmg_logits_sample)", s.V, a->K, s.k);
   MMG_CHECK_ARG(s.rng_mode == 0 || (s.rng_mode == 1 && s.aten_stride >= 256 && s.aten_stride % 256 == 0 && s.aten_offset % 4 == 0 && !s.u),
                 "mmg_logits_fused: rng_mode=%d aten_stride=%u", s.rng_mode, s.aten_stride);
+  MMG_CHECK_ARG(!s.image_seed || (s.rng_mode == 0 && !s.u), "mmg_logits_fused: image_seed needs rng_mode 0 and u == NULL");
   const int64_t R = (int64_t)s.B * s.num_masked;
   if (R == 0) return MMG_OK;
   const int64_t R_cap = a->rows_capacity > 0 ? a->rows_capacity : R;

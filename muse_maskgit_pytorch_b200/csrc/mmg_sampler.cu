@@ -301,8 +301,8 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   __syncthreads();
   const int cut = s_cut;
   // 2. statistics + perturbed argmax over the kept set
-  const int64_t grow = a.row_offset + (int64_t)b * a.n + pos;
-  const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  uint64_t seed; int64_t grow;
+  row_noise_key<MODE>(a, b, pos, seed, grow);
   const float inv_t = 1.0f / s_tdiv;
   uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
   if (MODE == 2) {
@@ -465,12 +465,14 @@ edit_select_kernel(const mmg_edit_select_args a) {
   int* flag = reinterpret_cast<int*>(sc + n);
   uint8_t* fz = reinterpret_cast<uint8_t*>(sc + 2 * n);
   const int64_t base = (int64_t)b * n;
-  const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  // per-image seeds: image b's own key and the image-local position as the row counter
+  const uint64_t seed = a.image_seed ? a.image_seed[b] : a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  const int64_t row0 = a.image_seed ? 0 : a.row_offset + base;
   for (int i = tid; i < n; i += 256) {
     float u;
     if (a.u) u = a.u[base + i];
     else {
-      const int64_t grow = a.row_offset + base + i;
+      const int64_t grow = row0 + i;
       u = (float)(philox_first(0xFFFFFFFEu, (uint32_t)a.iteration, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed,
                                (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
     }
@@ -544,8 +546,9 @@ critic_score_kernel(mmg_critic_score_args a) {
     float u;
     if (a.u) u = a.u[row];
     else {
-      const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
-      const int64_t grow = a.row_offset + row;
+      // per-row keys: the row's image seed and image-local position
+      const uint64_t seed = a.row_key ? a.row_key[2 * row] : a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+      const int64_t grow = a.row_key ? (int64_t)a.row_key[2 * row + 1] : a.row_offset + row;
       if (a.rng_mode == 1) {      // ATen stream of `uniform(scores.shape)`: flat index = global position
         const uint64_t k = (uint64_t)grow / a.aten_stride;
         u = aten_uniform((uint32_t)((uint64_t)grow - k * a.aten_stride), k, (a.aten_offset + (a.aten_offset_dev ? *a.aten_offset_dev : 0ull)) >> 2, seed);
@@ -571,6 +574,7 @@ extern "C" int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream) 
   static const size_t smem = (size_t)SMP_CAP * 8 + (size_t)SMP_THREADS * 64;
   MMG_CHECK_ARG(a->rng_mode == 0 || (a->rng_mode == 1 && a->aten_stride >= 256 && a->aten_stride % 256 == 0 && a->aten_offset % 4 == 0 && !a->u),
                 "mmg_logits_sample: rng_mode=%d aten_stride=%u", a->rng_mode, a->aten_stride);
+  MMG_CHECK_ARG(!a->image_seed || (a->rng_mode == 0 && !a->u), "mmg_logits_sample: image_seed needs rng_mode 0 and u == NULL");
   static cudaError_t attr0 = cudaFuncSetAttribute(logits_sample_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   static cudaError_t attr1 = cudaFuncSetAttribute(logits_sample_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   static cudaError_t attr2 = cudaFuncSetAttribute(logits_sample_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -618,6 +622,7 @@ extern "C" int mmg_edit_select(const mmg_edit_select_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MMG_CHECK_ARG(a && a->ids && a->scores && a->frozen_out && a->keep && a->num_select, "mmg_edit_select: NULL pointer");
   MMG_CHECK_ARG(a->B >= 0 && a->n > 0 && a->n <= 16384 && a->iteration >= 0, "mmg_edit_select: B=%d n=%d iteration=%d", a->B, a->n, a->iteration);
+  MMG_CHECK_ARG(!a->image_seed || !a->u, "mmg_edit_select: image_seed needs u == NULL");
   if (a->B == 0) return MMG_OK;
   const size_t smem = (size_t)a->n * 9;                 // keys, flags, keep bytes
   static const cudaError_t attr = cudaFuncSetAttribute(edit_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 9);
@@ -648,6 +653,7 @@ extern "C" int mmg_critic_score(const mmg_critic_score_args* a, void* stream) {
   MMG_CHECK_ARG(a && a->x_cond && a->gamma && a->w && a->scores, "mmg_critic_score: NULL pointer");
   MMG_CHECK_ARG(a->dim > 0 && a->rows >= 0, "mmg_critic_score: dim=%d", a->dim);
   MMG_CHECK_ARG(a->rng_mode == 0 || (a->rng_mode == 1 && a->aten_stride >= 256 && a->aten_offset % 4 == 0), "mmg_critic_score: rng_mode=%d aten_stride=%u", a->rng_mode, a->aten_stride);
+  MMG_CHECK_ARG(!a->row_key || (a->rng_mode == 0 && !a->u), "mmg_critic_score: row_key needs rng_mode 0 and u == NULL");
   if (a->rows == 0) return MMG_OK;
   MMG_CUDA(launch_pdl(critic_score_kernel, dim3((unsigned)((a->rows + 7) / 8)), dim3(256), 0, st, *a));
   MMG_LAUNCHED();

@@ -172,6 +172,15 @@ __device__ __forceinline__ float image_tdiv(const mmg_logits_sample_args& a, int
   return t < 1e-10f ? 1e-10f : t;
 }
 
+// Philox key and row counter of sampled row (b, pos): with per-image seeds (MODE 0 only) image b's own seed and the image-local position,
+// so its noise does not depend on the batch around it; otherwise seed + *seed_dev and the global row.
+template <int MODE>
+__device__ __forceinline__ void row_noise_key(const mmg_logits_sample_args& a, int b, int pos, uint64_t& seed, int64_t& grow) {
+  if (MODE == 0 && a.image_seed) { seed = a.image_seed[b]; grow = pos; return; }
+  seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  grow = a.row_offset + (int64_t)b * a.n + pos;
+}
+
 // ---------------- phase C: perturbed argmax restricted to the exact top-k ----------------
 // lval / lidx: the n candidates of the row (every element >= some threshold, n >= k or the complete exact top-k); (b, pos): the row.
 // MODE 1 = injected-noise parity mode, MODE 2 = ATen-compatible in-kernel Philox (the stream a seeded torch.cuda run of the reference
@@ -183,8 +192,8 @@ __device__ __forceinline__ float image_tdiv(const mmg_logits_sample_args& a, int
 template <int MODE>
 __device__ __forceinline__ void sample_from_list(const mmg_logits_sample_args& a, float tdiv, const float* lval, const int* lidx, int n, int k, int V,
                                                  int b, int pos, SampleScratch& sc, int tid, int warp, int lane, int& win_v, float& win_x) {
-  const int64_t grow = a.row_offset + (int64_t)b * a.n + pos;
-  const uint64_t seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  uint64_t seed; int64_t grow;
+  row_noise_key<MODE>(a, b, pos, seed, grow);
   const float inv_t = 1.0f / tdiv;
   uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
   if (MODE == 2) {            // flat index of logit (grow, v) in the reference's [B, n, V] noise tensor = grow * V + v = ar0 + v + S * aq0

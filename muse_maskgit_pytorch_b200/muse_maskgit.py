@@ -588,6 +588,57 @@ def _per_image(name, value, b):
     return vals
 
 
+_U64 = 1 << 64
+
+
+def splitmix64(x):
+    """SplitMix64's output for the state x in [0, 2^64) (Steele, Lea and Flood, "Fast splittable pseudorandom number generators", 2014):
+    z = x + 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9; z = (z ^ (z >> 27)) * 0x94D049BB133111EB; z ^ (z >> 31), all
+    mod 2^64.  Muse.forward derives the super-resolution stage's per-image seeds from the base stage's with it."""
+    z = (int(x) + 0x9E3779B97F4A7C15) % _U64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) % _U64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) % _U64
+    return z ^ (z >> 31)
+
+
+def _image_seeds(value, b):
+    """Per-image sampling seeds as a tuple of b Python ints in [0, 2^64), or None for None: `value` is one int s (the seeds s, s + 1, ...,
+    s + b - 1 mod 2^64), a length-b sequence of ints, or a 1-D integer tensor on any device (an int64 tensor holds the two's-complement
+    bits of uint64 seeds).  Raises ValueError on a wrong length, a value outside [0, 2^64) or a non-integer dtype."""
+    if value is None:
+        return None
+    if isinstance(value, torch.Tensor):
+        if value.dtype.is_floating_point or value.dtype.is_complex or value.dtype == torch.bool:
+            raise ValueError(f"image_seeds must hold integers, got a tensor of dtype {value.dtype}")
+        if value.dim() != 1:
+            raise ValueError(f"image_seeds must be 1-D, got a tensor of shape {tuple(value.shape)}")
+        vals = value.detach().cpu().tolist()
+        if value.dtype == torch.int64:
+            vals = [v % _U64 for v in vals]
+    elif isinstance(value, numbers.Integral) and not isinstance(value, bool):
+        if not 0 <= int(value) < _U64:
+            raise ValueError(f"image_seeds must lie in [0, 2^64), got {value}")
+        return tuple((int(value) + i) % _U64 for i in range(b))
+    else:
+        try:
+            vals = list(value)
+        except TypeError:
+            raise ValueError(f"image_seeds must be an int, a sequence of ints or a 1-D integer tensor, got {value!r}") from None
+        if not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in vals):
+            raise ValueError(f"image_seeds must hold ints, got {vals!r}")
+        vals = [int(v) for v in vals]
+    if len(vals) != b:
+        raise ValueError(f"image_seeds has {len(vals)} values for {b} texts")
+    if not all(0 <= v < _U64 for v in vals):
+        raise ValueError(f"image_seeds must lie in [0, 2^64), got {vals}")
+    return tuple(vals)
+
+
+def _seed_bits(seeds):
+    """uint64 seeds as the int64 tensor of their two's-complement bits (the device layout of libmmg's image_seed tables)."""
+    return torch.tensor([v - _U64 if v >= 1 << 63 else v for v in seeds], dtype=torch.int64)
+
+
 def _fill_on_device(t, device):
     """Host tensor `t` rebuilt on `device` with one fill kernel per run of equal values.  Used when a caller captures the whole call into
     their own CUDA graph, where a host-to-device copy cannot be recorded; the values are then fixed in that graph, as scalar arguments are."""
@@ -604,7 +655,7 @@ def _fill_on_device(t, device):
 @dataclasses.dataclass(frozen=True)
 class _DecodeRequest:
     """One validated generate() / inpaint() / edit() / extrapolate() call.  temperature, cond_scale, critic_noise_scale: one float per image.
-    seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs)."""
+    seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs).  image_seeds: one uint64 seed per image, or None."""
     texts: List[str]
     cond_images: Optional[torch.Tensor]
     fmap_size: int
@@ -618,6 +669,7 @@ class _DecodeRequest:
     return_ids: bool
     region: Optional[_Region] = None
     seed: Optional[int] = None
+    image_seeds: Optional[tuple] = None
 
     @property
     def branches(self):
@@ -627,13 +679,16 @@ class _DecodeRequest:
     def settings(self, n):
         """The host fp32 tables the sampling kernels read, each value the float64 expression of a scalar call rounded once: temps and
         crit_noise [timesteps, b] (step s anneals by steps_until_x0 / timesteps, muse_maskgit_pytorch.py:578, 600), cond_scale [b]; with a
-        critic, its per-row copies over the n positions of each image (crit_cond_scale [b*n], crit_noise [timesteps, b*n])."""
+        critic, its per-row copies over the n positions of each image (crit_cond_scale [b*n], crit_noise [timesteps, b*n]); with per-image
+        seeds, image_seeds int64 [b] (the bits of the uint64 seeds)."""
         anneal = [until / self.timesteps for until in reversed(range(self.timesteps))]
         f32 = lambda v: torch.tensor(v, dtype=torch.float32)
         out = dict(temps=f32([[t * a for t in self.temperature] for a in anneal]), cond_scale=f32(self.cond_scale))
         if self.use_critic:
             out["crit_cond_scale"] = out["cond_scale"].repeat_interleave(n)
             out["crit_noise"] = f32([[c * a for c in self.critic_noise_scale] for a in anneal]).repeat_interleave(n, dim=1)
+        if self.image_seeds is not None:
+            out["image_seeds"] = _seed_bits(self.image_seeds)
         return out
 
 
@@ -712,13 +767,25 @@ class MaskGit(nn.Module):
     @torch.no_grad()
     def generate(self, texts: List[str], negative_texts: Optional[List[str]] = None, cond_images: Optional[torch.Tensor] = None,
                  fmap_size=None, temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False,
-                 force_not_use_token_critic=False, timesteps=18, cond_scale=3, critic_noise_scale=1, return_ids=False):
+                 force_not_use_token_critic=False, timesteps=18, cond_scale=3, critic_noise_scale=1, return_ids=False, image_seeds=None):
         """ref: muse_maskgit_pytorch.py:491-621.  Returns fp32 NCHW images (b, 3, H, W), unclamped.
 
         temperature, cond_scale and critic_noise_scale are each a number (every image) or per image, a length-b sequence of numbers or a
         1-D tensor on any device: image i is decoded as if the whole call had been made with its own values (values must be finite,
         temperature >= 0).  The settings reach the kernels as device data, so one captured CUDA graph replays for any of them; only
-        whether every image has cond_scale == 1 (no null-CFG forward) selects a different graph.  inpaint() and edit() take them alike."""
+        whether every image has cond_scale == 1 (no null-CFG forward) selects a different graph.  inpaint() and edit() take them alike.
+
+        image_seeds: None (the default: every noise draw is keyed on the call's seed and the image's row in the global batch, so an image
+        depends on its slot), or one seed per image in [0, 2^64): a length-b sequence of ints, a 1-D integer tensor on any device (int64 is
+        read as the bits of a uint64), or one int s for the seeds s, s + 1, ..., s + b - 1 (mod 2^64).  Image b then draws every libmmg noise
+        value (gumbel, token critic, edit keys) from Philox keyed on image_seeds[b] with its own token positions as the row counters, so its
+        ids and pixels depend only on its text, region or mask, per-image settings, seed and the call's shape arguments (timesteps,
+        topk_filter_thres, iterations / fraction, direction / amount / stride), not on the batch around it, row_offset or the GPU count
+        (DESIGN.md "Per-image seeds" reports the fused tail's split count and the text padding as checked).  No call seed is drawn, so torch's
+        host generator is deliberately left untouched; the seeds are device data, and one captured graph replays for any of them.  Raises
+        ValueError with sampler_rng = "aten" (one reference stream per batch) or sampler_noise_fn.  inpaint(), edit() and extrapolate()
+        take it alike."""
+        seeds = self._image_seeds_arg(image_seeds, len(texts))
         if self.use_native_step and self.transformer.precision == "fp8":
             raise ValueError('use_native_step=True runs mmg_decode_step, whose weights carry no fp8 scales: it cannot run precision="fp8"; '
                              "set use_native_step = False")
@@ -729,12 +796,13 @@ class MaskGit(nn.Module):
             raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
         return self._decode(self._request(texts, cond_images=cond_images, fmap_size=fmap_size, temperature=temperature, timesteps=timesteps,
                                           topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
-                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
+                                          image_seeds=seeds))
 
     @torch.no_grad()
     def inpaint(self, texts: List[str], images: torch.Tensor, mask: torch.Tensor, cond_images: Optional[torch.Tensor] = None, temperature=1.,
                 topk_filter_thres=0.9, can_remask_prev_masked=False, force_not_use_token_critic=False, timesteps=18, cond_scale=3,
-                critic_noise_scale=1, return_ids=False):
+                critic_noise_scale=1, return_ids=False, image_seeds=None):
         """Regenerates the masked region of `images` and keeps the rest (an extension: the reference has no inpainting).
 
         images: fp32 NCHW (b, C, image_size, image_size), as `vae.encode` takes them.  mask: bool or {0, 1}, True = regenerate, either
@@ -746,8 +814,10 @@ class MaskGit(nn.Module):
         number of regenerated tokens, 0 when it has none).  Every other token id equals the encoded one bit for bit.  The pixels are
         vae.decode_from_ids(ids): the unmasked region is the VAE reconstruction, not the input pixels; pasting the input back is the
         caller's job.  With every token masked the result equals generate() under the same seed or injected noise.
-        Returns what generate() returns.  `use_native_step` does not apply here (mmg_decode_step has no frozen positions)."""
+        Returns what generate() returns.  `use_native_step` does not apply here (mmg_decode_step has no frozen positions).
+        image_seeds: per-image seeds, as for generate()."""
         b = len(texts)
+        seeds = self._image_seeds_arg(image_seeds, b)
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
         self._check_images(images, b)
         regen = regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1)
@@ -755,12 +825,13 @@ class MaskGit(nn.Module):
         region = self._region(images, counts, timesteps, frozen=(~regen).to(torch.uint8))
         return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=timesteps, region=region,
                                           topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
-                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
+                                          image_seeds=seeds))
 
     @torch.no_grad()
     def edit(self, texts: List[str], images: torch.Tensor, mask: Optional[torch.Tensor] = None, iterations=8, fraction=0.1, timesteps=4,
              cond_images: Optional[torch.Tensor] = None, temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False,
-             force_not_use_token_critic=False, cond_scale=3, critic_noise_scale=1, return_ids=False):
+             force_not_use_token_critic=False, cond_scale=3, critic_noise_scale=1, return_ids=False, image_seeds=None):
         """Mask-free editing (an extension, as inpaint() is; the Muse paper's third editing mode): moves `images` towards the prompts while
         keeping their layout, by repeatedly re-masking a random subset of their tokens and resampling it.
 
@@ -779,7 +850,8 @@ class MaskGit(nn.Module):
         Tokens outside the selections keep their ids bit for bit; the token grid stays on the device for the whole call (one encode, one
         decode).  iterations = 1, fraction = 1 is inpaint(mask) (generate() for mask=None) under the same seed; iterations = 0 returns
         ids0 and its decode.  The defaults (8 iterations of 4 steps on 10 % of the tokens) are this project's provisional choice, not
-        settings from the paper.  Returns what generate() returns.  `use_native_step` does not apply here, as for inpaint()."""
+        settings from the paper.  Returns what generate() returns.  `use_native_step` does not apply here, as for inpaint().
+        image_seeds: per-image seeds, as for generate(); image b's keys are then Philox with counter (0xFFFFFFFE, i, p) under image_seeds[b]."""
         if isinstance(iterations, bool) or not isinstance(iterations, int) or iterations < 0:
             raise ValueError(f"iterations must be an int >= 0, got {iterations!r}")
         if not 0 < fraction <= 1:
@@ -789,6 +861,7 @@ class MaskGit(nn.Module):
         if self.sampler_rng == "aten":
             raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
         b = len(texts)
+        seeds = self._image_seeds_arg(image_seeds, b)
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
         self._check_images(images, b)
         editable = (torch.ones((b, fmap_size ** 2), dtype=torch.bool) if mask is None
@@ -798,12 +871,13 @@ class MaskGit(nn.Module):
         region = self._region(images, select, timesteps, iterations, keep=(~editable).to(torch.uint8), num_select=torch.tensor(select, dtype=torch.int32))
         return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=timesteps, region=region,
                                           topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
-                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
+                                          image_seeds=seeds))
 
     @torch.no_grad()
     def extrapolate(self, texts: List[str], images: torch.Tensor, direction="right", amount=256, stride=None, timesteps=18, cond_scale=3,
                     temperature=1., topk_filter_thres=0.9, can_remask_prev_masked=False, force_not_use_token_critic=False, critic_noise_scale=1,
-                    return_ids=False):
+                    return_ids=False, image_seeds=None):
         """Grows `images` past their frame by `amount` pixels on one side (an extension, as inpaint() is; MaskGIT's image extrapolation),
         window by window, on a token canvas that stays on the device.
 
@@ -824,17 +898,30 @@ class MaskGit(nn.Module):
         return_ids the int64 canvas (b, H'/p, W'/p).  temperature, cond_scale and critic_noise_scale are per image or scalar, as for generate().
         Raises ValueError before any launch on a wrong direction, amount, stride, timesteps or image shape, for sampler_rng = "aten" (no
         reference stream), for a MaskGit conditioned on a low-resolution image, and for an fp8 VAE without conv tiles for the canvas.
-        `use_native_step` does not apply here, as for inpaint()."""
+        `use_native_step` does not apply here, as for inpaint().  image_seeds: per-image seeds, as for generate(); every window of image b
+        draws under image_seeds[b] with the window-local position p as the row counter."""
         if isinstance(timesteps, bool) or not isinstance(timesteps, int) or timesteps < 1:
             raise ValueError(f"timesteps must be an int >= 1, got {timesteps!r}")
         b = len(texts)
+        seeds = self._image_seeds_arg(image_seeds, b)
         window = self._extrapolate_plan(images, b, direction, amount, stride)
         f = self.vae.get_encoded_fmap_size(self.image_size)
         frozen = (~self._window_strip(direction, f, window.stride)).reshape(1, -1).to(torch.uint8).repeat(b, 1)
         region = self._region(images, [f * window.stride] * b, timesteps, len(window.corners), window, frozen=frozen)
         return self._decode(self._request(texts, temperature=temperature, timesteps=timesteps, region=region, cond_images=None,
                                           topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
-                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids))
+                                          force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
+                                          image_seeds=seeds))
+
+    def _image_seeds_arg(self, image_seeds, b):
+        """image_seeds of a call with b texts as a tuple of uint64 ints (None: not given); ValueError where no per-image stream exists."""
+        if image_seeds is None:
+            return None
+        if self.sampler_rng == "aten":
+            raise ValueError('image_seeds has no "aten" noise stream (ATen draws one stream per batch): use sampler_rng = "mmg"')
+        if self.sampler_noise_fn is not None:
+            raise ValueError("image_seeds cannot be combined with sampler_noise_fn, which supplies the noise itself")
+        return _image_seeds(image_seeds, b)
 
     def _check_images(self, images, b):
         if not isinstance(images, torch.Tensor) or tuple(images.shape) != (b, self.vae.channels, self.image_size, self.image_size):
@@ -979,7 +1066,8 @@ class MaskGit(nn.Module):
         aten, seed = None, req.seed
         if self.sampler_rng == "aten" and self.sampler_noise_fn is None:
             aten = self._aten_plan(device, b, req.fmap_size ** 2, tr.num_tokens, req.timesteps, req.use_critic)
-        elif self.sampler_noise_fn is None:      # (injected noise: the host generator is the caller's stream — nothing is drawn from it here)
+        elif self.sampler_noise_fn is None and req.image_seeds is None:
+            # (injected noise: the host generator is the caller's stream; per-image seeds: the kernels read no call seed — nothing is drawn)
             if seed is None:                     # (a rerun on the materialised path keeps the seed of the attempt it repeats)
                 seed = self.sampler_seed if self.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
             self._seed_dev.fill_(seed)
@@ -993,7 +1081,8 @@ class MaskGit(nn.Module):
         key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), req.fmap_size,
                float(req.topk_filter_thres), int(req.timesteps), req.branches, int(self.row_offset),
                tr.precision, self.vae.precision, req.use_critic, bool(req.can_remask_prev_masked),
-               None if aten is None else aten["key"], bool(self.use_native_step), id(self.noise_schedule), bool(self.use_fused_tail))
+               None if aten is None else aten["key"], bool(self.use_native_step), id(self.noise_schedule), bool(self.use_fused_tail),
+               req.image_seeds is not None)
         if req.region is not None and req.region.window is not None:
             key += (req.region.window.key,)
         elif req.region is not None:
@@ -1105,11 +1194,11 @@ class MaskGit(nn.Module):
         return bufs
 
     def _sample_tail(self, x, nb, pos, rows_b, ids, scores, temp, step, u, cond_scale, k_keep, tail, seed_dev=None, only_masked_id=None, aten=None,
-                     temp_dev=None, cond_scale_dev=None):
+                     temp_dev=None, cond_scale_dev=None, image_seed=None):
         """The sampling tail of one decode step (muse_maskgit_pytorch.py:576-609) on the rows listed in `pos` (b, rows_b): final LayerNorm +
         CFG combine in embedding space, to_logits, top-k filter, gumbel argmax, confidence score; ids / scores are updated in place.
         x: residual stream [nb*b*n, dim] after the blocks (cond rows first, then the null-CFG rows).  temp_dev / cond_scale_dev: fp32 [b]
-        per-image values the kernels read in place of the scalars `temp` / `cond_scale`."""
+        per-image values the kernels read in place of the scalars `temp` / `cond_scale`; image_seed: int64 [b] per-image Philox keys or None."""
         tr = self.transformer
         P = tr._packed()
         b, n = ids.shape
@@ -1118,7 +1207,7 @@ class MaskGit(nn.Module):
         e = tail["e"]
         ops.final_embed(x[:bn], x[bn:2 * bn] if nb == 2 else None, P["gf"], pos, e, b, n, rows_b, cond_scale, cond_scale_dev=cond_scale_dev)
         kw = dict(u=u, seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, only_masked_id=only_masked_id, aten=aten,
-                  temperature_dev=temp_dev)
+                  temperature_dev=temp_dev, image_seed=image_seed)
         if "fused_ws" in tail:      # logits never reach HBM: candidate lists out of the GEMM epilogue, sampled by the finishing kernel
             ops.logits_fused(e[:R], P["wlog"], pos, ids, scores, rows_b, k_keep, temp, tail["fused_ws"], tail["status"],
                              rows_capacity=b * tail["rows_max"], **kw)
@@ -1176,6 +1265,11 @@ class MaskGit(nn.Module):
         if req.use_critic:
             cnet, cnb, cctx, whead, bhead, gcrit = self._resolve_critic(text_embeds, cond_ids, [False, True][:nb], ctx)
         seed_dev = self._seed_dev if aten is None else self._aten_dev[0:1]
+        # per-image seeds: [b] keys for the sampler and edit keys; the critic, which has no image index, takes a per-row (key, position) table
+        seeds = settings.get("image_seeds")
+        crit_key = None
+        if seeds is not None and req.use_critic:
+            crit_key = torch.stack((seeds[:, None].expand(b, n), torch.arange(n, device=device).expand(b, n)), dim=-1)
 
         def aten_draw(step, critic=False):      # (Philox offset, device offset word, stride) of the step's gumbel or critic draw
             return None if aten is None else (step * aten["per_step"] + (aten["inc_g"] if critic else 0), self._aten_dev[1:2],
@@ -1189,7 +1283,8 @@ class MaskGit(nn.Module):
             s = step % timesteps
             if edit and s == 0:
                 ops.edit_select(ids, scores, frozen, region["keep"], region["num_select"], self.mask_id, step // timesteps,
-                                u=self._injected_noise(step, (b, n), device), seed_dev=self._seed_dev, row_offset=self.row_offset * n)
+                                u=self._injected_noise(step, (b, n), device), seed_dev=self._seed_dev, row_offset=self.row_offset * n,
+                                image_seed=seeds)
             if window is not None and s == 0:
                 ops.extrapolate_window(canvas, ids, scores, window.corners[step // timesteps], window.direction, window.stride, self.mask_id)
             if nvtx:
@@ -1206,6 +1301,7 @@ class MaskGit(nn.Module):
                 a.temperature = float(temp); a.cond_scale = float(lead(req.cond_scale))
                 a.temperature_dev = temp_dev.data_ptr(); a.cond_scale_dev = settings["cond_scale"].data_ptr()
                 a.u = None if u is None else u.data_ptr(); a.seed = 0; a.seed_dev = self._seed_dev.data_ptr(); a.row_offset = self.row_offset * n
+                a.image_seed = None if seeds is None else seeds.data_ptr()
                 _lib.call("mmg_decode_step", a)
                 continue
             if req.region is None:
@@ -1219,13 +1315,13 @@ class MaskGit(nn.Module):
             pos, rows_b = (all_pos, n) if score_all else (masked_pos, num_masked)
             self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(lead(req.cond_scale)), k_keep, tail, seed_dev=seed_dev,
                               only_masked_id=self.mask_id if score_all or req.region is not None else None, aten=aten_draw(step),
-                              temp_dev=temp_dev, cond_scale_dev=settings["cond_scale"])
+                              temp_dev=temp_dev, cond_scale_dev=settings["cond_scale"], image_seed=seeds)
             if req.use_critic:
                 xc = cnet._run_blocks(ids, cctx, cnb)
                 ops.critic_score(xc[:bn], xc[bn:2 * bn] if cnb == 2 else None, gcrit, whead, float(bhead), float(lead(req.cond_scale)),
                                  float(lead(req.critic_noise_scale) * (steps_until_x0 / timesteps)), scores, u=self._injected_noise(step, (b, n), device),
                                  seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, aten=aten_draw(step, critic=True),
-                                 cond_scale_dev=settings["crit_cond_scale"], noise_mul_dev=settings["crit_noise"][s])
+                                 cond_scale_dev=settings["crit_cond_scale"], noise_mul_dev=settings["crit_noise"][s], row_key=crit_key)
             if window is not None and s == timesteps - 1:
                 ops.extrapolate_window(canvas, ids, scores, window.corners[step // timesteps], window.direction, window.stride, self.mask_id,
                                        store=True)
@@ -1380,11 +1476,15 @@ class Muse(nn.Module):
 
     @torch.no_grad()
     def forward(self, texts: List[str], cond_scale=3., temperature=1., timesteps=18, superres_timesteps=None,
-                return_lowres=False, return_pil_images=True):
-        """cond_scale / temperature: a number or per image (see MaskGit.generate), used by both stages."""
-        lowres = self.base_maskgit.generate(texts=texts, cond_scale=cond_scale, temperature=temperature, timesteps=timesteps)
+                return_lowres=False, return_pil_images=True, image_seeds=None):
+        """cond_scale / temperature: a number or per image (see MaskGit.generate), used by both stages.  image_seeds: per-image seeds in any
+        form MaskGit.generate takes.  The base stage samples with them as given and the super-resolution stage with splitmix64 of each, so the
+        two stages do not draw the same stream at shared positions; either stage alone is reproduced by its generate() with those seeds."""
+        seeds = _image_seeds(image_seeds, len(texts))
+        lowres = self.base_maskgit.generate(texts=texts, cond_scale=cond_scale, temperature=temperature, timesteps=timesteps, image_seeds=seeds)
         superres = self.superres_maskgit.generate(texts=texts, cond_scale=cond_scale, cond_images=lowres, temperature=temperature,
-                                                  timesteps=superres_timesteps if superres_timesteps is not None else timesteps)
+                                                  timesteps=superres_timesteps if superres_timesteps is not None else timesteps,
+                                                  image_seeds=None if seeds is None else [splitmix64(v) for v in seeds])
         return _muse_result(superres, lowres, return_lowres, return_pil_images)
 
 

@@ -343,10 +343,11 @@ def remask_frozen(ids, scores, masked_pos, frozen, num_masked, rows, mask_id):
     L.call("mmg_remask_frozen", a)
 
 
-def edit_select(ids, scores, frozen_out, keep, num_select, mask_id, iteration, u=None, seed=0, seed_dev=None, row_offset=0):
+def edit_select(ids, scores, frozen_out, keep, num_select, mask_id, iteration, u=None, seed=0, seed_dev=None, row_offset=0, image_seed=None):
     """One mask-free editing selection: each sequence selects its num_select (int32 [B]) largest keys among the positions with keep == 0
     (uint8 [B, n]); keys are u (fp32 [B, n]) or libmmg's Philox stream for `iteration`.  Writes frozen_out (uint8 [B, n], 1 = not
-    selected), mask_id at the selected ids and 0 into every score."""
+    selected), mask_id at the selected ids and 0 into every score.  image_seed: int64 [B] per-image Philox keys (uint64 bits), keyed on
+    the image-local position in place of (seed, global position)."""
     for t, name in ((ids, "ids"), (scores, "scores"), (frozen_out, "frozen_out"), (keep, "keep"), (num_select, "num_select")):
         _chk(t, name)
     assert frozen_out.dtype == keep.dtype == torch.uint8 and frozen_out.shape == keep.shape == ids.shape == scores.shape
@@ -357,6 +358,7 @@ def edit_select(ids, scores, frozen_out, keep, num_select, mask_id, iteration, u
     a = L.EditSelectArgs()
     a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.frozen_out = frozen_out.data_ptr(); a.keep = keep.data_ptr()
     a.num_select = num_select.data_ptr(); a.u = L.ptr(u); a.seed = seed; a.seed_dev = L.ptr(seed_dev); a.row_offset = row_offset
+    a.image_seed = _seed_table(image_seed, ids.shape[0], "image_seed")
     a.B, a.n = ids.shape; a.iteration = iteration; a.mask_id = mask_id
     L.call("mmg_edit_select", a)
 
@@ -387,6 +389,14 @@ def _per_row_table(t, rows, name):
     return L.ptr(t)
 
 
+def _seed_table(t, rows, name, width=1):
+    """An int64 device table of `rows` x `width` Philox words (read as uint64), or None."""
+    if t is not None:
+        _chk(t, name)
+        assert t.dtype == torch.int64 and t.numel() == rows * width, f"{name}: int64 [{rows}{', %d' % width if width > 1 else ''}]"
+    return L.ptr(t)
+
+
 def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_scale, cond_scale_dev=None):
     """cond_scale_dev: fp32 [B] per-image scales (read on the device in place of cond_scale); an image at exactly 1 takes LN(x_cond)."""
     a = L.FinalEmbedArgs()
@@ -398,14 +408,16 @@ def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_sca
 
 
 def logits_sample(logits, masked_pos, ids, scores, num_masked, k, temperature, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
-                  only_masked_id=None, aten=None, temperature_dev=None):
+                  only_masked_id=None, aten=None, temperature_dev=None, image_seed=None):
     """aten = (offset, offset_dev, stride): draw the noise from ATen's CUDA uniform_ stream instead of libmmg's keying.
-    temperature_dev: fp32 [B] per-image temperatures, read on the device in place of `temperature`."""
+    temperature_dev: fp32 [B] per-image temperatures, read on the device in place of `temperature`.  image_seed: int64 [B] per-image
+    Philox keys (uint64 bits): image b draws with its own key and its positions as row counters, in place of (seed, global row)."""
     a = L.LogitsSampleArgs()
     a.logits = _chk(logits).data_ptr(); a.masked_pos = masked_pos.data_ptr(); a.ids = ids.data_ptr(); a.scores = scores.data_ptr()
     a.u = L.ptr(u)
     a.B, a.n = ids.shape; a.num_masked = num_masked; a.V = logits.shape[-1]; a.k = k; a.temperature = temperature
     a.temperature_dev = _per_row_table(temperature_dev, a.B, "temperature_dev")
+    a.image_seed = _seed_table(image_seed, a.B, "image_seed")
     a.seed = seed; a.step = step; a.row_offset = row_offset; a.seed_dev = L.ptr(seed_dev)
     if only_masked_id is not None:
         a.only_masked = 1; a.mask_id = only_masked_id
@@ -420,9 +432,9 @@ def logits_fused_workspace_bytes(rows_capacity, V, K, k):
 
 
 def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, workspace, status, rows_capacity=0, u=None, seed=0, step=0,
-                 row_offset=0, seed_dev=None, only_masked_id=None, aten=None, temperature_dev=None):
+                 row_offset=0, seed_dev=None, only_masked_id=None, aten=None, temperature_dev=None, image_seed=None):
     """to_logits + top-k / gumbel argmax / confidence on the rows listed in masked_pos without a [rows, V] logits buffer.
-    temperature_dev: as for logits_sample."""
+    temperature_dev, image_seed: as for logits_sample."""
     a = L.LogitsFusedArgs()
     a.e = _chk(e).data_ptr(); a.w = _chk(w).data_ptr(); a.K = e.shape[1]; a.rows_capacity = rows_capacity
     assert e.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and w.shape[1] == e.shape[1]
@@ -431,6 +443,7 @@ def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, work
     s.masked_pos = masked_pos.data_ptr(); s.ids = ids.data_ptr(); s.scores = scores.data_ptr(); s.u = L.ptr(u)
     s.B, s.n = ids.shape; s.num_masked = num_masked; s.V = w.shape[0]; s.k = k; s.temperature = temperature
     s.temperature_dev = _per_row_table(temperature_dev, s.B, "temperature_dev")
+    s.image_seed = _seed_table(image_seed, s.B, "image_seed")
     s.seed = seed; s.step = step; s.row_offset = row_offset; s.seed_dev = L.ptr(seed_dev)
     if only_masked_id is not None:
         s.only_masked = 1; s.mask_id = only_masked_id
@@ -471,14 +484,16 @@ def logits_xent_rows(logits, labels, nll):
 
 
 def critic_score(x_cond, x_null, gamma, w, bias, cond_scale, noise_mul, scores, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
-                 aten=None, cond_scale_dev=None, noise_mul_dev=None):
+                 aten=None, cond_scale_dev=None, noise_mul_dev=None, row_key=None):
     """scores[r] = CFG(dot(LN(x[r]) * gamma, w) + bias) + (u[r] - 0.5) * noise_mul   (ref: muse_maskgit_pytorch.py:590-600)
-    cond_scale_dev / noise_mul_dev: fp32 [rows] per-row values read on the device in place of the scalars."""
+    cond_scale_dev / noise_mul_dev: fp32 [rows] per-row values read on the device in place of the scalars.  row_key: int64 [rows, 2]
+    per-row (Philox key, row counter), read as uint64, in place of (seed, row_offset + r)."""
     a = L.CriticScoreArgs()
     a.x_cond = _chk(x_cond).data_ptr(); a.x_null = L.ptr(x_null); a.gamma = gamma.data_ptr(); a.w = _chk(w).data_ptr()
     a.bias = bias; a.cond_scale = cond_scale; a.noise_mul = noise_mul; a.dim = x_cond.shape[-1]
     a.cond_scale_dev = _per_row_table(cond_scale_dev, scores.numel(), "cond_scale_dev")
     a.noise_mul_dev = _per_row_table(noise_mul_dev, scores.numel(), "noise_mul_dev")
+    a.row_key = _seed_table(row_key, scores.numel(), "row_key", width=2)
     a.u = L.ptr(u); a.scores = scores.data_ptr(); a.rows = scores.numel(); a.row_offset = row_offset
     a.seed = seed; a.seed_dev = L.ptr(seed_dev); a.step = step
     assert x_cond.dtype == torch.float32 and w.dtype == torch.float32 and x_cond.shape[0] >= a.rows

@@ -1,13 +1,14 @@
 """Batch-sharded generation and editing over the GPUs of one node (SURVEY.md 8e): every sequence is independent through the whole
 of generate(), inpaint(), edit(), extrapolate() and the Muse cascade, so rank r runs a contiguous slice of the batch with replicated weights and the
 results are assembled with all-gathers at the end.  No collective runs inside the decode loop.  The sampler's Philox counters are
-keyed on the global sequence index (MaskGit.row_offset), so token ids do not depend on the number of ranks."""
+keyed on the global sequence index (MaskGit.row_offset), so token ids do not depend on the number of ranks; with `image_seeds` (one seed
+per image, sliced by global row like the per-image settings) each image's noise depends on its own seed alone."""
 import numbers
 
 import torch
 import torch.distributed as dist
 
-from .muse_maskgit import _muse_result
+from .muse_maskgit import _image_seeds, _muse_result
 
 PER_IMAGE_SETTINGS = ("temperature", "cond_scale", "critic_noise_scale")
 ROW_INPUTS = ("images", "mask", "cond_images")      # call inputs indexed by global row, sliced like `texts`
@@ -75,7 +76,9 @@ def _run_shard(method, maskgits, texts, lo, hi, total, empty, *, group=None, see
     total and one seed shared by every rank: seeds[i] when given (no communication), else its sampler_seed or a draw from torch's
     generator, as rank 0 of `group` has them.  text_embeds (rows of the whole batch) or text_embeds_shard (rows [lo, hi)) replace every
     maskgit transformer's encode_text.  kwargs named in ROW_INPUTS and per-image settings given per image are indexed by global row and
-    sliced here; cond_images_shard replaces the slice of cond_images.  The attributes are restored on return, also when the call raises."""
+    sliced here; cond_images_shard replaces the slice of cond_images.  image_seeds (per-image seeds in any form generate() takes, for the
+    whole batch) become this rank's rows' seeds; no call seed is then drawn or broadcast, since no kernel reads it.  The attributes are
+    restored on return, also when the call raises."""
     for name in PER_IMAGE_SETTINGS:       # per-image settings (a sequence or 1-D tensor of `total` values) are sliced like text_embeds
         value = kwargs.get(name)
         if value is None or isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
@@ -92,6 +95,10 @@ def _run_shard(method, maskgits, texts, lo, hi, total, empty, *, group=None, see
         kwargs[name] = value[lo:hi]
     if cond_images_shard is not None:
         kwargs["cond_images"] = cond_images_shard
+    if kwargs.get("image_seeds") is not None:
+        kwargs["image_seeds"] = _image_seeds(kwargs["image_seeds"], total)[lo:hi]
+        if seeds is None:
+            seeds = [m.sampler_seed for m in maskgits]
     if seeds is None:
         seeds = [m.sampler_seed if m.sampler_seed is not None else int(torch.randint(0, 2 ** 62, (1,)).item()) for m in maskgits]
         if dist.is_initialized() and dist.get_world_size(group) > 1:
@@ -138,7 +145,9 @@ def generate_sharded(maskgit, texts, text_embeds=None, cond_images=None, group=N
     The sampler noise is keyed on the global sequence index, so the token ids do not depend on the number of ranks:
     "mmg" mode uses ONE seed for all ranks — `seed` when the caller passes the same value on every rank (no communication), else rank
     0's `sampler_seed` or its draw from torch's generator, broadcast; "aten" mode is told the size of the whole batch the reference would
-    have drawn noise for (`global_batch`).  Not with `sampler_noise_fn`: the callable sees only this rank's shape."""
+    have drawn noise for (`global_batch`).  Not with `sampler_noise_fn`: the callable sees only this rank's shape.  `image_seeds` (one
+    seed per image of the whole batch, a keyword separate from the call-wide `seed`) is sliced by global row; each image's result then
+    depends on its own seed, not on `seed`, its rank or row_offset."""
     return _sharded_call(maskgit, maskgit.generate, texts, group, seed,
                          dict(generate_kwargs, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard, cond_images=cond_images,
                               cond_images_shard=cond_images_shard))
@@ -151,7 +160,7 @@ def inpaint_sharded(maskgit, texts, images, mask, text_embeds=None, cond_images=
     rank counts the regenerated tokens of its own rows only, and samples mask_schedule(its largest count) rows per image and step.
 
     Seeds and the rank-count invariance of the token ids are generate_sharded's: one seed for every rank in "mmg" mode, `global_batch`
-    in "aten" mode; not with `sampler_noise_fn`."""
+    in "aten" mode; not with `sampler_noise_fn`.  `image_seeds` is sliced by global row, as for generate_sharded."""
     return _sharded_call(maskgit, maskgit.inpaint, texts, group, seed,
                          dict(inpaint_kwargs, images=images, mask=mask, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard,
                               cond_images=cond_images, cond_images_shard=cond_images_shard))
@@ -161,7 +170,8 @@ def edit_sharded(maskgit, texts, images, mask=None, text_embeds=None, cond_image
                  cond_images_shard=None, seed=None, **edit_kwargs):
     """maskgit.edit over this rank's rows, then the all-gather, sliced as inpaint_sharded (`mask` may be None: every token editable).
     The selection keys are keyed on the global position too, so with one seed for every rank ("mmg" mode) the token ids do not depend
-    on the number of ranks.  sampler_rng = "aten" raises ValueError on every rank, as edit() does; `sampler_noise_fn` is not covered."""
+    on the number of ranks.  sampler_rng = "aten" raises ValueError on every rank, as edit() does; `sampler_noise_fn` is not covered.
+    `image_seeds` is sliced by global row, as for generate_sharded."""
     if maskgit.sampler_rng == "aten":          # raised here, before any collective, so that ranks without rows raise it too
         raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
     return _sharded_call(maskgit, maskgit.edit, texts, group, seed,
@@ -176,7 +186,7 @@ def extrapolate_sharded(maskgit, texts, images, direction="right", amount=256, t
     (0, C, H', W') / (0, H'/p, W'/p) shapes.  The arguments are checked on the whole batch before any collective, so every rank raises the
     same ValueError.  The sampler noise is keyed on the global row and the window-local position, so with one seed for every rank ("mmg"
     mode) the token ids do not depend on the number of ranks; sampler_rng = "aten" raises ValueError, as extrapolate() does, and
-    `sampler_noise_fn` is not covered."""
+    `sampler_noise_fn` is not covered.  `image_seeds` is sliced by global row, as for generate_sharded."""
     window = maskgit._extrapolate_plan(images, len(texts), direction, amount, extrapolate_kwargs.get("stride"))
     p = maskgit.vae.dim_divisor
     return _sharded_call(maskgit, maskgit.extrapolate, texts, group, seed,
@@ -192,7 +202,8 @@ def muse_sharded(muse, texts, text_embeds=None, group=None, *, text_embeds_shard
 
     Seeds: each stage's own `sampler_seed`, else a draw from torch's generator, base first, as one process draws them; rank 0's pair
     reaches every rank in one broadcast.  text_embeds / text_embeds_shard are handed to both stages' transformers.  Per-image
-    cond_scale / temperature are sliced by global row.  Token ids do not depend on the number of ranks, as for generate_sharded."""
+    cond_scale / temperature are sliced by global row.  Token ids do not depend on the number of ranks, as for generate_sharded.
+    `image_seeds` is sliced by global row; Muse.forward derives the super-resolution seeds from each rank's slice."""
     return_lowres = forward_kwargs.pop("return_lowres", False)
     return_pil_images = forward_kwargs.pop("return_pil_images", True)
     world = dist.get_world_size(group) if dist.is_initialized() else 1
