@@ -467,18 +467,7 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
   bool fallback = s_bad || n < k;
   if (!fallback) {
     const uint2* row_lists = f.lists + r * (int64_t)nseg * f.cap;
-    uint64_t seed; int64_t grow;
-    row_noise_key<MODE>(a, b, pos, seed, grow);
-    tdiv = image_tdiv(a, b, tdiv);
-    const float inv_t = 1.0f / tdiv;
-    uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
-    if (MODE == 2) {            // flat index of logit (grow, v) in the reference's [B, n, V] noise tensor = grow * V + v = ar0 + v + S * aq0
-      const uint64_t base = (uint64_t)grow * (uint64_t)V;
-      aq0 = base / a.aten_stride; ar0 = (uint32_t)(base - aq0 * a.aten_stride);
-      aoff4 = (a.aten_offset + (a.aten_offset_dev ? *a.aten_offset_dev : 0ull)) >> 2;
-    }
-    PhiloxRow prow;
-    if (MODE == 0) prow = philox_row((uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed, (uint32_t)(seed >> 32));
+    const RowNoise<MODE> noise = row_noise<MODE>(a, b, pos, V, tdiv);
     int win_v = -1; float win_x = 0.f;
     for (int nex = 0; ; ++nex) {
       // ---- pass 1: perturbed argmax over the candidates that have not failed the rank test
@@ -488,19 +477,7 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
         bool skip = false;
         for (int e = 0; e < nex; ++e) skip |= s_excl[e] == v;
         if (skip) return;
-        const float x = __uint_as_float(xb);
-        float p;
-        if (MODE != 0) {
-          float u;
-          if (MODE == 1) u = a.u[((int64_t)b * a.n + pos) * V + v];
-          else { const uint32_t q = ar0 + (uint32_t)v, dq = q / a.aten_stride; u = aten_uniform(q - dq * a.aten_stride, aq0 + dq, aoff4, seed); }
-          const float l1 = logf(fmaxf(u, 1e-20f));
-          p = __fdiv_rn(x, tdiv) - logf(fmaxf(-l1, 1e-20f));
-        } else {
-          const float u = (float)(philox_first_row((uint32_t)v, prow) >> 8) * (1.0f / 16777216.0f);
-          const float l1 = __logf(fmaxf(u, 1e-20f));
-          p = fmaf(x, inv_t, -__logf(fmaxf(-l1, 1e-20f)));
-        }
+        const float p = noise.perturbed(__uint_as_float(xb), v);
         if (bi == 0x7fffffff || better(p, v, bv, bi)) { bv = p; bi = v; bx = xb; }
       });
 #pragma unroll
@@ -539,9 +516,7 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
     if (!fallback) {
       if (tid == 0) {
         if (win_v < 0) { const uint2 e0 = row_lists[0]; win_v = (int)e0.y; win_x = __uint_as_float(e0.x); }    // degenerate rows (NaN logits)
-        const float pr = expf(win_x - s_max) / s_sum;
-        if (!a.only_masked || a.ids[(int64_t)b * a.n + pos] == a.mask_id) a.ids[(int64_t)b * a.n + pos] = win_v;
-        a.scores[(int64_t)b * a.n + pos] = 1.0f - pr;
+        write_sample(a, b, pos, win_v, expf(win_x - s_max) / s_sum);
       }
       return;
     }
@@ -738,9 +713,7 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
   const mmg_logits_sample_args& s = a->s;
   MMG_CHECK_ARG(s.masked_pos && s.ids && s.scores, "mmg_logits_fused: NULL sampler pointer");
   MMG_CHECK_ARG(lf_supported(s.V, a->K, s.k), "mmg_logits_fused: unsupported V=%d K=%d k=%d (use mmg_linear + mmg_logits_sample)", s.V, a->K, s.k);
-  MMG_CHECK_ARG(s.rng_mode == 0 || (s.rng_mode == 1 && s.aten_stride >= 256 && s.aten_stride % 256 == 0 && s.aten_offset % 4 == 0 && !s.u),
-                "mmg_logits_fused: rng_mode=%d aten_stride=%u", s.rng_mode, s.aten_stride);
-  MMG_CHECK_ARG(!s.image_seed || (s.rng_mode == 0 && !s.u), "mmg_logits_fused: image_seed needs rng_mode 0 and u == NULL");
+  if (int rc = check_noise_args(s, "mmg_logits_fused")) return rc;
   const int64_t R = (int64_t)s.B * s.num_masked;
   if (R == 0) return MMG_OK;
   const int64_t R_cap = a->rows_capacity > 0 ? a->rows_capacity : R;
@@ -786,10 +759,9 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
     f.parts = parts; f.lists = lists; f.S = pl.S; f.cap = pl.cap; f.e = reinterpret_cast<const bf16*>(a->e); f.K = a->K;
     f.fb_count = fb_count; f.fb_rows = fb_rows; f.e_fb = e_fb; f.fb_cap = LF_FB_CAP; f.status = a->status;
     static const int minb = [] { const char* e = getenv("MMG_FINISH_MINB"); return e ? atoi(e) : 4; }();
-    if (s.u) MMG_CUDA(launch_pdl(logits_finish_kernel<1, 4>, dim3((unsigned)R), dim3(LFN_THREADS), 0, st, s, t, f));
-    else if (s.rng_mode == 1) MMG_CUDA(launch_pdl(logits_finish_kernel<2, 4>, dim3((unsigned)R), dim3(LFN_THREADS), 0, st, s, t, f));
-    else if (minb == 6) MMG_CUDA(launch_pdl(logits_finish_kernel<0, 6>, dim3((unsigned)R), dim3(LFN_THREADS), 0, st, s, t, f));
-    else MMG_CUDA(launch_pdl(logits_finish_kernel<0, 4>, dim3((unsigned)R), dim3(LFN_THREADS), 0, st, s, t, f));
+    static void (*const finish_kernels[3])(mmg_logits_sample_args, float, LfFinish) = {
+        minb == 6 ? logits_finish_kernel<0, 6> : logits_finish_kernel<0, 4>, logits_finish_kernel<1, 4>, logits_finish_kernel<2, 4>};
+    MMG_CUDA(launch_pdl(finish_kernels[noise_mode(s)], dim3((unsigned)R), dim3(LFN_THREADS), 0, st, s, t, f));
     MMG_LAUNCHED();
   }
   {   // 5. fallback rows: materialised logits of at most LF_FB_CAP rows (the kernel exits at once when no row was flagged)

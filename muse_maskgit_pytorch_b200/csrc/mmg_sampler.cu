@@ -15,9 +15,7 @@
 
 namespace mmg {
 
-// MODE 1 = injected-noise parity mode, MODE 2 = ATen-compatible in-kernel Philox (the stream a seeded torch.cuda run of the
-// reference draws): IEEE division and accurate logf so the perturbed values match the reference's fp32 arithmetic as closely
-// as a GPU can; MODE 0 (libmmg's own Philox keying) uses fast MUFU-based logs and a reciprocal multiply.
+// MODE: the noise stream (RowNoise in mmg_sampler.cuh)
 template <int MODE>
 __global__ void __launch_bounds__(SMP_THREADS)
 logits_sample_kernel(const mmg_logits_sample_args a, float tdiv) {
@@ -231,12 +229,10 @@ logits_sample_kernel(const mmg_logits_sample_args a, float tdiv) {
 
   // ---------------- phase C: perturbed argmax restricted to the exact top-k ----------------
   int win_v; float win_x;
-  sample_from_list<MODE>(a, image_tdiv(a, b, tdiv), lval, lidx, n, k, V, b, pos, sc, tid, warp, lane, win_v, win_x);
+  sample_from_list(row_noise<MODE>(a, b, pos, V, tdiv), lval, lidx, n, k, sc, tid, warp, lane, win_v, win_x);
   if (tid == 0) {
     if (win_v < 0) { win_v = 0; win_x = row[0]; }                 // degenerate rows (all -inf / NaN)
-    const float p = expf(win_x - s_max) / s_sum;
-    if (!a.only_masked || a.ids[(int64_t)b * a.n + pos] == a.mask_id) a.ids[(int64_t)b * a.n + pos] = win_v;
-    a.scores[(int64_t)b * a.n + pos] = 1.0f - p;
+    write_sample(a, b, pos, win_v, expf(win_x - s_max) / s_sum);
   }
 }
 
@@ -253,7 +249,8 @@ __global__ void __launch_bounds__(SMP_THREADS)
 logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   __shared__ SampleScratch sc;
   __shared__ int s_cut;
-  __shared__ float s_m, s_s, s_tdiv;
+  __shared__ float s_m, s_s;
+  __shared__ RowNoise<MODE> s_noise;
   pdl_wait(); pdl_trigger();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int V = a.V, k = a.k;
@@ -262,8 +259,9 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   if (a.row_index) { if ((int)blockIdx.x >= *a.row_count_dev) return; r = a.row_index[blockIdx.x]; }
   const int b = (int)(r / a.num_masked);
   const int pos = a.masked_pos[r];
-  // the row's temperature, read after the descent loop's barriers.  Held in a register across that loop, it made MODE 2 spill 8 bytes.
-  if (tid == 0) s_tdiv = image_tdiv(a, b, tdiv);
+  // the row's noise, set up by one thread and read after the descent loop's barriers.  Held in registers across that loop, the
+  // temperature made MODE 2 spill 8 bytes.
+  if (tid == 0) s_noise = row_noise<MODE>(a, b, pos, V, tdiv);
   // 1. k-th largest key
   uint32_t prefix = 0;
   for (int bit = 31; bit >= 0; --bit) {
@@ -301,15 +299,7 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   __syncthreads();
   const int cut = s_cut;
   // 2. statistics + perturbed argmax over the kept set
-  uint64_t seed; int64_t grow;
-  row_noise_key<MODE>(a, b, pos, seed, grow);
-  const float inv_t = 1.0f / s_tdiv;
-  uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
-  if (MODE == 2) {
-    const uint64_t base = (uint64_t)grow * (uint64_t)V;
-    aq0 = base / a.aten_stride; ar0 = (uint32_t)(base - aq0 * a.aten_stride);
-    aoff4 = (a.aten_offset + (a.aten_offset_dev ? *a.aten_offset_dev : 0ull)) >> 2;
-  }
+  const RowNoise<MODE> noise = s_noise;
   constexpr float LOG2E = 1.4426950408889634f;
   float m_t = -1e30f, s_t = 0.f;
   float bv = -FLT_MAX, bx = 0.f; int bi = 0x7fffffff;
@@ -319,18 +309,7 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
     s_t += ex2_approx((x - m_t) * LOG2E);
     const uint32_t key = fkey(x);
     if (key > prefix || (key == prefix && v <= cut)) {
-      float p;
-      if (MODE != 0) {
-        float u;
-        if (MODE == 1) u = a.u[((int64_t)b * a.n + pos) * V + v];
-        else { const uint32_t rr = ar0 + (uint32_t)v, dq = rr / a.aten_stride; u = aten_uniform(rr - dq * a.aten_stride, aq0 + dq, aoff4, seed); }
-        const float l1 = logf(fmaxf(u, 1e-20f));
-        p = __fdiv_rn(x, s_tdiv) - logf(fmaxf(-l1, 1e-20f));
-      } else {
-        const float u = (float)(philox_first((uint32_t)v, (uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed, (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
-        const float l1 = __logf(fmaxf(u, 1e-20f));
-        p = fmaf(x, inv_t, -__logf(fmaxf(-l1, 1e-20f)));
-      }
+      const float p = noise.perturbed(x, v);
       if (bi == 0x7fffffff || better(p, v, bv, bi)) { bv = p; bi = v; bx = x; }
     }
   }
@@ -363,9 +342,7 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
       if (oi != 0x7fffffff && (bi == 0x7fffffff || better(ov, oi, bv, bi))) { bv = ov; bi = oi; bx = __int_as_float(sc.redj[w]); }
     }
     if (bi == 0x7fffffff) { bi = 0; bx = row[0]; }                 // degenerate rows (all -inf / NaN)
-    const float pr = expf(bx - s_m) / s_s;
-    if (!a.only_masked || a.ids[(int64_t)b * a.n + pos] == a.mask_id) a.ids[(int64_t)b * a.n + pos] = bi;
-    a.scores[(int64_t)b * a.n + pos] = 1.0f - pr;
+    write_sample(a, b, pos, bi, expf(bx - s_m) / s_s);
   }
 }
 
@@ -466,17 +443,10 @@ edit_select_kernel(const mmg_edit_select_args a) {
   uint8_t* fz = reinterpret_cast<uint8_t*>(sc + 2 * n);
   const int64_t base = (int64_t)b * n;
   // per-image seeds: image b's own key and the image-local position as the row counter
-  const uint64_t seed = a.image_seed ? a.image_seed[b] : a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+  const uint64_t seed = a.image_seed ? a.image_seed[b] : call_seed(a.seed, a.seed_dev);
   const int64_t row0 = a.image_seed ? 0 : a.row_offset + base;
   for (int i = tid; i < n; i += 256) {
-    float u;
-    if (a.u) u = a.u[base + i];
-    else {
-      const int64_t grow = row0 + i;
-      u = (float)(philox_first(0xFFFFFFFEu, (uint32_t)a.iteration, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed,
-                               (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
-    }
-    sc[i] = u;
+    sc[i] = a.u ? a.u[base + i] : philox_uniform(PHILOX_C0_EDIT, (uint32_t)a.iteration, row0 + i, seed);
     fz[i] = a.keep[base + i] != 0;
   }
   __syncthreads();
@@ -547,13 +517,13 @@ critic_score_kernel(mmg_critic_score_args a) {
     if (a.u) u = a.u[row];
     else {
       // per-row keys: the row's image seed and image-local position
-      const uint64_t seed = a.row_key ? a.row_key[2 * row] : a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
+      const uint64_t seed = a.row_key ? a.row_key[2 * row] : call_seed(a.seed, a.seed_dev);
       const int64_t grow = a.row_key ? (int64_t)a.row_key[2 * row + 1] : a.row_offset + row;
       if (a.rng_mode == 1) {      // ATen stream of `uniform(scores.shape)`: flat index = global position
         const uint64_t k = (uint64_t)grow / a.aten_stride;
-        u = aten_uniform((uint32_t)((uint64_t)grow - k * a.aten_stride), k, (a.aten_offset + (a.aten_offset_dev ? *a.aten_offset_dev : 0ull)) >> 2, seed);
+        u = aten_uniform((uint32_t)((uint64_t)grow - k * a.aten_stride), k, aten_offset4(a.aten_offset, a.aten_offset_dev), seed);
       } else
-        u = (float)(philox_first(0xFFFFFFFFu, (uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed, (uint32_t)(seed >> 32)) >> 8) * (1.0f / 16777216.0f);
+        u = philox_uniform(PHILOX_C0_CRITIC, (uint32_t)a.step, grow, seed);
     }
     a.scores[row] = s + (u - 0.5f) * (a.noise_mul_dev ? a.noise_mul_dev[row] : a.noise_mul);
   }
@@ -572,25 +542,22 @@ extern "C" int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream) 
   const int64_t R = a->row_index ? a->row_index_cap : (int64_t)a->B * a->num_masked;
   if (R == 0) return MMG_OK;
   static const size_t smem = (size_t)SMP_CAP * 8 + (size_t)SMP_THREADS * 64;
-  MMG_CHECK_ARG(a->rng_mode == 0 || (a->rng_mode == 1 && a->aten_stride >= 256 && a->aten_stride % 256 == 0 && a->aten_offset % 4 == 0 && !a->u),
-                "mmg_logits_sample: rng_mode=%d aten_stride=%u", a->rng_mode, a->aten_stride);
-  MMG_CHECK_ARG(!a->image_seed || (a->rng_mode == 0 && !a->u), "mmg_logits_sample: image_seed needs rng_mode 0 and u == NULL");
-  static cudaError_t attr0 = cudaFuncSetAttribute(logits_sample_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  static cudaError_t attr1 = cudaFuncSetAttribute(logits_sample_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  static cudaError_t attr2 = cudaFuncSetAttribute(logits_sample_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (attr0 != cudaSuccess || attr1 != cudaSuccess || attr2 != cudaSuccess)
-    return fail(MMG_ECUDA, "cudaFuncSetAttribute(logits_sample): %s", cudaGetErrorString(attr0 != cudaSuccess ? attr0 : attr1 != cudaSuccess ? attr1 : attr2));
+  if (int rc = check_noise_args(*a, "mmg_logits_sample")) return rc;
+  static void (*const list_kernels[3])(mmg_logits_sample_args, float) = {logits_sample_kernel<0>, logits_sample_kernel<1>, logits_sample_kernel<2>};
+  static void (*const bigk_kernels[3])(mmg_logits_sample_args, float) = {logits_sample_bigk_kernel<0>, logits_sample_bigk_kernel<1>,
+                                                                         logits_sample_bigk_kernel<2>};
+  static const cudaError_t attr = [] {
+    for (auto kern : list_kernels)
+      if (cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return e;
+    return cudaSuccess;
+  }();
+  if (attr != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(logits_sample): %s", cudaGetErrorString(attr));
   float t = a->temperature; if (t < 1e-10f) t = 1e-10f;      // max(temperature, 1e-10): muse_maskgit_pytorch.py:411
-  if (a->k > SMP_CAP) {                                        // kept set larger than the candidate list: the row-walking kernel
-    if (a->u) MMG_CUDA(launch_pdl(logits_sample_bigk_kernel<1>, dim3((unsigned)R), dim3(SMP_THREADS), 0, st, *a, t));
-    else if (a->rng_mode == 1) MMG_CUDA(launch_pdl(logits_sample_bigk_kernel<2>, dim3((unsigned)R), dim3(SMP_THREADS), 0, st, *a, t));
-    else MMG_CUDA(launch_pdl(logits_sample_bigk_kernel<0>, dim3((unsigned)R), dim3(SMP_THREADS), 0, st, *a, t));
-    MMG_LAUNCHED();
-    return MMG_OK;
-  }
-  if (a->u) MMG_CUDA(launch_pdl(logits_sample_kernel<1>, dim3((unsigned)R), dim3(SMP_THREADS), smem, st, *a, t));
-  else if (a->rng_mode == 1) MMG_CUDA(launch_pdl(logits_sample_kernel<2>, dim3((unsigned)R), dim3(SMP_THREADS), smem, st, *a, t));
-  else MMG_CUDA(launch_pdl(logits_sample_kernel<0>, dim3((unsigned)R), dim3(SMP_THREADS), smem, st, *a, t));
+  const int mode = noise_mode(*a);
+  if (a->k > SMP_CAP)                                          // kept set larger than the candidate list: the row-walking kernel
+    MMG_CUDA(launch_pdl(bigk_kernels[mode], dim3((unsigned)R), dim3(SMP_THREADS), 0, st, *a, t));
+  else
+    MMG_CUDA(launch_pdl(list_kernels[mode], dim3((unsigned)R), dim3(SMP_THREADS), smem, st, *a, t));
   MMG_LAUNCHED();
   return MMG_OK;
 }

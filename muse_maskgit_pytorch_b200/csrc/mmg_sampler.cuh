@@ -172,58 +172,87 @@ __device__ __forceinline__ float image_tdiv(const mmg_logits_sample_args& a, int
   return t < 1e-10f ? 1e-10f : t;
 }
 
-// Philox key and row counter of sampled row (b, pos): with per-image seeds (MODE 0 only) image b's own seed and the image-local position,
-// so its noise does not depend on the batch around it; otherwise seed + *seed_dev and the global row.
+// ---------------- the sampling noise ----------------
+// libmmg's noise streams are Philox4x32-10 with counter (c0, c1, row_lo, row_hi) and a 64-bit key (oracle/philox.py restates them).  The
+// gumbel noise takes c0 = the vocabulary index and c1 = the decode step; the token critic and the edit keys take c0 words no vocabulary
+// index reaches, so the three streams never share a counter.
+constexpr uint32_t PHILOX_C0_CRITIC = 0xFFFFFFFFu;
+constexpr uint32_t PHILOX_C0_EDIT = 0xFFFFFFFEu;
+
+// the uniform in [0, 1) of a Philox output word: its top 24 bits times 2^-24
+__device__ __forceinline__ float philox_unit(uint32_t w) { return (float)(w >> 8) * (1.0f / 16777216.0f); }
+__device__ __forceinline__ float philox_uniform(uint32_t c0, uint32_t c1, int64_t row, uint64_t seed) {
+  return philox_unit(philox_first(c0, c1, (uint32_t)row, (uint32_t)((uint64_t)row >> 32), (uint32_t)seed, (uint32_t)(seed >> 32)));
+}
+// the call's key: seed + *seed_dev (the device word lets a captured graph replay with a new seed)
+__device__ __forceinline__ uint64_t call_seed(uint64_t seed, const uint64_t* seed_dev) { return seed + (seed_dev ? *seed_dev : 0ull); }
+// ATen's generator offset (aten_offset + *aten_offset_dev) as a Philox counter word
+__device__ __forceinline__ uint64_t aten_offset4(uint64_t offset, const uint64_t* offset_dev) { return (offset + (offset_dev ? *offset_dev : 0ull)) >> 2; }
+
+// The noise of sampled row (b, pos), set up once per row: perturbed(x, v) = x / t - log(-log u_v) for the logit x of vocabulary index v.
+// MODE 0: libmmg's Philox, keyed on image b's own seed and the image-local position with per-image seeds, so the noise does not depend on
+//         the batch around it, else on the call seed and the global row; fast MUFU-based logs and a reciprocal multiply.
+// MODE 1: injected u.  MODE 2: the ATen stream a seeded torch.cuda run of the reference draws.  Both use IEEE division and accurate logf,
+//         so the perturbed values match the reference's fp32 arithmetic as closely as a GPU can.
 template <int MODE>
-__device__ __forceinline__ void row_noise_key(const mmg_logits_sample_args& a, int b, int pos, uint64_t& seed, int64_t& grow) {
-  if (MODE == 0 && a.image_seed) { seed = a.image_seed[b]; grow = pos; return; }
-  seed = a.seed + (a.seed_dev ? *a.seed_dev : 0ull);
-  grow = a.row_offset + (int64_t)b * a.n + pos;
+struct RowNoise {
+  const float* u;                       // MODE 1: the row's V injected uniforms
+  uint64_t seed, aq0, aoff4;            // MODE 2: logit v's flat index in the reference's [B, n, V] noise tensor is ar0 + v + stride * aq0
+  uint32_t ar0, stride;
+  float tdiv, inv_t;
+  PhiloxRow prow;                       // MODE 0
+  __device__ __forceinline__ float perturbed(float x, int v) const {
+    if (MODE == 0) {
+      const float l1 = __logf(fmaxf(philox_unit(philox_first_row((uint32_t)v, prow)), 1e-20f));
+      return fmaf(x, inv_t, -__logf(fmaxf(-l1, 1e-20f)));
+    }
+    float uv;
+    if (MODE == 1) uv = u[v];
+    else { const uint32_t r = ar0 + (uint32_t)v, dq = r / stride; uv = aten_uniform(r - dq * stride, aq0 + dq, aoff4, seed); }
+    const float l1 = logf(fmaxf(uv, 1e-20f));
+    return __fdiv_rn(x, tdiv) - logf(fmaxf(-l1, 1e-20f));
+  }
+};
+// tdiv: the launcher's clamped temperature; image b's own is read here.  The order of the reads below (key, temperature, then the Philox
+// row) keeps logits_finish_kernel<0, 4> at the instructions and registers it was tuned for.
+template <int MODE>
+__device__ __forceinline__ RowNoise<MODE> row_noise(const mmg_logits_sample_args& a, int b, int pos, int V, float tdiv) {
+  RowNoise<MODE> r{};
+  const bool own = MODE == 0 && a.image_seed;
+  r.seed = own ? a.image_seed[b] : call_seed(a.seed, a.seed_dev);
+  const int64_t grow = own ? pos : a.row_offset + (int64_t)b * a.n + pos;
+  if (MODE == 2) {
+    const uint64_t base = (uint64_t)grow * (uint64_t)V;
+    r.stride = a.aten_stride; r.aq0 = base / r.stride; r.ar0 = (uint32_t)(base - r.aq0 * r.stride);
+    r.aoff4 = aten_offset4(a.aten_offset, a.aten_offset_dev);
+  }
+  r.tdiv = image_tdiv(a, b, tdiv); r.inv_t = 1.0f / r.tdiv;
+  if (MODE == 0) r.prow = philox_row((uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)r.seed, (uint32_t)(r.seed >> 32));
+  if (MODE == 1) r.u = a.u + ((int64_t)b * a.n + pos) * V;
+  return r;
+}
+
+// the sampled token and its confidence 1 - p into (b, pos) of ids / scores; with only_masked the id lands only on a mask_id
+__device__ __forceinline__ void write_sample(const mmg_logits_sample_args& a, int b, int pos, int id, float p) {
+  const int64_t i = (int64_t)b * a.n + pos;
+  if (!a.only_masked || a.ids[i] == a.mask_id) a.ids[i] = id;
+  a.scores[i] = 1.0f - p;
 }
 
 // ---------------- phase C: perturbed argmax restricted to the exact top-k ----------------
-// lval / lidx: the n candidates of the row (every element >= some threshold, n >= k or the complete exact top-k); (b, pos): the row.
-// MODE 1 = injected-noise parity mode, MODE 2 = ATen-compatible in-kernel Philox (the stream a seeded torch.cuda run of the reference
-// draws): IEEE division and accurate logf so the perturbed values match the reference's fp32 arithmetic as closely as a GPU can;
-// MODE 0 (libmmg's own Philox keying) uses fast MUFU-based logs and a reciprocal multiply.
+// lval / lidx: the n candidates of the row (every element >= some threshold, n >= k or the complete exact top-k); noise: the row's.
 // Block argmax of the perturbed value, accepted iff the candidate's exact rank (#greater + #equal-with-lower-index) is < k, else
 // excluded and repeated: equals argmax over torch.topk's kept set without ever forming the set.  Returns (token, its logit) to every
 // thread; token < 0 for degenerate rows (all -inf / NaN).
 template <int MODE>
-__device__ __forceinline__ void sample_from_list(const mmg_logits_sample_args& a, float tdiv, const float* lval, const int* lidx, int n, int k, int V,
-                                                 int b, int pos, SampleScratch& sc, int tid, int warp, int lane, int& win_v, float& win_x) {
-  uint64_t seed; int64_t grow;
-  row_noise_key<MODE>(a, b, pos, seed, grow);
-  const float inv_t = 1.0f / tdiv;
-  uint64_t aq0 = 0, aoff4 = 0; uint32_t ar0 = 0;
-  if (MODE == 2) {            // flat index of logit (grow, v) in the reference's [B, n, V] noise tensor = grow * V + v = ar0 + v + S * aq0
-    const uint64_t base = (uint64_t)grow * (uint64_t)V;
-    aq0 = base / a.aten_stride; ar0 = (uint32_t)(base - aq0 * a.aten_stride);
-    aoff4 = (a.aten_offset + (a.aten_offset_dev ? *a.aten_offset_dev : 0ull)) >> 2;
-  }
+__device__ __forceinline__ void sample_from_list(const RowNoise<MODE>& noise, const float* lval, const int* lidx, int n, int k,
+                                                 SampleScratch& sc, int tid, int warp, int lane, int& win_v, float& win_x) {
   constexpr int PER = (SMP_CAP + SMP_THREADS - 1) / SMP_THREADS;
   float pv[PER];
-  PhiloxRow prow;
-  if (MODE == 0) prow = philox_row((uint32_t)a.step, (uint32_t)grow, (uint32_t)((uint64_t)grow >> 32), (uint32_t)seed, (uint32_t)(seed >> 32));
 #pragma unroll
   for (int j = 0; j < PER; ++j) {
     const int s = tid + j * SMP_THREADS;
-    float p = -FLT_MAX;
-    if (s < n) {
-      const int v = lidx[s];
-      if (MODE != 0) {
-        float u;
-        if (MODE == 1) u = a.u[((int64_t)b * a.n + pos) * V + v];
-        else { const uint32_t r = ar0 + (uint32_t)v, dq = r / a.aten_stride; u = aten_uniform(r - dq * a.aten_stride, aq0 + dq, aoff4, seed); }
-        const float l1 = logf(fmaxf(u, 1e-20f));
-        p = __fdiv_rn(lval[s], tdiv) - logf(fmaxf(-l1, 1e-20f));
-      } else {
-        const float u = (float)(philox_first_row((uint32_t)v, prow) >> 8) * (1.0f / 16777216.0f);
-        const float l1 = __logf(fmaxf(u, 1e-20f));
-        p = fmaf(lval[s], inv_t, -__logf(fmaxf(-l1, 1e-20f)));
-      }
-    }
-    pv[j] = p;
+    pv[j] = s < n ? noise.perturbed(lval[s], lidx[s]) : -FLT_MAX;
   }
   win_v = -1; win_x = 0.f;
   for (int iter = 0; iter < n; ++iter) {
@@ -259,6 +288,17 @@ __device__ __forceinline__ void sample_from_list(const mmg_logits_sample_args& a
 #pragma unroll
     for (int j = 0; j < PER; ++j) if (tid + j * SMP_THREADS == bs) pv[j] = -FLT_MAX;
   }
+}
+
+// ---------------- host side ----------------
+// the RowNoise MODE of a sampling call
+inline int noise_mode(const mmg_logits_sample_args& a) { return a.u ? 1 : a.rng_mode == 1 ? 2 : 0; }
+// the noise arguments mmg_logits_sample and mmg_logits_fused accept; `fn` names the entry point in the error text
+inline int check_noise_args(const mmg_logits_sample_args& a, const char* fn) {
+  MMG_CHECK_ARG(a.rng_mode == 0 || (a.rng_mode == 1 && a.aten_stride >= 256 && a.aten_stride % 256 == 0 && a.aten_offset % 4 == 0 && !a.u),
+                "%s: rng_mode=%d aten_stride=%u", fn, a.rng_mode, a.aten_stride);
+  MMG_CHECK_ARG(!a.image_seed || (a.rng_mode == 0 && !a.u), "%s: image_seed needs rng_mode 0 and u == NULL", fn);
+  return MMG_OK;
 }
 
 }  // namespace mmg

@@ -407,22 +407,34 @@ def final_embed(x_cond, x_null, gamma, masked_pos, e, B, n, num_masked, cond_sca
     return e
 
 
+def _set_aten(a, aten):
+    """aten = (offset, offset_dev, stride): the args draw their noise from ATen's CUDA uniform_ stream instead of libmmg's keying."""
+    if aten is not None:
+        a.rng_mode = 1; a.aten_offset = aten[0]; a.aten_offset_dev = L.ptr(aten[1]); a.aten_stride = aten[2]
+
+
+def _set_sampling(a, masked_pos, ids, scores, num_masked, V, k, temperature, u, seed, step, row_offset, seed_dev, only_masked_id, aten,
+                  temperature_dev, image_seed):
+    """Fills everything of a LogitsSampleArgs but the logits (the arguments of logits_sample)."""
+    a.masked_pos = masked_pos.data_ptr(); a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.u = L.ptr(u)
+    a.B, a.n = ids.shape; a.num_masked = num_masked; a.V = V; a.k = k; a.temperature = temperature
+    a.temperature_dev = _per_row_table(temperature_dev, a.B, "temperature_dev")
+    a.image_seed = _seed_table(image_seed, a.B, "image_seed")
+    a.seed = seed; a.step = step; a.row_offset = row_offset; a.seed_dev = L.ptr(seed_dev)
+    if only_masked_id is not None:
+        a.only_masked = 1; a.mask_id = only_masked_id
+    _set_aten(a, aten)
+
+
 def logits_sample(logits, masked_pos, ids, scores, num_masked, k, temperature, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
                   only_masked_id=None, aten=None, temperature_dev=None, image_seed=None):
     """aten = (offset, offset_dev, stride): draw the noise from ATen's CUDA uniform_ stream instead of libmmg's keying.
     temperature_dev: fp32 [B] per-image temperatures, read on the device in place of `temperature`.  image_seed: int64 [B] per-image
     Philox keys (uint64 bits): image b draws with its own key and its positions as row counters, in place of (seed, global row)."""
     a = L.LogitsSampleArgs()
-    a.logits = _chk(logits).data_ptr(); a.masked_pos = masked_pos.data_ptr(); a.ids = ids.data_ptr(); a.scores = scores.data_ptr()
-    a.u = L.ptr(u)
-    a.B, a.n = ids.shape; a.num_masked = num_masked; a.V = logits.shape[-1]; a.k = k; a.temperature = temperature
-    a.temperature_dev = _per_row_table(temperature_dev, a.B, "temperature_dev")
-    a.image_seed = _seed_table(image_seed, a.B, "image_seed")
-    a.seed = seed; a.step = step; a.row_offset = row_offset; a.seed_dev = L.ptr(seed_dev)
-    if only_masked_id is not None:
-        a.only_masked = 1; a.mask_id = only_masked_id
-    if aten is not None:
-        a.rng_mode = 1; a.aten_offset = aten[0]; a.aten_offset_dev = L.ptr(aten[1]); a.aten_stride = aten[2]
+    a.logits = _chk(logits).data_ptr()
+    _set_sampling(a, masked_pos, ids, scores, num_masked, logits.shape[-1], k, temperature, u, seed, step, row_offset, seed_dev,
+                  only_masked_id, aten, temperature_dev, image_seed)
     L.call("mmg_logits_sample", a)
 
 
@@ -439,16 +451,8 @@ def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, work
     a.e = _chk(e).data_ptr(); a.w = _chk(w).data_ptr(); a.K = e.shape[1]; a.rows_capacity = rows_capacity
     assert e.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and w.shape[1] == e.shape[1]
     a.workspace = workspace.data_ptr(); a.workspace_bytes = workspace.numel() * workspace.element_size(); a.status = status.data_ptr()
-    s = a.s
-    s.masked_pos = masked_pos.data_ptr(); s.ids = ids.data_ptr(); s.scores = scores.data_ptr(); s.u = L.ptr(u)
-    s.B, s.n = ids.shape; s.num_masked = num_masked; s.V = w.shape[0]; s.k = k; s.temperature = temperature
-    s.temperature_dev = _per_row_table(temperature_dev, s.B, "temperature_dev")
-    s.image_seed = _seed_table(image_seed, s.B, "image_seed")
-    s.seed = seed; s.step = step; s.row_offset = row_offset; s.seed_dev = L.ptr(seed_dev)
-    if only_masked_id is not None:
-        s.only_masked = 1; s.mask_id = only_masked_id
-    if aten is not None:
-        s.rng_mode = 1; s.aten_offset = aten[0]; s.aten_offset_dev = L.ptr(aten[1]); s.aten_stride = aten[2]
+    _set_sampling(a.s, masked_pos, ids, scores, num_masked, w.shape[0], k, temperature, u, seed, step, row_offset, seed_dev,
+                  only_masked_id, aten, temperature_dev, image_seed)
     L.call("mmg_logits_fused", a)
 
 
@@ -497,8 +501,7 @@ def critic_score(x_cond, x_null, gamma, w, bias, cond_scale, noise_mul, scores, 
     a.u = L.ptr(u); a.scores = scores.data_ptr(); a.rows = scores.numel(); a.row_offset = row_offset
     a.seed = seed; a.seed_dev = L.ptr(seed_dev); a.step = step
     assert x_cond.dtype == torch.float32 and w.dtype == torch.float32 and x_cond.shape[0] >= a.rows
-    if aten is not None:
-        a.rng_mode = 1; a.aten_offset = aten[0]; a.aten_offset_dev = L.ptr(aten[1]); a.aten_stride = aten[2]
+    _set_aten(a, aten)
     L.call("mmg_critic_score", a)
     return scores
 
