@@ -410,6 +410,13 @@ typedef struct {
   const uint64_t* image_seed;    /* [B] per-image Philox keys or NULL (rng_mode 0, u == NULL only): image b (found as for temperature_dev)
                                     draws with counter (v, step, pos, 0) and key image_seed[b] in place of (v, step, global row) and
                                     seed + *seed_dev; seed, seed_dev and row_offset are then not read                              */
+  const int32_t* k_dev;          /* [B] per-image top-k counts or NULL (use `k`): image b (found as for temperature_dev) keeps its k_dev[b]
+                                    largest logits.  `k` alone routes the call: k > 9216 takes the row-walking kernel, and
+                                    mmg_logits_fused needs lf_supported(V, K, k) (mmg_logits_fused_workspace_bytes != 0).  Every k_dev[b]
+                                    must lie in [1, V] on the same route as `k`: on the same side of 9216, and for mmg_logits_fused
+                                    supported like `k` (its largest value is the natural choice of `k`; nothing else is sized by k, so a
+                                    captured launch replays for any such table).  The candidate-list kernel clamps a count above 9216 to
+                                    9216, so a table off its route cannot write past the list                                         */
 } mmg_logits_sample_args;
 int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream);
 
@@ -562,6 +569,7 @@ typedef struct {
   const float* cond_scale_dev; const float* temperature_dev;   /* [b] per-image settings or NULL (use cond_scale / temperature): passed
                                                      to mmg_final_embed_args.cond_scale_dev / mmg_logits_sample_args.temperature_dev */
   const uint64_t* image_seed;                     /* [b] per-image Philox keys or NULL: passed to mmg_logits_sample_args.image_seed */
+  const int32_t* k_dev;                           /* [b] per-image top-k counts on the route of k_keep, or NULL: passed to mmg_logits_sample_args.k_dev */
 } mmg_decode_step_args;
 uint64_t mmg_decode_step_workspace_bytes(int32_t b, int32_t branches, int32_t n, int32_t dim, int32_t heads, int32_t Fp, int32_t V, int32_t max_masked);
 int mmg_decode_step(const mmg_decode_step_args* a, void* stream);

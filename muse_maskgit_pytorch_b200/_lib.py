@@ -120,7 +120,8 @@ class LogitsSampleArgs(C.Structure):
                 ("B", i32), ("n", i32), ("num_masked", i32), ("V", i32), ("k", i32), ("temperature", f32),
                 ("seed", u64), ("step", u64), ("row_offset", i64), ("seed_dev", vp), ("mask_id", i64), ("only_masked", i32), ("rng_mode", i32),
                 ("aten_offset", u64), ("aten_offset_dev", vp), ("aten_stride", C.c_uint32), ("_pad", i32),
-                ("row_index", vp), ("row_count_dev", vp), ("row_index_cap", i32), ("_pad2", i32), ("temperature_dev", vp), ("image_seed", vp)]
+                ("row_index", vp), ("row_count_dev", vp), ("row_index_cap", i32), ("_pad2", i32), ("temperature_dev", vp), ("image_seed", vp),
+                ("k_dev", vp)]
 
 
 class LogitsFusedArgs(C.Structure):
@@ -165,7 +166,7 @@ class DecodeStepArgs(C.Structure):
                 ("ctx_key_mask", vp), ("ctx_keys", i32), ("ctx_alloc", i32), ("ids", vp), ("scores", vp), ("masked_pos", vp), ("mask_id", i64),
                 ("num_masked", i32), ("k_keep", i32), ("step", i32), ("temperature", f32), ("cond_scale", f32), ("_pad", i32),
                 ("u", vp), ("seed", u64), ("seed_dev", vp), ("row_offset", i64), ("workspace", vp), ("workspace_bytes", u64),
-                ("cond_scale_dev", vp), ("temperature_dev", vp), ("image_seed", vp)]
+                ("cond_scale_dev", vp), ("temperature_dev", vp), ("image_seed", vp), ("k_dev", vp)]
 
 
 class LfqEncodeArgs(C.Structure):

@@ -325,12 +325,14 @@ __device__ __forceinline__ uint32_t half_key(uint32_t h) { return (h & 0x8000u) 
 __device__ __forceinline__ uint32_t key_half(uint32_t k) { return (k & 0x8000u) ? (k & 0x7fffu) : (~k & 0xffffu); }      // and back
 
 __global__ void __launch_bounds__(THR_WARPS * 32)
-logits_threshold_exact_kernel(const float* __restrict__ S, int ns, int k, float* __restrict__ thr, int64_t R, int* __restrict__ fb_count) {
+logits_threshold_exact_kernel(const float* __restrict__ S, int ns, int k, const int32_t* __restrict__ k_dev, int num_masked, float* __restrict__ thr,
+                              int64_t R, int* __restrict__ fb_count) {
   pdl_wait(); pdl_trigger();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (blockIdx.x == 0 && threadIdx.x == 0) *fb_count = 0;
   const int64_t r = (int64_t)blockIdx.x * THR_WARPS + warp;
   if (r >= R) return;
+  if (k_dev) k = k_dev[r / num_masked];                     // the row's own image's k
   const float* row = S + r * ns;
   uint32_t sk[THR_KEYS];
 #pragma unroll
@@ -348,12 +350,15 @@ logits_threshold_exact_kernel(const float* __restrict__ S, int ns, int k, float*
 }
 
 __global__ void __launch_bounds__(THR_WARPS * 32)
-logits_threshold_kernel(const float* __restrict__ S, int ns, int V, int k, float* __restrict__ thr, int64_t R, int* __restrict__ fb_count) {
+logits_threshold_kernel(const float* __restrict__ S, int ns, int V, int k, const int32_t* __restrict__ k_dev, int num_masked, float* __restrict__ thr,
+                        int64_t R, int* __restrict__ fb_count) {
   pdl_wait(); pdl_trigger();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (blockIdx.x == 0 && threadIdx.x == 0) *fb_count = 0;   // per-step fallback counter (the previous step's fallback kernels are done: stream order)
   const int64_t r = (int64_t)blockIdx.x * THR_WARPS + warp;
   if (r >= R) return;
+  if (k_dev) k = k_dev[r / num_masked];                     // the row's own image's k: its sample rank rs below
+
   const float* row = S + r * ns;
   // sampled rows: ns == SMP_SAMPLE (lf_supported), 128 samples per lane as 64 half2 (float4 loads: lane owns 4 consecutive samples per 128)
   __half2 x2[THR_KEYS / 2];
@@ -438,10 +443,11 @@ logits_finish_kernel(const mmg_logits_sample_args a, float tdiv, const LfFinish 
 
   pdl_wait(); pdl_trigger();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int V = a.V, k = a.k;
+  const int V = a.V;
   const int64_t r = blockIdx.x;
   const int b = (int)(r / a.num_masked);
   const int pos = a.masked_pos[r];
+  const int k = image_k(a, b);
   const int nseg = LF_SEGS * f.S;
   if (tid == 0) s_bad = 0;
   __syncthreads();
@@ -740,8 +746,8 @@ extern "C" int mmg_logits_fused(const mmg_logits_fused_args* a, void* stream) {
     if ((rc = linear_impl(&l, nullptr, stream))) return rc;
   }
   // 2. per-row candidate threshold
-  if (pl.ns == s.V) MMG_CUDA(launch_pdl(logits_threshold_exact_kernel, dim3((unsigned)((R + THR_WARPS - 1) / THR_WARPS)), dim3(THR_WARPS * 32), 0, st, (const float*)S, pl.ns, s.k, thr, R, fb_count));
-  else MMG_CUDA(launch_pdl(logits_threshold_kernel, dim3((unsigned)((R + THR_WARPS - 1) / THR_WARPS)), dim3(THR_WARPS * 32), 0, st, (const float*)S, pl.ns, s.V, s.k, thr, R, fb_count));
+  if (pl.ns == s.V) MMG_CUDA(launch_pdl(logits_threshold_exact_kernel, dim3((unsigned)((R + THR_WARPS - 1) / THR_WARPS)), dim3(THR_WARPS * 32), 0, st, (const float*)S, pl.ns, s.k, s.k_dev, s.num_masked, thr, R, fb_count));
+  else MMG_CUDA(launch_pdl(logits_threshold_kernel, dim3((unsigned)((R + THR_WARPS - 1) / THR_WARPS)), dim3(THR_WARPS * 32), 0, st, (const float*)S, pl.ns, s.V, s.k, s.k_dev, s.num_masked, thr, R, fb_count));
   MMG_LAUNCHED();
   {   // 3. the logits GEMM with the candidate / softmax epilogue
     LfParams p{};

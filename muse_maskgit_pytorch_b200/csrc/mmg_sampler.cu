@@ -23,13 +23,13 @@ logits_sample_kernel(const mmg_logits_sample_args a, float tdiv) {
   float* lval = reinterpret_cast<float*>(smraw);                 // [SMP_CAP] candidate logits
   int* lidx = reinterpret_cast<int*>(lval + SMP_CAP);            // [SMP_CAP] candidate vocabulary indices
   float4* scr = reinterpret_cast<float4*>(lidx + SMP_CAP);       // [4][SMP_THREADS] per-thread staging of the 16 values in flight
-  __shared__ int s_count, s_n;
+  __shared__ int s_count, s_n, s_k;
   __shared__ SampleScratch sc;
   __shared__ float s_max, s_sum;
 
   pdl_wait(); pdl_trigger();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int V = a.V, k = a.k;
+  const int V = a.V;
   int64_t r = blockIdx.x;
   const float* row = a.logits + r * (int64_t)V;
   if (a.row_index) {                                  // fallback leg of mmg_logits_fused: logits row j belongs to sampled row row_index[j]
@@ -56,8 +56,10 @@ logits_sample_kernel(const mmg_logits_sample_args a, float tdiv) {
       sk[j] = key;
     }
   }
-  if (tid == 0) s_count = 0;
-  const float tlo = sample_threshold(sk, ns, V, k, sc, warp, lane);
+  // the row's own k (per-image table): parked in shared memory across phase B, where a register holding it made MODE 0 spill.  A count
+  // above the list capacity belongs to the row-walking kernel's route (mmg.h); clamped, it cannot make the exact rebuild write past the list.
+  if (tid == 0) { s_count = 0; s_k = min(image_k(a, b), SMP_CAP); }
+  const float tlo = sample_threshold(sk, ns, V, image_k(a, b), sc, warp, lane);
   const bool degenerate = (tlo == -FLT_MAX);                         // no usable threshold: every element is a candidate (-> exact rebuild)
 
   // ---------------- phase B: one streaming pass over the row ----------------
@@ -183,6 +185,7 @@ logits_sample_kernel(const mmg_logits_sample_args a, float tdiv) {
     __syncthreads();
   }
   int n = s_n;
+  const int k = s_k;
 
   // ---------------- rare: exact rebuild when the sample threshold missed ----------------
   if (n < k || n > SMP_CAP) {
@@ -253,12 +256,13 @@ logits_sample_bigk_kernel(const mmg_logits_sample_args a, float tdiv) {
   __shared__ RowNoise<MODE> s_noise;
   pdl_wait(); pdl_trigger();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int V = a.V, k = a.k;
+  const int V = a.V;
   int64_t r = blockIdx.x;
   const float* row = a.logits + r * (int64_t)V;
   if (a.row_index) { if ((int)blockIdx.x >= *a.row_count_dev) return; r = a.row_index[blockIdx.x]; }
   const int b = (int)(r / a.num_masked);
   const int pos = a.masked_pos[r];
+  const int k = image_k(a, b);                       // this row's own k: the call reached this kernel by its largest one
   // the row's noise, set up by one thread and read after the descent loop's barriers.  Held in registers across that loop, the
   // temperature made MODE 2 spill 8 bytes.
   if (tid == 0) s_noise = row_noise<MODE>(a, b, pos, V, tdiv);
@@ -404,6 +408,9 @@ __device__ __forceinline__ void remask_row(int64_t* __restrict__ ids, float* __r
     if (selected < rows) {
       int first = n;
       for (int i = 0; i < n; ++i) if (fz[i]) { first = i; break; }
+      // no frozen position (generate() with per-image step counts: an image that needs fewer rows than the step's largest count): the pad
+      // rows repeat the image's first selected row, whose id and score they recompute bit for bit, so no other position's score changes
+      if (first == n) for (int i = 0; i < n; ++i) if (flag[i]) { first = i; break; }
       for (int r = selected + tid; r < rows; r += 256) masked_pos[(int64_t)b * rows + r] = first < n ? first : 0;
     }
   }
@@ -554,7 +561,7 @@ extern "C" int mmg_logits_sample(const mmg_logits_sample_args* a, void* stream) 
   if (attr != cudaSuccess) return fail(MMG_ECUDA, "cudaFuncSetAttribute(logits_sample): %s", cudaGetErrorString(attr));
   float t = a->temperature; if (t < 1e-10f) t = 1e-10f;      // max(temperature, 1e-10): muse_maskgit_pytorch.py:411
   const int mode = noise_mode(*a);
-  if (a->k > SMP_CAP)                                          // kept set larger than the candidate list: the row-walking kernel
+  if (a->k > SMP_CAP)                                          // kept set larger than the candidate list (of the largest per-image k): the row-walking kernel
     MMG_CUDA(launch_pdl(bigk_kernels[mode], dim3((unsigned)R), dim3(SMP_THREADS), 0, st, *a, t));
   else
     MMG_CUDA(launch_pdl(list_kernels[mode], dim3((unsigned)R), dim3(SMP_THREADS), smem, st, *a, t));

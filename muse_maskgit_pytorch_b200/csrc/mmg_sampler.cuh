@@ -171,6 +171,8 @@ __device__ __forceinline__ float image_tdiv(const mmg_logits_sample_args& a, int
   const float t = a.temperature_dev[b];
   return t < 1e-10f ? 1e-10f : t;
 }
+// the top-k count of image b: the per-image table when given, else the call's k
+__device__ __forceinline__ int image_k(const mmg_logits_sample_args& a, int b) { return a.k_dev ? a.k_dev[b] : a.k; }
 
 // ---------------- the sampling noise ----------------
 // libmmg's noise streams are Philox4x32-10 with counter (c0, c1, row_lo, row_hi) and a 64-bit key (oracle/philox.py restates them).  The

@@ -140,7 +140,7 @@ extern "C" int mmg_decode_step(const mmg_decode_step_args* a, void* stream) {
     if ((rc = linear_bf16(e, a->w_logits, Rm, a->V, a->dim, MMG_EPI_STORE, ep, stream))) return rc; }
   {   // top-k filter + gumbel argmax + confidence (:576-609)
     mmg_logits_sample_args s{}; s.logits = logits; s.masked_pos = a->masked_pos; s.ids = a->ids; s.scores = a->scores; s.u = a->u;
-    s.B = a->b; s.n = a->n; s.num_masked = a->num_masked; s.V = a->V; s.k = a->k_keep; s.temperature = a->temperature; s.temperature_dev = a->temperature_dev; s.image_seed = a->image_seed;
+    s.B = a->b; s.n = a->n; s.num_masked = a->num_masked; s.V = a->V; s.k = a->k_keep; s.temperature = a->temperature; s.temperature_dev = a->temperature_dev; s.image_seed = a->image_seed; s.k_dev = a->k_dev;
     s.seed = a->seed; s.step = (uint64_t)a->step; s.row_offset = a->row_offset; s.seed_dev = a->seed_dev;
     if ((rc = mmg_logits_sample(&s, stream))) return rc;
   }

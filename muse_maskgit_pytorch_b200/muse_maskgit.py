@@ -16,7 +16,7 @@ import os
 import random
 from functools import partial
 from pathlib import Path
-from typing import Callable, List, NamedTuple, Optional
+from typing import Callable, List, NamedTuple, Optional, Union
 
 import torch
 from torch import nn
@@ -558,13 +558,14 @@ class _Window:
 class _Region:
     """The tokens inpaint() regenerates, edit() resamples or extrapolate() generates.  n_max: the most an image regenerates per round (its
     schedule gives the rows sampled per step); iterations: None for inpaint(), else the rounds of edit() (each opened by an mmg_edit_select
-    that writes its frozen map) or of extrapolate() (one per window); tensors: images, counts int32 [timesteps, b], and frozen uint8 [b, n]
+    that writes its frozen map) or of extrapolate() (one per window); tensors: images (absent for generate() with per-image timesteps: every token starts masked), counts int32 [timesteps, b], and frozen uint8 [b, n]
     or keep uint8 [b, n] (1 = not editable) + num_select int32 [b]; window: extrapolate()'s plan, whose rounds load their window from the
     token canvas and store its new strip back (frozen is then the map of every window: 1 outside the strip)."""
     n_max: int
     iterations: Optional[int]
     tensors: dict
     window: Optional[_Window] = None
+    rows: tuple = ()      # rows sampled per image at each step of a round: the step's largest count (at least 1); images below it pad
 
 
 def _per_image(name, value, b):
@@ -586,6 +587,37 @@ def _per_image(name, value, b):
     if not all(math.isfinite(v) for v in vals):
         raise ValueError(f"{name} must be finite, got {vals}")
     return vals
+
+
+def _is_scalar(value):
+    return isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0)
+
+
+def _per_image_steps(value, b):
+    """`timesteps` of generate() / inpaint() / Muse.forward: a number is returned as it is (every image, handled as it always was); a
+    length-b sequence of ints or a 1-D integer tensor gives each image its own count, returned as one int when all are equal, else as a
+    tuple of b ints.  Raises ValueError on a wrong length or a value that is not an int >= 1."""
+    if _is_scalar(value):
+        return value.item() if isinstance(value, torch.Tensor) else value
+    if isinstance(value, torch.Tensor):
+        if value.dim() != 1 or value.dtype.is_floating_point or value.dtype.is_complex or value.dtype == torch.bool:
+            raise ValueError(f"timesteps must be an int or 1-D integer, got a tensor of shape {tuple(value.shape)} and dtype {value.dtype}")
+        value = value.detach().cpu().tolist()
+    try:
+        vals = list(value)
+    except TypeError:
+        raise ValueError(f"timesteps must be an int, a sequence of ints or a 1-D integer tensor, got {value!r}") from None
+    if not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) and v >= 1 for v in vals):
+        raise ValueError(f"timesteps must hold ints >= 1, got {vals!r}")
+    if len(vals) != b:
+        raise ValueError(f"timesteps has {len(vals)} values for {b} texts")
+    vals = tuple(int(v) for v in vals)
+    return vals[0] if len(set(vals)) == 1 else vals
+
+
+def _keep_count(thres, V):
+    """The logits an image keeps per sampled row for top-k threshold `thres` (muse_maskgit_pytorch.py:414)."""
+    return math.ceil((1 - thres) * V)
 
 
 _U64 = 1 << 64
@@ -655,13 +687,14 @@ def _fill_on_device(t, device):
 @dataclasses.dataclass(frozen=True)
 class _DecodeRequest:
     """One validated generate() / inpaint() / edit() / extrapolate() call.  temperature, cond_scale, critic_noise_scale: one float per image.
+    topk_filter_thres: a number or one per image.  timesteps: an int, or (generate / inpaint) a tuple of b ints that are not all equal.
     seed: the libmmg sampling seed (None: sampler_seed or a draw when it runs).  image_seeds: one uint64 seed per image, or None."""
     texts: List[str]
     cond_images: Optional[torch.Tensor]
     fmap_size: int
     temperature: tuple
-    topk_filter_thres: float
-    timesteps: int
+    topk_filter_thres: Union[float, tuple]
+    timesteps: Union[int, tuple]
     cond_scale: tuple
     critic_noise_scale: tuple
     can_remask_prev_masked: bool
@@ -676,19 +709,37 @@ class _DecodeRequest:
         """CFG branches of the call: 1 when every image's cond_scale is 1 (no null forward, as the reference), else 2."""
         return 1 if all(c == 1 for c in self.cond_scale) else 2
 
-    def settings(self, n):
-        """The host fp32 tables the sampling kernels read, each value the float64 expression of a scalar call rounded once: temps and
-        crit_noise [timesteps, b] (step s anneals by steps_until_x0 / timesteps, muse_maskgit_pytorch.py:578, 600), cond_scale [b]; with a
-        critic, its per-row copies over the n positions of each image (crit_cond_scale [b*n], crit_noise [timesteps, b*n]); with per-image
-        seeds, image_seeds int64 [b] (the bits of the uint64 seeds)."""
-        anneal = [until / self.timesteps for until in reversed(range(self.timesteps))]
+    @property
+    def steps(self):
+        """The decode steps of each image (a tuple of b ints)."""
+        return self.timesteps if isinstance(self.timesteps, tuple) else (self.timesteps,) * len(self.texts)
+
+    @property
+    def max_steps(self):
+        """The decode steps the call runs: the largest of the images' counts."""
+        return max(self.timesteps) if isinstance(self.timesteps, tuple) else self.timesteps
+
+    def keep(self, V):
+        """The logits each image keeps per sampled row (a tuple of b ints)."""
+        thres = self.topk_filter_thres if isinstance(self.topk_filter_thres, tuple) else (self.topk_filter_thres,) * len(self.texts)
+        return tuple(_keep_count(t, V) for t in thres)
+
+    def settings(self, n, V=None):
+        """The host tables the sampling kernels read, each fp32 value the float64 expression of a scalar call rounded once: temps and
+        crit_noise [T, b] (T = max_steps; image b at step s < T_b anneals by (T_b - 1 - s) / T_b, muse_maskgit_pytorch.py:578, 600, and
+        holds 0 from its last step on), cond_scale [b]; with a critic, its per-row copies over the n positions of each image (crit_cond_scale
+        [b*n], crit_noise [T, b*n]); with per-image seeds, image_seeds int64 [b] (the bits of the uint64 seeds); given the vocabulary size V,
+        k int32 [b] (the logits each image keeps)."""
+        anneal = [[(T - 1 - s) / T if s < T else 0. for T in self.steps] for s in range(self.max_steps)]
         f32 = lambda v: torch.tensor(v, dtype=torch.float32)
-        out = dict(temps=f32([[t * a for t in self.temperature] for a in anneal]), cond_scale=f32(self.cond_scale))
+        out = dict(temps=f32([[t * a for t, a in zip(self.temperature, row)] for row in anneal]), cond_scale=f32(self.cond_scale))
         if self.use_critic:
             out["crit_cond_scale"] = out["cond_scale"].repeat_interleave(n)
-            out["crit_noise"] = f32([[c * a for c in self.critic_noise_scale] for a in anneal]).repeat_interleave(n, dim=1)
+            out["crit_noise"] = f32([[c * a for c, a in zip(self.critic_noise_scale, row)] for row in anneal]).repeat_interleave(n, dim=1)
         if self.image_seeds is not None:
             out["image_seeds"] = _seed_bits(self.image_seeds)
+        if V is not None:
+            out["k"] = torch.tensor(self.keep(V), dtype=torch.int32)
         return out
 
 
@@ -784,8 +835,16 @@ class MaskGit(nn.Module):
         (DESIGN.md "Per-image seeds" reports the fused tail's split count and the text padding as checked).  No call seed is drawn, so torch's
         host generator is deliberately left untouched; the seeds are device data, and one captured graph replays for any of them.  Raises
         ValueError with sampler_rng = "aten" (one reference stream per batch) or sampler_noise_fn.  inpaint(), edit() and extrapolate()
-        take it alike."""
-        seeds = self._image_seeds_arg(image_seeds, len(texts))
+        take it alike.
+
+        timesteps and topk_filter_thres may be per image too (a length-b sequence or 1-D tensor; timesteps ints >= 1): the call runs
+        max(timesteps) decode steps and image b follows its own schedule mask_schedule(n, timesteps[b]) with its own annealing, then rests;
+        it keeps ceil((1 - topk_filter_thres[b]) * V) logits per sampled row.  With image_seeds, each image equals the scalar call with its
+        own settings (DESIGN.md, "Per-image sampling settings").  Mixed timesteps decode through inpaint()'s loop over an all-masked grid,
+        so use_native_step does not apply to them, and raise ValueError with sampler_rng = "aten" (one reference stream, one schedule)."""
+        b = len(texts)
+        steps, thres = self._steps_arg(timesteps, b), self._thres_arg(topk_filter_thres, b)
+        seeds = self._image_seeds_arg(image_seeds, b)
         if self.use_native_step and self.transformer.precision == "fp8":
             raise ValueError('use_native_step=True runs mmg_decode_step, whose weights carry no fp8 scales: it cannot run precision="fp8"; '
                              "set use_native_step = False")
@@ -794,8 +853,12 @@ class MaskGit(nn.Module):
                              f"{self.transformer.transformer_blocks.dim_head}; set use_native_step = False")
         if negative_texts is not None:
             raise NotImplementedError("negative_texts raises TypeError in the reference (defect B2); not supported")
-        return self._decode(self._request(texts, cond_images=cond_images, fmap_size=fmap_size, temperature=temperature, timesteps=timesteps,
-                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+        region = None
+        if isinstance(steps, tuple):      # per-image step counts: inpaint()'s loop, every token regenerated, none frozen
+            n = (fmap_size if fmap_size is not None else self.vae.get_encoded_fmap_size(self.image_size)) ** 2
+            region = self._region(None, [n] * b, steps, frozen=torch.zeros((b, n), dtype=torch.uint8))
+        return self._decode(self._request(texts, cond_images=cond_images, fmap_size=fmap_size, temperature=temperature, timesteps=steps,
+                                          region=region, topk_filter_thres=thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
                                           force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
                                           image_seeds=seeds))
 
@@ -815,16 +878,18 @@ class MaskGit(nn.Module):
         vae.decode_from_ids(ids): the unmasked region is the VAE reconstruction, not the input pixels; pasting the input back is the
         caller's job.  With every token masked the result equals generate() under the same seed or injected noise.
         Returns what generate() returns.  `use_native_step` does not apply here (mmg_decode_step has no frozen positions).
-        image_seeds: per-image seeds, as for generate()."""
+        image_seeds: per-image seeds, as for generate().  timesteps and topk_filter_thres may be per image, as for generate(): image b then
+        follows max(int(noise_schedule(t) * N_b), 1) over its own timesteps[b] steps."""
         b = len(texts)
+        steps, thres = self._steps_arg(timesteps, b), self._thres_arg(topk_filter_thres, b)
         seeds = self._image_seeds_arg(image_seeds, b)
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
         self._check_images(images, b)
         regen = regen_tokens(mask, b, self.image_size, fmap_size).reshape(b, -1)
         counts = [int(c) for c in regen.sum(dim=1).tolist()]                      # N_b: the call's one device-to-host read for a GPU mask
-        region = self._region(images, counts, timesteps, frozen=(~regen).to(torch.uint8))
-        return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=timesteps, region=region,
-                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+        region = self._region(images, counts, steps, frozen=(~regen).to(torch.uint8))
+        return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=steps, region=region,
+                                          topk_filter_thres=thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
                                           force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
                                           image_seeds=seeds))
 
@@ -851,7 +916,9 @@ class MaskGit(nn.Module):
         decode).  iterations = 1, fraction = 1 is inpaint(mask) (generate() for mask=None) under the same seed; iterations = 0 returns
         ids0 and its decode.  The defaults (8 iterations of 4 steps on 10 % of the tokens) are this project's provisional choice, not
         settings from the paper.  Returns what generate() returns.  `use_native_step` does not apply here, as for inpaint().
-        image_seeds: per-image seeds, as for generate(); image b's keys are then Philox with counter (0xFFFFFFFE, i, p) under image_seeds[b]."""
+        image_seeds: per-image seeds, as for generate(); image b's keys are then Philox with counter (0xFFFFFFFE, i, p) under image_seeds[b].
+        topk_filter_thres may be per image, as for generate(); timesteps is one int for every image (see _round_steps)."""
+        self._round_steps("edit", timesteps)
         if isinstance(iterations, bool) or not isinstance(iterations, int) or iterations < 0:
             raise ValueError(f"iterations must be an int >= 0, got {iterations!r}")
         if not 0 < fraction <= 1:
@@ -861,6 +928,7 @@ class MaskGit(nn.Module):
         if self.sampler_rng == "aten":
             raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
         b = len(texts)
+        thres = self._thres_arg(topk_filter_thres, b)
         seeds = self._image_seeds_arg(image_seeds, b)
         fmap_size = self.vae.get_encoded_fmap_size(self.image_size)
         self._check_images(images, b)
@@ -870,7 +938,7 @@ class MaskGit(nn.Module):
         select = [max(int(fraction * c), 1) if c else 0 for c in counts]          # r_b
         region = self._region(images, select, timesteps, iterations, keep=(~editable).to(torch.uint8), num_select=torch.tensor(select, dtype=torch.int32))
         return self._decode(self._request(texts, cond_images=cond_images, temperature=temperature, timesteps=timesteps, region=region,
-                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+                                          topk_filter_thres=thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
                                           force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
                                           image_seeds=seeds))
 
@@ -899,19 +967,49 @@ class MaskGit(nn.Module):
         Raises ValueError before any launch on a wrong direction, amount, stride, timesteps or image shape, for sampler_rng = "aten" (no
         reference stream), for a MaskGit conditioned on a low-resolution image, and for an fp8 VAE without conv tiles for the canvas.
         `use_native_step` does not apply here, as for inpaint().  image_seeds: per-image seeds, as for generate(); every window of image b
-        draws under image_seeds[b] with the window-local position p as the row counter."""
+        draws under image_seeds[b] with the window-local position p as the row counter.  topk_filter_thres may be per image, as for
+        generate(); timesteps is one int for every image (see _round_steps)."""
+        self._round_steps("extrapolate", timesteps)
         if isinstance(timesteps, bool) or not isinstance(timesteps, int) or timesteps < 1:
             raise ValueError(f"timesteps must be an int >= 1, got {timesteps!r}")
         b = len(texts)
+        thres = self._thres_arg(topk_filter_thres, b)
         seeds = self._image_seeds_arg(image_seeds, b)
         window = self._extrapolate_plan(images, b, direction, amount, stride)
         f = self.vae.get_encoded_fmap_size(self.image_size)
         frozen = (~self._window_strip(direction, f, window.stride)).reshape(1, -1).to(torch.uint8).repeat(b, 1)
         region = self._region(images, [f * window.stride] * b, timesteps, len(window.corners), window, frozen=frozen)
         return self._decode(self._request(texts, temperature=temperature, timesteps=timesteps, region=region, cond_images=None,
-                                          topk_filter_thres=topk_filter_thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
+                                          topk_filter_thres=thres, can_remask_prev_masked=can_remask_prev_masked, cond_scale=cond_scale,
                                           force_not_use_token_critic=force_not_use_token_critic, critic_noise_scale=critic_noise_scale, return_ids=return_ids,
                                           image_seeds=seeds))
+
+    def _steps_arg(self, timesteps, b):
+        """timesteps of generate() / inpaint() for b texts (_per_image_steps); ValueError for per-image counts under sampler_rng = "aten"."""
+        steps = _per_image_steps(timesteps, b)
+        if isinstance(steps, tuple) and self.sampler_rng == "aten":
+            raise ValueError('per-image timesteps have no "aten" noise stream (the reference draws one stream for one schedule): use '
+                             'sampler_rng = "mmg" or one timesteps for every image')
+        return steps
+
+    def _thres_arg(self, topk_filter_thres, b):
+        """topk_filter_thres for b texts: a number as given (checked where it always was), else a tuple of b floats whose kept counts
+        ceil((1 - thres) * V) must lie in [1, V] (ValueError)."""
+        if _is_scalar(topk_filter_thres):
+            return topk_filter_thres.item() if isinstance(topk_filter_thres, torch.Tensor) else topk_filter_thres
+        vals = _per_image("topk_filter_thres", topk_filter_thres, b)
+        V = self.transformer.num_tokens
+        bad = [t for t in vals if not 1 <= _keep_count(t, V) <= V]
+        if bad:
+            raise ValueError(f"topk_filter_thres {bad} keep ceil((1 - thres) * {V}) logits per row, outside [1, {V}]")
+        return vals
+
+    @staticmethod
+    def _round_steps(method, timesteps):
+        """edit() / extrapolate() take one timesteps for every image: ValueError for a sequence or 1-D tensor."""
+        if isinstance(timesteps, (list, tuple)) or (isinstance(timesteps, torch.Tensor) and timesteps.dim() > 0):
+            raise ValueError(f"{method}() takes one int timesteps for every image, got {timesteps!r}: decode step s of round i has the Philox "
+                             "step counter i * timesteps + s, and per-image rounds would need a per-image step counter in every noise kernel")
 
     def _image_seeds_arg(self, image_seeds, b):
         """image_seeds of a call with b texts as a tuple of uint64 ints (None: not given); ValueError where no per-image stream exists."""
@@ -929,11 +1027,18 @@ class MaskGit(nn.Module):
                              f"{tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__}")
 
     def _region(self, images, counts, timesteps, iterations=None, window=None, **tensors):
-        """The _Region of a call whose image b regenerates counts[b] tokens per round, on the schedule of that count (none: 0 throughout)."""
-        table = [self.mask_schedule(c, timesteps) if c else [0] * timesteps for c in counts]
-        tensors.update(images=images.to(torch.float32), counts=torch.tensor(table, dtype=torch.int32).t())        # counts: [timesteps, b]
+        """The _Region of a call whose image b regenerates counts[b] tokens per round, on the schedule of that count over its own steps
+        (timesteps: an int, or one per image) and 0 after them (none: 0 throughout).  images None: nothing to encode (every token masked)."""
+        steps = timesteps if isinstance(timesteps, tuple) else (timesteps,) * len(counts)
+        T = max(timesteps) if isinstance(timesteps, tuple) else timesteps
+        table = [(self.mask_schedule(c, t) if c else [0] * t) + [0] * (T - t) for c, t in zip(counts, steps)]
+        # the rows of a step: its largest count, mask_schedule(max(counts), T) for one timesteps (the schedule grows with the count)
+        rows = tuple(max([1] + [col[s] for col in table]) for s in range(T))
+        tensors.update(counts=torch.tensor(table, dtype=torch.int32).t())        # counts: [T, b]
+        if images is not None:
+            tensors.update(images=images.to(torch.float32))
         device = next(self.parameters()).device
-        return _Region(max(counts, default=0), iterations, {k: v.to(device).contiguous() for k, v in tensors.items()}, window)
+        return _Region(max(counts, default=0), iterations, {k: v.to(device).contiguous() for k, v in tensors.items()}, window, rows)
 
     def _extrapolate_plan(self, images, b, direction, amount, stride):
         """Validates extrapolate()'s arguments for b images (ValueError naming the constraint) and returns its _Window."""
@@ -1065,7 +1170,7 @@ class MaskGit(nn.Module):
             self._seed_dev = torch.zeros((1,), dtype=torch.int64, device=device)
         aten, seed = None, req.seed
         if self.sampler_rng == "aten" and self.sampler_noise_fn is None:
-            aten = self._aten_plan(device, b, req.fmap_size ** 2, tr.num_tokens, req.timesteps, req.use_critic)
+            aten = self._aten_plan(device, b, req.fmap_size ** 2, tr.num_tokens, req.max_steps, req.use_critic)
         elif self.sampler_noise_fn is None and req.image_seeds is None:
             # (injected noise: the host generator is the caller's stream; per-image seeds: the kernels read no call seed — nothing is drawn)
             if seed is None:                     # (a rerun on the materialised path keeps the seed of the attempt it repeats)
@@ -1074,19 +1179,24 @@ class MaskGit(nn.Module):
         region = None if req.region is None else req.region.tensors
         # per-image sampling settings as device data: a captured graph copies them in like the region, so they are not in its key
         upload = _fill_on_device if torch.cuda.is_current_stream_capturing() else (lambda t, dev: t.to(dev))
-        settings = {k: upload(v, device) for k, v in req.settings(req.fmap_size ** 2).items()}
+        settings = {k: upload(v, device) for k, v in req.settings(req.fmap_size ** 2, tr.num_tokens).items()}
         if not self.use_cuda_graph or self.sampler_noise_fn is not None:
             return self._generate_body(req, text_embeds, cond_images, region, settings, aten) + (seed,)
         # ---- whole-call CUDA graph: 18 decode steps + VAE decode replayed as one launch (no per-kernel host work) ----
+        # the top-k counts are device data too: the key keeps only the route the largest one picks (fused tail or materialised logits,
+        # candidate list or row-walking kernel), and the rows sampled per step in place of the step counts
+        k_max = max(req.keep(tr.num_tokens), default=1)
+        route = (ops.logits_fused_workspace_bytes(1, tr.num_tokens, tr.dim, k_max) > 0, k_max > ops.SAMPLE_LIST_CAP)
         key = (b, tuple(text_embeds.shape), text_embeds.dtype, None if cond_images is None else tuple(cond_images.shape), req.fmap_size,
-               float(req.topk_filter_thres), int(req.timesteps), req.branches, int(self.row_offset),
+               route, req.timesteps if req.region is None else req.region.rows, req.branches, int(self.row_offset),
                tr.precision, self.vae.precision, req.use_critic, bool(req.can_remask_prev_masked),
                None if aten is None else aten["key"], bool(self.use_native_step), id(self.noise_schedule), bool(self.use_fused_tail),
                req.image_seeds is not None)
         if req.region is not None and req.region.window is not None:
             key += (req.region.window.key,)
         elif req.region is not None:
-            key += (("inpaint", req.region.n_max) if req.region.iterations is None else ("edit", req.region.iterations, req.region.n_max),)
+            key += ((("inpaint" if "images" in region else "generate"), req.region.n_max) if req.region.iterations is None
+                    else ("edit", req.region.iterations, req.region.n_max),)
         critic_net = self.token_critic if isinstance(self.token_critic, Transformer) and req.use_critic else None
         pack_ids = lambda: (id(tr._pack), id(self.vae._pack), id(self.cond_vae._pack), id(critic_net._pack) if critic_net is not None else 0,
                             id(self.token_critic._head_cache) if isinstance(self.token_critic, SelfCritic) else 0)
@@ -1194,11 +1304,12 @@ class MaskGit(nn.Module):
         return bufs
 
     def _sample_tail(self, x, nb, pos, rows_b, ids, scores, temp, step, u, cond_scale, k_keep, tail, seed_dev=None, only_masked_id=None, aten=None,
-                     temp_dev=None, cond_scale_dev=None, image_seed=None):
+                     temp_dev=None, cond_scale_dev=None, image_seed=None, k_dev=None):
         """The sampling tail of one decode step (muse_maskgit_pytorch.py:576-609) on the rows listed in `pos` (b, rows_b): final LayerNorm +
         CFG combine in embedding space, to_logits, top-k filter, gumbel argmax, confidence score; ids / scores are updated in place.
         x: residual stream [nb*b*n, dim] after the blocks (cond rows first, then the null-CFG rows).  temp_dev / cond_scale_dev: fp32 [b]
-        per-image values the kernels read in place of the scalars `temp` / `cond_scale`; image_seed: int64 [b] per-image Philox keys or None."""
+        per-image values the kernels read in place of the scalars `temp` / `cond_scale`; image_seed: int64 [b] per-image Philox keys or None;
+        k_dev: int32 [b] per-image top-k counts, each at most k_keep."""
         tr = self.transformer
         P = tr._packed()
         b, n = ids.shape
@@ -1207,7 +1318,7 @@ class MaskGit(nn.Module):
         e = tail["e"]
         ops.final_embed(x[:bn], x[bn:2 * bn] if nb == 2 else None, P["gf"], pos, e, b, n, rows_b, cond_scale, cond_scale_dev=cond_scale_dev)
         kw = dict(u=u, seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, only_masked_id=only_masked_id, aten=aten,
-                  temperature_dev=temp_dev, image_seed=image_seed)
+                  temperature_dev=temp_dev, image_seed=image_seed, k_dev=k_dev)
         if "fused_ws" in tail:      # logits never reach HBM: candidate lists out of the GEMM epilogue, sampled by the finishing kernel
             ops.logits_fused(e[:R], P["wlog"], pos, ids, scores, rows_b, k_keep, temp, tail["fused_ws"], tail["status"],
                              rows_capacity=b * tail["rows_max"], **kw)
@@ -1221,7 +1332,7 @@ class MaskGit(nn.Module):
         tensors of req.region and req.settings() (or a captured graph's static copies of them)."""
         tr = self.transformer
         device = text_embeds.device
-        b, n, V, timesteps = len(req.texts), req.fmap_size ** 2, tr.num_tokens, req.timesteps
+        b, n, V, timesteps = len(req.texts), req.fmap_size ** 2, tr.num_tokens, req.max_steps
         cond_ids = self.cond_vae.encode_ids(cond_images) if cond_images is not None else None
         nb = req.branches
         # the kernels read the settings from the device tables; the scalar argument fields carry image 0's values, which are what a call
@@ -1246,11 +1357,15 @@ class MaskGit(nn.Module):
             frozen = torch.empty((b, n), dtype=torch.uint8, device=device)          # written by each round's mmg_edit_select
         else:
             frozen = region["frozen"]
-            ids = self.vae.encode_ids(region["images"]).reshape(b, n).masked_fill(frozen == 0, self.mask_id)
+            if "images" in region:
+                ids = self.vae.encode_ids(region["images"]).reshape(b, n).masked_fill(frozen == 0, self.mask_id)
+            else:                     # generate() with per-image step counts
+                ids = torch.full((b, n), self.mask_id, dtype=torch.long, device=device)
         scores = torch.zeros((b, n), dtype=torch.float32, device=device)
         masked_pos = torch.empty((b, n), dtype=torch.int32, device=device)
-        k_keep = math.ceil((1 - req.topk_filter_thres) * V)                    # muse_maskgit_pytorch.py:414
-        sched = self.mask_schedule(n if req.region is None else req.region.n_max, timesteps)
+        # the kernels read each image's k from settings["k"]; the scalar k_keep is the largest, which routes the call and sizes the tail
+        k_keep = max(req.keep(V), default=1)
+        sched = self.mask_schedule(n, timesteps) if req.region is None else list(req.region.rows)
         score_all = bool(req.can_remask_prev_masked) and not req.use_critic
         bn = b * n
         native = None
@@ -1279,8 +1394,10 @@ class MaskGit(nn.Module):
         iterations = req.region.iterations if req.region is not None and req.region.iterations is not None else 1
         # edit() / extrapolate(): `iterations` rounds of the token loop (edit's iterations, extrapolate's windows), step = the global step
         # index (round * timesteps + s); one round otherwise
-        for step, (num_masked, steps_until_x0) in enumerate(zip(sched * iterations, list(reversed(range(timesteps))) * iterations)):
+        T0 = lead(req.steps)
+        for step, num_masked in enumerate(sched * iterations):
             s = step % timesteps
+            anneal0 = (T0 - 1 - s) / T0 if s < T0 else 0.                   # image 0's steps_until_x0 / timesteps
             if edit and s == 0:
                 ops.edit_select(ids, scores, frozen, region["keep"], region["num_select"], self.mask_id, step // timesteps,
                                 u=self._injected_noise(step, (b, n), device), seed_dev=self._seed_dev, row_offset=self.row_offset * n,
@@ -1291,7 +1408,7 @@ class MaskGit(nn.Module):
                 if step:
                     torch.cuda.nvtx.range_pop()
                 torch.cuda.nvtx.range_push(f"mmg.decode_step[{step}] masked={num_masked}")
-            temp = lead(req.temperature) * (steps_until_x0 / timesteps)        # annealed, muse_maskgit_pytorch.py:578
+            temp = lead(req.temperature) * anneal0                             # annealed, muse_maskgit_pytorch.py:578
             temp_dev = settings["temps"][s]
             u = self._injected_noise(step, (b, n, V), device)
             if native is not None:
@@ -1301,7 +1418,7 @@ class MaskGit(nn.Module):
                 a.temperature = float(temp); a.cond_scale = float(lead(req.cond_scale))
                 a.temperature_dev = temp_dev.data_ptr(); a.cond_scale_dev = settings["cond_scale"].data_ptr()
                 a.u = None if u is None else u.data_ptr(); a.seed = 0; a.seed_dev = self._seed_dev.data_ptr(); a.row_offset = self.row_offset * n
-                a.image_seed = None if seeds is None else seeds.data_ptr()
+                a.image_seed = None if seeds is None else seeds.data_ptr(); a.k_dev = settings["k"].data_ptr()
                 _lib.call("mmg_decode_step", a)
                 continue
             if req.region is None:
@@ -1315,11 +1432,11 @@ class MaskGit(nn.Module):
             pos, rows_b = (all_pos, n) if score_all else (masked_pos, num_masked)
             self._sample_tail(x, nb, pos, rows_b, ids, scores, float(temp), step, u, float(lead(req.cond_scale)), k_keep, tail, seed_dev=seed_dev,
                               only_masked_id=self.mask_id if score_all or req.region is not None else None, aten=aten_draw(step),
-                              temp_dev=temp_dev, cond_scale_dev=settings["cond_scale"], image_seed=seeds)
+                              temp_dev=temp_dev, cond_scale_dev=settings["cond_scale"], image_seed=seeds, k_dev=settings["k"])
             if req.use_critic:
                 xc = cnet._run_blocks(ids, cctx, cnb)
                 ops.critic_score(xc[:bn], xc[bn:2 * bn] if cnb == 2 else None, gcrit, whead, float(bhead), float(lead(req.cond_scale)),
-                                 float(lead(req.critic_noise_scale) * (steps_until_x0 / timesteps)), scores, u=self._injected_noise(step, (b, n), device),
+                                 float(lead(req.critic_noise_scale) * anneal0), scores, u=self._injected_noise(step, (b, n), device),
                                  seed=0, seed_dev=seed_dev, step=step, row_offset=self.row_offset * n, aten=aten_draw(step, critic=True),
                                  cond_scale_dev=settings["crit_cond_scale"], noise_mul_dev=settings["crit_noise"][s], row_key=crit_key)
             if window is not None and s == timesteps - 1:
@@ -1477,10 +1594,15 @@ class Muse(nn.Module):
     @torch.no_grad()
     def forward(self, texts: List[str], cond_scale=3., temperature=1., timesteps=18, superres_timesteps=None,
                 return_lowres=False, return_pil_images=True, image_seeds=None):
-        """cond_scale / temperature: a number or per image (see MaskGit.generate), used by both stages.  image_seeds: per-image seeds in any
+        """cond_scale / temperature: a number or per image (see MaskGit.generate), used by both stages.  timesteps (base stage) and
+        superres_timesteps (super-resolution stage, default: timesteps): an int or one int >= 1 per image, each stage's own.  image_seeds: per-image seeds in any
         form MaskGit.generate takes.  The base stage samples with them as given and the super-resolution stage with splitmix64 of each, so the
         two stages do not draw the same stream at shared positions; either stage alone is reproduced by its generate() with those seeds."""
         seeds = _image_seeds(image_seeds, len(texts))
+        # per-image step counts of both stages are checked before the base stage runs (numbers are checked where they always were)
+        for mg, steps in ((self.base_maskgit, timesteps), (self.superres_maskgit, superres_timesteps)):
+            if steps is not None and not _is_scalar(steps):
+                mg._steps_arg(steps, len(texts))
         lowres = self.base_maskgit.generate(texts=texts, cond_scale=cond_scale, temperature=temperature, timesteps=timesteps, image_seeds=seeds)
         superres = self.superres_maskgit.generate(texts=texts, cond_scale=cond_scale, cond_images=lowres, temperature=temperature,
                                                   timesteps=superres_timesteps if superres_timesteps is not None else timesteps,

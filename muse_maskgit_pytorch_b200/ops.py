@@ -414,12 +414,16 @@ def _set_aten(a, aten):
 
 
 def _set_sampling(a, masked_pos, ids, scores, num_masked, V, k, temperature, u, seed, step, row_offset, seed_dev, only_masked_id, aten,
-                  temperature_dev, image_seed):
+                  temperature_dev, image_seed, k_dev):
     """Fills everything of a LogitsSampleArgs but the logits (the arguments of logits_sample)."""
     a.masked_pos = masked_pos.data_ptr(); a.ids = ids.data_ptr(); a.scores = scores.data_ptr(); a.u = L.ptr(u)
     a.B, a.n = ids.shape; a.num_masked = num_masked; a.V = V; a.k = k; a.temperature = temperature
     a.temperature_dev = _per_row_table(temperature_dev, a.B, "temperature_dev")
     a.image_seed = _seed_table(image_seed, a.B, "image_seed")
+    if k_dev is not None:
+        _chk(k_dev, "k_dev")
+        assert k_dev.dtype == torch.int32 and k_dev.numel() == a.B, f"k_dev: int32 [{a.B}]"
+    a.k_dev = L.ptr(k_dev)
     a.seed = seed; a.step = step; a.row_offset = row_offset; a.seed_dev = L.ptr(seed_dev)
     if only_masked_id is not None:
         a.only_masked = 1; a.mask_id = only_masked_id
@@ -427,15 +431,20 @@ def _set_sampling(a, masked_pos, ids, scores, num_masked, V, k, temperature, u, 
 
 
 def logits_sample(logits, masked_pos, ids, scores, num_masked, k, temperature, u=None, seed=0, step=0, row_offset=0, seed_dev=None,
-                  only_masked_id=None, aten=None, temperature_dev=None, image_seed=None):
+                  only_masked_id=None, aten=None, temperature_dev=None, image_seed=None, k_dev=None):
     """aten = (offset, offset_dev, stride): draw the noise from ATen's CUDA uniform_ stream instead of libmmg's keying.
     temperature_dev: fp32 [B] per-image temperatures, read on the device in place of `temperature`.  image_seed: int64 [B] per-image
-    Philox keys (uint64 bits): image b draws with its own key and its positions as row counters, in place of (seed, global row)."""
+    Philox keys (uint64 bits): image b draws with its own key and its positions as row counters, in place of (seed, global row).
+    k_dev: int32 [B] per-image top-k counts read in place of `k`, each on the route `k` picks (same side of SAMPLE_LIST_CAP; the largest
+    count is the natural `k`)."""
     a = L.LogitsSampleArgs()
     a.logits = _chk(logits).data_ptr()
     _set_sampling(a, masked_pos, ids, scores, num_masked, logits.shape[-1], k, temperature, u, seed, step, row_offset, seed_dev,
-                  only_masked_id, aten, temperature_dev, image_seed)
+                  only_masked_id, aten, temperature_dev, image_seed, k_dev)
     L.call("mmg_logits_sample", a)
+
+
+SAMPLE_LIST_CAP = 9216      # SMP_CAP of mmg_sampler.cuh: mmg_logits_sample takes its row-walking kernel for a larger k
 
 
 def logits_fused_workspace_bytes(rows_capacity, V, K, k):
@@ -444,15 +453,15 @@ def logits_fused_workspace_bytes(rows_capacity, V, K, k):
 
 
 def logits_fused(e, w, masked_pos, ids, scores, num_masked, k, temperature, workspace, status, rows_capacity=0, u=None, seed=0, step=0,
-                 row_offset=0, seed_dev=None, only_masked_id=None, aten=None, temperature_dev=None, image_seed=None):
+                 row_offset=0, seed_dev=None, only_masked_id=None, aten=None, temperature_dev=None, image_seed=None, k_dev=None):
     """to_logits + top-k / gumbel argmax / confidence on the rows listed in masked_pos without a [rows, V] logits buffer.
-    temperature_dev, image_seed: as for logits_sample."""
+    temperature_dev, image_seed, k_dev: as for logits_sample (k, the largest count, decides whether the shape is supported)."""
     a = L.LogitsFusedArgs()
     a.e = _chk(e).data_ptr(); a.w = _chk(w).data_ptr(); a.K = e.shape[1]; a.rows_capacity = rows_capacity
     assert e.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and w.shape[1] == e.shape[1]
     a.workspace = workspace.data_ptr(); a.workspace_bytes = workspace.numel() * workspace.element_size(); a.status = status.data_ptr()
     _set_sampling(a.s, masked_pos, ids, scores, num_masked, w.shape[0], k, temperature, u, seed, step, row_offset, seed_dev,
-                  only_masked_id, aten, temperature_dev, image_seed)
+                  only_masked_id, aten, temperature_dev, image_seed, k_dev)
     L.call("mmg_logits_fused", a)
 
 

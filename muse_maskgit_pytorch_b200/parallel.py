@@ -8,9 +8,9 @@ import numbers
 import torch
 import torch.distributed as dist
 
-from .muse_maskgit import _image_seeds, _muse_result
+from .muse_maskgit import MaskGit, _image_seeds, _is_scalar, _muse_result
 
-PER_IMAGE_SETTINGS = ("temperature", "cond_scale", "critic_noise_scale")
+PER_IMAGE_SETTINGS = ("temperature", "cond_scale", "critic_noise_scale", "topk_filter_thres", "timesteps", "superres_timesteps")
 ROW_INPUTS = ("images", "mask", "cond_images")      # call inputs indexed by global row, sliced like `texts`
 
 
@@ -78,7 +78,18 @@ def _run_shard(method, maskgits, texts, lo, hi, total, empty, *, group=None, see
     maskgit transformer's encode_text.  kwargs named in ROW_INPUTS and per-image settings given per image are indexed by global row and
     sliced here; cond_images_shard replaces the slice of cond_images.  image_seeds (per-image seeds in any form generate() takes, for the
     whole batch) become this rank's rows' seeds; no call seed is then drawn or broadcast, since no kernel reads it.  The attributes are
-    restored on return, also when the call raises."""
+    restored on return, also when the call raises.
+
+    Per-image timesteps and top-k thresholds are checked on the whole batch first, by every maskgit, so every rank raises the same
+    ValueError before any collective: checked on its own slice only, a rank could pass where another raises and wait in the all-gather,
+    or (sampler_rng = "aten", mixed counts that are uniform per slice) run and advance its CUDA generator differently from the others."""
+    for name in ("timesteps", "superres_timesteps"):
+        if kwargs.get(name) is not None and not _is_scalar(kwargs[name]):
+            for m in maskgits:
+                m._steps_arg(kwargs[name], total)
+    if kwargs.get("topk_filter_thres") is not None and not _is_scalar(kwargs["topk_filter_thres"]):
+        for m in maskgits:
+            m._thres_arg(kwargs["topk_filter_thres"], total)
     for name in PER_IMAGE_SETTINGS:       # per-image settings (a sequence or 1-D tensor of `total` values) are sliced like text_embeds
         value = kwargs.get(name)
         if value is None or isinstance(value, numbers.Real) or (isinstance(value, torch.Tensor) and value.dim() == 0):
@@ -174,6 +185,7 @@ def edit_sharded(maskgit, texts, images, mask=None, text_embeds=None, cond_image
     `image_seeds` is sliced by global row, as for generate_sharded."""
     if maskgit.sampler_rng == "aten":          # raised here, before any collective, so that ranks without rows raise it too
         raise ValueError('edit() has no "aten" noise stream (the reference has no editing): use sampler_rng = "mmg" or sampler_noise_fn')
+    MaskGit._round_steps("edit", edit_kwargs.get("timesteps", 4))
     return _sharded_call(maskgit, maskgit.edit, texts, group, seed,
                          dict(edit_kwargs, images=images, mask=mask, text_embeds=text_embeds, text_embeds_shard=text_embeds_shard,
                               cond_images=cond_images, cond_images_shard=cond_images_shard))
@@ -187,6 +199,7 @@ def extrapolate_sharded(maskgit, texts, images, direction="right", amount=256, t
     same ValueError.  The sampler noise is keyed on the global row and the window-local position, so with one seed for every rank ("mmg"
     mode) the token ids do not depend on the number of ranks; sampler_rng = "aten" raises ValueError, as extrapolate() does, and
     `sampler_noise_fn` is not covered.  `image_seeds` is sliced by global row, as for generate_sharded."""
+    MaskGit._round_steps("extrapolate", extrapolate_kwargs.get("timesteps", 18))
     window = maskgit._extrapolate_plan(images, len(texts), direction, amount, extrapolate_kwargs.get("stride"))
     p = maskgit.vae.dim_divisor
     return _sharded_call(maskgit, maskgit.extrapolate, texts, group, seed,
@@ -202,7 +215,7 @@ def muse_sharded(muse, texts, text_embeds=None, group=None, *, text_embeds_shard
 
     Seeds: each stage's own `sampler_seed`, else a draw from torch's generator, base first, as one process draws them; rank 0's pair
     reaches every rank in one broadcast.  text_embeds / text_embeds_shard are handed to both stages' transformers.  Per-image
-    cond_scale / temperature are sliced by global row.  Token ids do not depend on the number of ranks, as for generate_sharded.
+    cond_scale / temperature / timesteps / superres_timesteps are sliced by global row.  Token ids do not depend on the number of ranks, as for generate_sharded.
     `image_seeds` is sliced by global row; Muse.forward derives the super-resolution seeds from each rank's slice."""
     return_lowres = forward_kwargs.pop("return_lowres", False)
     return_pil_images = forward_kwargs.pop("return_pil_images", True)
