@@ -158,6 +158,8 @@ template <> struct Vec64<bf16> {
 
 __device__ __forceinline__ float rcp_fast(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float ex2_fast(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+// GLU output a * sigmoid(g) of the bf16 tensor-core epilogues (the register GLU and the GLU tile epilogue: the same instructions in both)
+__device__ __forceinline__ float glu_fast(float a, float g) { return a * rcp_fast(1.0f + ex2_fast(-g * 1.4426950408889634f)); }
 // exact-erf GELU for the bf16 tensor-core epilogues in 11 FP32 ops + one MUFU:  gelu(x) = max(x, 0) - 0.5 |x| erfc(|x| / sqrt 2), with
 // log2 erfc(a / sqrt 2) as a degree-6 polynomial on [0, 6] (weighted minimax fit, scripts/fit_gelu.py); beyond 6 the correction term is
 // below 1e-8 |x|.  Max abs error 6e-7 over all x (fp32 rounding included), relative error < 1e-4 in the negative tail — the output is

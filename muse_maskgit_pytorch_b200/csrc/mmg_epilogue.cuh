@@ -208,7 +208,7 @@ struct Epilogue {
           for (int i = 0; i < 32; ++i) {
             float a = v[i] + (p.bias ? __ldg(p.bias + col0 + i) : 0.f);
             float g = v[32 + i] + (p.bias ? __ldg(p.bias + col0 + 32 + i) : 0.f);
-            o[i] = FAST ? a * rcp_fast(1.0f + ex2_fast(-g * 1.4426950408889634f)) : a * (1.0f / (1.0f + expf(-g)));
+            o[i] = FAST ? glu_fast(a, g) : a * (1.0f / (1.0f + expf(-g)));
           }
         }
         const int oc = col0 >> 1;

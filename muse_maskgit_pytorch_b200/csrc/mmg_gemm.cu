@@ -26,7 +26,7 @@ static int launch_tc(const TcGemmParams& p, cudaStream_t st) {
   return MMG_OK;
 }
 
-// every instantiation of tc_gemm_kernel: 15 with bf16 operands, 8 with e4m3 ones
+// every instantiation of tc_gemm_kernel: 17 with bf16 operands, 8 with e4m3 ones
 static constexpr int tc_key(bool fp8, int bn, int mode) { return (fp8 ? 1 << 16 : 0) | bn << 4 | mode; }
 
 static int launch_instantiation(bool fp8, int bn, int mode, const TcGemmParams& p, cudaStream_t st) {
@@ -47,6 +47,8 @@ static int launch_instantiation(bool fp8, int bn, int mode, const TcGemmParams& 
     case tc_key(false, 128, TC_EPI_QKV128): return launch_tc<128, TC_EPI_QKV128>(p, st);
     case tc_key(false, 256, TC_EPI_QKV128): return launch_tc<256, TC_EPI_QKV128>(p, st);
     case tc_key(false, 128, TC_EPI_QKV128_REGS): return launch_tc<128, TC_EPI_QKV128_REGS>(p, st);
+    case tc_key(false, 256, TC_EPI_GLU): return launch_tc<256, TC_EPI_GLU>(p, st);
+    case tc_key(false, 256, TC_EPI_CONVT): return launch_tc<256, TC_EPI_CONVT>(p, st);
     case tc_key(true, 64, TC_EPI_REGS): return launch_tc<64, TC_EPI_REGS, fp8e4>(p, st);
     case tc_key(true, 128, TC_EPI_REGS): return launch_tc<128, TC_EPI_REGS, fp8e4>(p, st);
     case tc_key(true, 256, TC_EPI_REGS): return launch_tc<256, TC_EPI_REGS, fp8e4>(p, st);  // CONVT_RGB only
@@ -81,6 +83,12 @@ static int plan_tc(const TcGemmParams& p, bool fp8, int* bn_out, int* mode_out) 
                          p.M % 128 == 0 && e.nk_heads == e.nv_heads && (!e.nq_heads || aligned16(e.q_out)) &&
                          (!e.nk_heads || (aligned16(e.k_out) && aligned16(e.v_out)));
   const bool geglu_tiles = kind == MMG_EPI_GEGLU && e.out_dtype == MMG_BF16 && p.mode == 0 && (e.ldo % 8) == 0 && aligned16(e.out);
+  // GLU / CONVT tile epilogues (the VAE decoder's long-K products): bf16 operands and output, conv mode, whole 256-column tiles.  CONVT
+  // also needs the launch's geometry in its epilogue (H, W) to be the grid's, W % 16 == 0 (a warp's 16 rows in one input row) and its
+  // output rows (b H + y) 2 W + x inside int32
+  const bool conv_tiles = !fp8 && p.mode == 1 && e.out_dtype == MMG_BF16 && (e.ldo % 8) == 0 && aligned16(e.out) && p.N % 256 == 0;
+  const bool glu_tiles = conv_tiles && kind == MMG_EPI_GLU;
+  const bool convt_tiles = conv_tiles && kind == MMG_EPI_CONVT && e.H == p.Ho && e.W == p.Wo && p.Wo % 16 == 0 && 2 * p.M < INT32_MAX;
   // A dense e4m3 product has no register-epilogue instantiation: its argument checks leave it only the shapes its tile epilogue takes, and
   // it runs that epilogue at every M: QKV at 128 where pick_bn gives 64 (where the bf16 product takes <64, REGS>), GEGLU at 256 whatever
   // pick_bn gives.  QKV128 (whole 128-column heads) runs its tile epilogue at 128 or 256 for either operand type.
@@ -97,9 +105,12 @@ static int plan_tc(const TcGemmParams& p, bool fp8, int* bn_out, int* mode_out) 
     mode = TC_EPI_QKV128_REGS; bn = 128;      // 64 accumulators per thread, stored from the fragments
   } else if (geglu_tiles && (bn == 256 || tile_at_any_bn)) {
     mode = TC_EPI_GEGLU; bn = 256;
+  } else if ((glu_tiles || convt_tiles) && bn == 256) {
+    mode = glu_tiles ? TC_EPI_GLU : TC_EPI_CONVT;
   } else {
     // 128 accumulator registers per thread at BN = 256 next to a 64-column row chunk would spill, so <256, TC_EPI_REGS> compiles only
-    // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128
+    // the fused RGB epilogue, which reduces the fragments in place; every other register-epilogue kind runs at BN <= 128 (GLU and
+    // CONVT where pick_bn gives 256 and the conditions above hold take their tile epilogues instead)
     mode = TC_EPI_REGS;
     if (bn == 256 && kind != MMG_EPI_CONVT_RGB) bn = 128;
   }
@@ -109,10 +120,19 @@ static int plan_tc(const TcGemmParams& p, bool fp8, int* bn_out, int* mode_out) 
   return MMG_OK;
 }
 
-// the output tensor maps of the tile epilogues: q / k / v heads (QKV, QKV128), bf16 [M, N / 2] (GEGLU), fp32 [M, N] (REDUCE, TSTORE)
+// the output tensor maps of the tile epilogues: q / k / v heads (QKV, QKV128), bf16 [M, N / 2] (GEGLU, GLU), fp32 [M, N] (REDUCE,
+// TSTORE), bf16 pixels of one conv-transpose parity (CONVT)
 static int tile_out_maps(TcGemmParams& p, int mode) {
   const mmg_epilogue_args& e = p.epi.p;
   int rc = MMG_OK;
+  if (mode == TC_EPI_CONVT) {
+    // out is [B, 2H, 2W, ldo]: pixel (b, 2 y + py, 2 x + px) sits (b H + y) 4 W ldo + 2 x ldo elements past pixel (0, py, px), so from
+    // there the parity's pixels are rows (b H + y) 2 W + x of 2 ldo elements; the last one is row (B H - 1) 2 W + W - 1
+    const uint64_t W = (uint64_t)p.Wo, BH = (uint64_t)(p.M / p.Wo);
+    const bf16* base = reinterpret_cast<const bf16*>(e.out) + (uint64_t)(e.py * 2 * W + e.px) * e.ldo;
+    uint64_t od[2] = {(uint64_t)p.N, BH * 2 * W - W}; uint64_t os[1] = {(uint64_t)e.ldo * 4}; uint32_t ob[2] = {64, 16};
+    return make_tmap_bf16(&p.tma_out, base, 2, od, os, ob);
+  }
   if (mode == TC_EPI_QKV || mode == TC_EPI_QKV128) {
     const uint64_t seqs = (uint64_t)(p.M / e.tokens) * (uint64_t)e.heads, hd = mode == TC_EPI_QKV ? 64 : 128;
     uint64_t str[1] = {hd * 2}; uint32_t box[2] = {64, 16};
@@ -122,7 +142,7 @@ static int tile_out_maps(TcGemmParams& p, int mode) {
       rc = make_tmap_bf16(&p.tma_qkv[1], e.k_out, 2, d, str, box); if (rc) return rc;
       rc = make_tmap_bf16(&p.tma_qkv[2], e.v_out, 2, d, str, box); if (rc) return rc;
     }
-  } else if (mode == TC_EPI_GEGLU) {
+  } else if (mode == TC_EPI_GEGLU || mode == TC_EPI_GLU) {
     uint64_t od[2] = {(uint64_t)(p.N / 2), (uint64_t)p.M}; uint64_t os[1] = {(uint64_t)e.ldo * 2}; uint32_t ob[2] = {64, 16};
     rc = make_tmap_bf16(&p.tma_out, e.out, 2, od, os, ob);
   } else if (mode == TC_EPI_REDUCE || mode == TC_EPI_TSTORE) {

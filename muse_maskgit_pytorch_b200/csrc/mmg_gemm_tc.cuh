@@ -38,6 +38,8 @@ enum TcEpiMode : int {
   TC_EPI_QKV128 = 7,    // QKV with 128-column heads (bf16, TC_EPI_QKV's conditions): per-warp tiles + TMA stores, two boxes per head
   TC_EPI_QKV128_REGS = 8,   // QKV with 128-column heads, any other call (fp32 out, tokens % 32 != 0, M % 128 != 0), BN = 128: stores
                             // straight from the fragments
+  TC_EPI_GLU = 9,       // conv GLU (bias, x * sigmoid(gate)), bf16 out, BN = 256: per-warp tiles + TMA store
+  TC_EPI_CONVT = 10,    // conv-transpose parity launch (bias + LeakyReLU), bf16 out, BN = 256: per-warp tiles + TMA store
 };
 // the modes whose epilogue writes whole output boxes with TMA; the others run an Epilogue kind on one row chunk per lane, or (QKV128_REGS)
 // store from the fragments
@@ -46,7 +48,8 @@ constexpr bool tc_tile_epilogue(int mode) { return mode != TC_EPI_REGS && mode !
 struct alignas(64) TcGemmParams {
   CUtensorMap tma_a[4];
   CUtensorMap tma_b;
-  CUtensorMap tma_out;      // REDUCE / TSTORE: the fp32 output [M, N] in boxes of 16 rows x 32 columns (128 B), SWIZZLE_128B; GEGLU: bf16 [M, N/2], 16 x 64
+  CUtensorMap tma_out;      // REDUCE / TSTORE: the fp32 output [M, N] in boxes of 16 rows x 32 columns (128 B), SWIZZLE_128B; GEGLU, GLU: bf16
+                            // [M, N/2], 16 x 64; CONVT: bf16 rows of 2 ldo elements from pixel (0, py, px) (tile_out_maps), 16 x 64
   CUtensorMap tma_qkv[3];   // QKV: q / k / v as [rows, 64] bf16 matrices in boxes of 16 rows x 64 columns (128 B); QKV128: [rows, 128], same boxes
   int64_t M, N;
   int num_kb, num_m_tiles, num_n_tiles;
@@ -94,6 +97,10 @@ template <int BN> struct TcCfg {
 // TC_EPI_QKV: the QKV epilogue (bf16; tokens % 32 == 0 and M % 128 == 0, so a warp's 16 rows are 16 consecutive tokens of one
 // sequence and land on 16 consecutive rows of one head of q / k / v): one box and one TMA store per warp and head chunk.
 // TC_EPI_GEGLU: the GEGLU epilogue (bf16 out, BN == 256): two 64-column chunks make 64 outputs = one box per warp.
+// TC_EPI_GLU: the GLU epilogue of a convolution (bf16 out, BN == 256): GEGLU's boxes with a bias and glu_fast in place of the GELU.
+// TC_EPI_CONVT: a conv-transpose parity launch (bf16 out, BN == 256, W % 16 == 0): one box per warp and 64-column chunk, its 16 rows
+// the pixels 2 x + px of 16 consecutive x.  Both run in conv mode, where a tile's 128 rows are 128 consecutive GEMM rows from
+// conv_tile_row0 (tile_geometry gives TW == Wo or TH == 1); rows of images past B lie past M and are clipped by the tensor map.
 // e4m3 operands (TA = __nv_fp8_e4m3; the dense QKV and GEGLU tile epilogues, and the register epilogues of the convolutions): a k-block
 // is 128 elements, four m64nBNk32 wgmma, and the epilogue starts by dequantising the fragment with dequant_acc (per-row A scales) or
 // dequant_acc_images (per-image A scales, conv mode); everything after it is the bf16 code.
@@ -127,6 +134,13 @@ __device__ __forceinline__ void dequant_acc_images(float (&acc)[BN / 2], const T
     acc[4 * j] *= sa0 * ws.x; acc[4 * j + 1] *= sa0 * ws.y;
     acc[4 * j + 2] *= sa1 * ws.x; acc[4 * j + 3] *= sa1 * ws.y;
   }
+}
+
+// conv mode: the GEMM row (output pixel (b, y, x) as (b Ho + y) Wo + x) of row 0 of tile m_blk; tile row r is this + r when TW == Wo
+// or TH == 1
+__device__ __forceinline__ int64_t conv_tile_row0(const TcGemmParams& p, int m_blk) {
+  const int xt = m_blk % p.tiles_x, yt = (m_blk / p.tiles_x) % p.tiles_y, bt = m_blk / (p.tiles_x * p.tiles_y);
+  return ((int64_t)bt * p.TB * p.Ho + yt * p.TH) * p.Wo + xt * p.TW;
 }
 
 // QKV128: F.normalize * scale of the 128-column head at fragment groups j0 .. j0 + 15 (columns 8 jj + 2 q + e of rows fr and fr + 8), in
@@ -188,6 +202,8 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
   constexpr bool RED = EPI_MODE == TC_EPI_REDUCE || EPI_MODE == TC_EPI_TSTORE, RED_ADD = EPI_MODE == TC_EPI_REDUCE;   // TSTORE: same tiles, plain TMA store
   constexpr bool QKVT = EPI_MODE == TC_EPI_QKV;
   constexpr bool GEGLUT = EPI_MODE == TC_EPI_GEGLU;
+  constexpr bool GLUT = EPI_MODE == TC_EPI_GLU, CONVTT = EPI_MODE == TC_EPI_CONVT;
+  static_assert(!(GLUT || CONVTT) || (BN == 256 && !FP8), "the GLU / CONVT tile epilogues: bf16 operands, 256-column tiles");
   constexpr bool ACTT = EPI_MODE == TC_EPI_ACT;
   static_assert((EPI_MODE != TC_EPI_QKV128 || BN >= 128) && (EPI_MODE != TC_EPI_QKV128_REGS || BN == 128), "QKV128: whole heads per tile");
   constexpr bool TILES = tc_tile_epilogue(EPI_MODE);
@@ -362,8 +378,10 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
               bulk_commit();
             }
           }
-        } else if constexpr (GEGLUT) {
+        } else if constexpr (GEGLUT || GLUT) {
           // rows past M are zero accumulators and are clipped by the tensor map
+          int64_t orow = brow;                                // the output row of the warp's first fragment row
+          if constexpr (GLUT) orow = conv_tile_row0(p, m_blk) + wg * 64 + 16 * wq;
 #pragma unroll
           for (int bx = 0; bx < 2; ++bx) {                    // one box = chunks 2 bx, 2 bx + 1 = 64 bf16 outputs
             const int col0 = n_blk * BN + 128 * bx;
@@ -374,15 +392,26 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
               for (int jj = 0; jj < 4; ++jj) {                // output columns 32 cc + 8 jj + 2 q + e = x column 8 jx + ..., gate column 8 jg + ...
                 const int jx = 8 * (2 * bx + cc) + jj, jg = jx + 4;
                 const uint32_t off = (uint32_t)(((4 * cc + jj) ^ fr) * 16 + 4 * q);
-                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowa + off),
-                             "r"(pack_bf16(acc[4 * jg] * gelu_fast(acc[4 * jx]), acc[4 * jg + 1] * gelu_fast(acc[4 * jx + 1]))) : "memory");
-                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowb + off),
-                             "r"(pack_bf16(acc[4 * jg + 2] * gelu_fast(acc[4 * jx + 2]), acc[4 * jg + 3] * gelu_fast(acc[4 * jx + 3]))) : "memory");
+                uint32_t va, vb;                              // rows fr, fr + 8
+                if constexpr (GLUT) {
+                  // the register GLU's terms: x + bias (0.f without one), gate + bias, glu_fast
+                  const int c = col0 + 64 * cc + 8 * jj + 2 * q;
+                  const float* bias = epi.p.bias;
+                  const float bx0 = bias ? __ldg(bias + c) : 0.f, bx1 = bias ? __ldg(bias + c + 1) : 0.f;
+                  const float bg0 = bias ? __ldg(bias + c + 32) : 0.f, bg1 = bias ? __ldg(bias + c + 33) : 0.f;
+                  va = pack_bf16(glu_fast(acc[4 * jx] + bx0, acc[4 * jg] + bg0), glu_fast(acc[4 * jx + 1] + bx1, acc[4 * jg + 1] + bg1));
+                  vb = pack_bf16(glu_fast(acc[4 * jx + 2] + bx0, acc[4 * jg + 2] + bg0), glu_fast(acc[4 * jx + 3] + bx1, acc[4 * jg + 3] + bg1));
+                } else {
+                  va = pack_bf16(acc[4 * jg] * gelu_fast(acc[4 * jx]), acc[4 * jg + 1] * gelu_fast(acc[4 * jx + 1]));
+                  vb = pack_bf16(acc[4 * jg + 2] * gelu_fast(acc[4 * jx + 2]), acc[4 * jg + 3] * gelu_fast(acc[4 * jx + 3]));
+                }
+                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowa + off), "r"(va) : "memory");
+                asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowb + off), "r"(vb) : "memory");
               }
             }
             box_ready();
-            if (lane == 0) { tma_store_2d(&p.tma_out, box, col0 >> 1, (int)brow); bulk_commit(); }
-            if (epi.p.row_stats) {
+            if (lane == 0) { tma_store_2d(&p.tma_out, box, col0 >> 1, (int)orow); bulk_commit(); }
+            if (GEGLUT && epi.p.row_stats) {
               // each chunk's (sum, sumsq) of its bf16 outputs in ascending column order (geglu_chunk's), read back from the box:
               // lane l sums row l % 16 of chunk 2 bx + l / 16
               const int rr = lane & 15, cc = lane >> 4, cs = col0 + 64 * cc;
@@ -486,6 +515,29 @@ tc_gemm_kernel(const __grid_constant__ TcGemmParams p) {
               if (lane == 0) { tma_store_2d(&p.tma_qkv[which], box, 64 * hh, (int)drow); bulk_commit(); }
             }
             if (lane == 0 && which != 0 && t0 == 0) qkv128_null_row(epi.p, which, bq, h);
+          }
+        } else if constexpr (CONVTT) {
+          // GEMM row m = (b H + y) W + x of parity launch (py, px) is output pixel (b, 2 y + py, 2 x + px), row (b H + y) 2 W + x of
+          // tma_out; W % 16 == 0, so the warp's 16 rows are x0 .. x0 + 15 of one input row
+          const int64_t m0 = conv_tile_row0(p, m_blk) + wg * 64 + 16 * wq, yy = m0 / p.Wo;
+          const int drow = (int)(yy * 2 * p.Wo + (m0 - yy * p.Wo));
+          const float* bias = epi.p.bias;
+#pragma unroll
+          for (int c = 0; c < BN / 64; ++c) {                 // one box = one 64-column chunk
+            const int col0 = n_blk * BN + 64 * c;
+            const uint32_t box = box_begin();
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * c + jj, col = col0 + 8 * jj + 2 * q;
+              const float b0 = bias ? __ldg(bias + col) : 0.f, b1 = bias ? __ldg(bias + col + 1) : 0.f;
+              const uint32_t off = (uint32_t)((jj ^ fr) * 16 + 4 * q);
+              asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowa + off),
+                           "r"(pack_bf16(leaky01(acc[4 * j] + b0), leaky01(acc[4 * j + 1] + b1))) : "memory");
+              asm volatile("st.shared.b32 [%0], %1;" :: "r"(box + rowb + off),
+                           "r"(pack_bf16(leaky01(acc[4 * j + 2] + b0), leaky01(acc[4 * j + 3] + b1))) : "memory");
+            }
+            box_ready();
+            if (lane == 0) { tma_store_2d(&p.tma_out, box, col0, drow); bulk_commit(); }
           }
         }
       } else if constexpr (EPI_MODE == TC_EPI_QKV128_REGS) {

@@ -32,6 +32,7 @@ runall edit 900 tests/test_gpu_edit.py
 runall maskgit_loss 900 tests/test_gpu_maskgit_loss.py
 runall fp8 1200 tests/test_gpu_fp8.py
 runall vae_fp8 1200 tests/test_gpu_vae_fp8.py
+runall vae_tile_epilogues 900 tests/test_gpu_vae_tile_epilogues.py
 runall launch_trace 600 tests/test_gpu_launch_trace.py
 runall batch_settings 900 tests/test_gpu_batch_settings.py
 runall dim_head128 1200 tests/test_gpu_dim_head128.py
